@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- plan-loop Hz / rollout-steps per second of the MPPI rollout hot path on B200.
+"""bench.py -- plan-loop Hz / rollout-steps per second of the MPPI rollout hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config c2|c3|c4|c5] [--scaling strong|weak]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is ONE MPPI plan of a BASELINE configuration: shift U -> K1 sample/clamp -> K2 articulated rollout -> Objective cost ->
@@ -19,6 +20,9 @@ Printed JSON (rank 0, one line):
   roofline      K3 (fused cost-softmax-weighted-sum) achieved HBM GB/s vs the measured peak (MEASURED_PEAKS.json)
   cpu_baseline  the CPU restatement of the reference pipeline (oracle/) on this box's host cores (N = 1 only), with its parallel efficiency
   correctness   N > 1: max |action| difference across ranks and between the peer-memory exchange and the NCCL all-gather
+--dump-outputs DIR writes what the last timed plan returned (DIR/action.npy, float32) and the control sequence it left for the
+next plan (DIR/U.npy, float32), so that two builds can be compared output for output: with the same arguments the inputs
+(seeded initial world, seeded sampling) are identical from run to run.
 --impl reference times that CPU restatement as the reference arm (the reference's own engines, IsaacGym/PhysX and mppi_torch, are
 closed / un-vendored and cannot run here: BASELINE.md section 2).
 """
@@ -141,15 +145,14 @@ def world_bytes(planner, q, qd, goal):
 
 
 class Clocks:
-    """SM clock and throttle reasons DURING the timed region, sampled IN PROCESS through NVML (what nvidia-smi reads) by a background
-    thread on rank 0 only (every 2 ms; the NVML call releases the GIL).  Not from the timing loop itself: with the exchange fused into
-    the kernels every rank waits for the slowest one, and 8 ranks calling into the driver's NVML lock between plans produced
-    millisecond stragglers (profiles/r2_multigpu.md).  No nvidia-smi subprocess either (round-1 review)."""
+    """SM clock and throttle reasons of the timed region, read IN PROCESS through NVML (what nvidia-smi reads) on rank 0 only: once
+    right before and once right after the timed plans, never while they run.  An NVML query while plans run stalls them: on an H100,
+    a sampler thread querying every 2 ms during the timed plans put single plans at up to 1.35 ms instead of 0.255 ms and moved the
+    mean of 50 plans by up to 30 %.  No nvidia-smi subprocess either."""
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap", 0x80: "hw_power_brake"}
 
-    def __init__(self, cuda_index, enabled=True, period_s=0.002):
-        self.ok, self.sm, self.mask, self.h, self.period = False, [], 0, None, period_s
-        self._stop, self._thread = threading.Event(), None
+    def __init__(self, cuda_index, enabled=True):
+        self.ok, self.sm, self.mask, self.h = False, [], 0, None
         if not enabled:
             self.err = "not sampled on this rank"
             return
@@ -182,23 +185,12 @@ class Clocks:
             pass
 
     def start(self):
-        if not self.ok:
-            return
-
-        def loop():
-            while not self._stop.is_set():
-                try:
-                    self.sample()
-                except Exception:  # noqa: BLE001
-                    return
-                self._stop.wait(self.period)
-        self._thread = threading.Thread(target=loop, daemon=True)
-        self._thread.start()
+        if self.ok:
+            self.sample()
 
     def stop(self):
-        self._stop.set()
-        if self._thread is not None:
-            self._thread.join(timeout=2)
+        if self.ok:
+            self.sample()
 
     def summary(self):
         if not self.ok:
@@ -206,7 +198,7 @@ class Clocks:
         busy = sorted(self.sm)
         return {"sm_mhz": busy[len(busy) // 2] if busy else None, "sm_max_mhz": self.max_mhz,
                 "reasons": sorted(n for bit, n in self.REASONS.items() if self.mask & bit), "samples": len(self.sm),
-                "how": f"NVML in process, background thread on rank 0, one sample per {int(self.period * 1e3)} ms while the timed plans run"}
+                "how": "NVML in process on rank 0, read right before and right after the timed plans (a query while they run stalls them)"}
 
 
 def measured_peak_gbs():
@@ -214,7 +206,7 @@ def measured_peak_gbs():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s; not a measured figure)"
 
 
 # --------------------------------------------------------------------------------------------------
@@ -380,7 +372,7 @@ def k3_roofline(planner, peak_gbs, K_list):
         be = CudaBackend(dev)
         be.create(planner.sim.scene.model, p)
         bytes_alg = 4 * K * T * (nu + 1) + 4 * (T * nu + 2)
-        nbuf = min(64, max(2, int(np.ceil(300e6 / bytes_alg))))            # > 2x the 126 MB L2
+        nbuf = min(64, max(2, int(np.ceil(300e6 / bytes_alg))))            # > 2x the 50 MB L2
         xs = [torch.randn((T, nu, K), device=dev) * 0.3 for _ in range(nbuf)]
         cs = [torch.rand((T, K), device=dev) * 10 for _ in range(nbuf)]
         U = torch.zeros((T, nu), device=dev)
@@ -423,6 +415,14 @@ def timed_plans(planner, steps, warmup, flush, barrier, clocks=None):
     return [s.elapsed_time(e) for s, e in zip(starts, ends)]
 
 
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy in float32 for every tensor of `arrays` (copied to the host after the device has finished)."""
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def run_gpu_arm(args, rank, world, local_rank):
     import torch.distributed as dist
     import __graft_entry__
@@ -453,11 +453,13 @@ def run_gpu_arm(args, rank, world, local_rank):
     planner = MPPIisaacPlanner(load_cfg(name, k_total, dev), make_objective(name), use_cuda_graph=True)
     init_world(planner, name)
     nu = planner.mppi.nu
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2
     clocks = Clocks(local_rank, enabled=(rank == 0 and os.environ.get("BENCH_NO_CLOCKS", "0") in ("", "0")))
 
     # ---- device-resident timing ------------------------------------------------------------------------------------
     per_step_ms = timed_plans(planner, args.steps, args.warmup, flush, barrier, clocks)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"action": planner.mppi._action, "U": planner.mppi.U})
     graph_on = planner.mppi._graph is not None
     total_s = reduce_max(sum(per_step_ms)) * 1e-3
     value = k_total * T * args.steps / total_s
@@ -603,12 +605,10 @@ def run_gpu_arm(args, rank, world, local_rank):
             ks = sorted({planner.sim.num_envs, 65536, 262144})
             roof = k3_roofline(planner, peak, ks)
             head = next(r for r in roof if r["K"] == planner.sim.num_envs)
-            traffic = {(10000, 30, 7): 9666560}.get((head["K"], T, nu))
             line["roofline"] = {"kernel": "K3 reduce_kernel (fused cost accumulate + softmax + weighted control sum)", "bound": "hbm",
-                                "achieved": head["GBps"], "peak": peak, "unit": "GB/s", "frac": head["frac"], "traffic": traffic,
-                                "traffic_source": "ncu --set full dram__bytes_read.sum + write of one K3 launch at this K (profiles/r2_ncu_summaries.txt): 1.007 x algorithmic; 1.0003 x at K = 262 144" if traffic else None,
+                                "achieved": head["GBps"], "peak": peak, "unit": "GB/s", "frac": head["frac"],
                                 "peak_source": peak_src, "bytes_per_launch": head["bytes"], "us_per_launch": head["us"], "K": head["K"],
-                                "note": "the named K is launch/latency bound (9.6 MB = 1.5 us of HBM time at C2*); the sweep shows the asymptote",
+                                "note": "the named K is launch/latency bound (9.6 MB = 2.9 us of HBM time at 3.35 TB/s at C2*); the sweep shows the asymptote",
                                 "sweep": roof}
             line["kernels_us"] = kt
             line["cpu_baseline"], _, _ = cpu_baseline(name)
@@ -644,6 +644,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed plan's action and control sequence as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,5 +1,5 @@
 /*
- * mppib.h -- C ABI of the B200-native MPPI rollout path ("mppib" = MPPI on Blackwell).
+ * mppib.h -- C ABI of the H100-native MPPI rollout path ("mppib").
  *
  * This is the drop-in boundary below the Python planner host.  Every entry point
  * replaces one piece of the reference's hot path (tud-airlab/mppi-isaac @ 2e6d5fb,
@@ -257,8 +257,8 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
                        float* action_out, float* stats, void* stream);
 
 /* multi-GPU exchange over peer memory (one process per GPU, one box) -----------------------------
- * Replaces the all-gather between K3 and K4 (the reference has no multi-GPU path; this is the B200
- * scale-out of its single-GPU mppi_torch reduction, SURVEY.md 8(e)).  Every rank owns a small
+ * Replaces the all-gather between K3 and K4 (the reference has no multi-GPU path; this is the
+ * multi-GPU scale-out of its single-GPU mppi_torch reduction, SURVEY.md 8(e)).  Every rank owns a small
  * WINDOW in its HBM: [2 parities][world] rows of 2 + T*nu floats plus one arrival flag per row.
  * With peers open, the last CTA of mppib_reduce stores this rank's (beta, eta, W) row straight
  * into the window of EVERY rank over NVLink (st.global + fence.sys + st.release.sys of the flag),

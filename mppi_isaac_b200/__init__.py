@@ -1,5 +1,5 @@
-"""mppi_isaac_b200 -- B200-native MPPI-with-simulated-rollouts hot path (drop-in for tud-airlab/mppi-isaac's
-``MPPIisaacPlanner`` rollout path).  The compute backend is the sm_100a CUDA library ``libmppib.so``
+"""mppi_isaac_b200 -- H100-native MPPI-with-simulated-rollouts hot path (drop-in for tud-airlab/mppi-isaac's
+``MPPIisaacPlanner`` rollout path).  The compute backend is the sm_90a CUDA library ``libmppib.so``
 (C ABI: ``include/mppib.h``); there is no CPU fallback."""
 from .planner.mppi_isaac import MPPIisaacPlanner  # noqa: F401
 from .planner.rollout_sim import RolloutSim  # noqa: F401

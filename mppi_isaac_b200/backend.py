@@ -1,7 +1,7 @@
 """ctypes binding of ``libmppib.so`` (the C ABI in ``include/mppib.h``).
 
 This is the only compute backend the package ships.  There is NO CPU fallback: if the CUDA
-library is missing or no sm_100a device is visible, construction fails loudly.  Device
+library is missing or no sm_90a device is visible, construction fails loudly.  Device
 memory, streams and ``torch.distributed`` come from PyTorch (plumbing); every kernel on the
 hot path is ours.  Tensors are passed as raw ``data_ptr()``s, the stream as
 ``torch.cuda.current_stream().cuda_stream`` -- no torch types cross the ABI.
@@ -39,7 +39,7 @@ def load_library():
     if not os.path.exists(_LIB_PATH):
         raise RuntimeError(
             f"{_LIB_PATH} not found: the CUDA extension is not built. Run `python __graft_entry__.py` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
     lib = C.CDLL(_LIB_PATH)
     lib.mppib_last_error.restype = C.c_char_p
     for name in SYMBOLS:
@@ -72,7 +72,7 @@ class CudaBackend:
         dev = torch.device(device)
         if dev.type != "cuda":
             raise RuntimeError(
-                f"mppi_isaac_b200 runs its hot path as sm_100a CUDA kernels only; device '{device}' is not a CUDA "
+                f"mppi_isaac_b200 runs its hot path as sm_90a CUDA kernels only; device '{device}' is not a CUDA "
                 "device and there is no CPU fallback (the reference's CPU pipeline is reproduced by oracle/ for tests only)")
         if not torch.cuda.is_available():
             raise RuntimeError("no CUDA device visible: mppi_isaac_b200 has no CPU fallback")

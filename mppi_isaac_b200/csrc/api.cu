@@ -91,7 +91,7 @@ int32_t mppib_create(const MppibModel* model_h, const MppibParams* params_h, int
     MPPIB_CHECK_CUDA(guard.err);
     cudaDeviceProp prop;
     MPPIB_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-    MPPIB_REQUIRE(prop.major == 10, "this library is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    MPPIB_REQUIRE(prop.major == 9 && prop.minor == 0, "this library is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     MppibContext* c = new MppibContext();
     memset(c, 0, sizeof(*c));
     c->device = device;

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of the mppib CUDA library (sm_100a only).
+// common.cuh -- shared declarations of the mppib CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

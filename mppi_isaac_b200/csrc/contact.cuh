@@ -370,8 +370,7 @@ __device__ __forceinline__ void shapes_world(const MppibModel& m, const Layout& 
 
 // Candidate partners of every shape as a bit mask (MPPIB_MAX_SHAPES <= 32), built once per CTA: a FREE shape is tested against every
 // shape of another body (free-free pairs once), a LINK shape against the STATIC ones.  The nested shape loops of detect() used to
-// re-derive this from the constant bank in every substep: 12 % of panda_pick's samples sat on those dependent constant loads
-// (profiles/r2_contact.md).
+// re-derive this from the constant bank in every substep, a chain of dependent constant loads.
 __device__ __forceinline__ uint32_t partner_mask(const MppibModel& m, int a) {
     const int ns = m.nshapes;
     uint32_t mask = 0;

@@ -46,7 +46,9 @@ int launch_cost_pose(long long n, const float* a, long long a_si, long long a_sr
     MPPIB_CHECK_CUDA(guard.err);
     const int block = 256;
     const long long want = (n + block - 1) / block;
-    const int grid = (int)(want < 148LL * 8 ? want : 148LL * 8);
+    int sms = 0;
+    MPPIB_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, attr.device));
+    const int grid = (int)(want < 8LL * sms ? want : 8LL * sms);
     mppib_cost_pose_kernel<<<grid, block, 0, s>>>(n, a, a_si, a_sr, b, b_si, b_sr, w_pos, w_ori, cost, accumulate);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -1,9 +1,8 @@
 // lanes_math.cuh -- vector / quaternion algebra of the lanes-per-rollout kernel (rollout_lanes.cu), generic in the scalar type:
 //   float : one rollout per lane group
-//   P2    : TWO rollouts per lane group, every arithmetic instruction a packed f32x2 one (FFMA2 / FMUL2 / FADD2 of sm_100: two
-//           IEEE fp32 results per issue slot; operands may be register pairs, negated pairs, broadcast scalars or immediates --
-//           checked in SASS).  One scheduler issues a 3-register FFMA every ~1.9 cycles and an FFMA2 every ~2.7
-//           (tools/ubench/fma_issue.cu): 1.4x the fp32 rate, and all non-arithmetic instructions are shared by the pair.
+//   P2    : TWO rollouts per lane group.  sm_90 has no packed f32x2 arithmetic, so every P2 operation is two independent
+//           scalar fp32 instructions (the same IEEE round-to-nearest results as the float instantiation); what the pair
+//           shares is the control, shuffle-index and address instructions, and the two chains give the scheduler ILP 2.
 // The formulas are written once against the few primitives below.
 #pragma once
 #include <cuda_runtime.h>
@@ -18,13 +17,13 @@ template <> struct scalar_traits<float> { static constexpr int N = 1; };
 template <> struct scalar_traits<P2> { static constexpr int N = 2; };
 
 // ---- arithmetic ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ P2 operator+(P2 a, P2 b) { P2 r; r.v = __fadd2_rn(a.v, b.v); return r; }
+__device__ __forceinline__ P2 operator+(P2 a, P2 b) { return mkp(__fadd_rn(a.v.x, b.v.x), __fadd_rn(a.v.y, b.v.y)); }
 __device__ __forceinline__ P2 operator-(P2 a) { return mkp(-a.v.x, -a.v.y); }                     // folds into the consumer's operand modifier
-__device__ __forceinline__ P2 operator-(P2 a, P2 b) { P2 r; r.v = __fadd2_rn(a.v, make_float2(-b.v.x, -b.v.y)); return r; }
-__device__ __forceinline__ P2 operator*(P2 a, P2 b) { P2 r; r.v = __fmul2_rn(a.v, b.v); return r; }
-__device__ __forceinline__ P2 operator*(P2 a, float c) { P2 r; r.v = __fmul2_rn(a.v, make_float2(c, c)); return r; }
+__device__ __forceinline__ P2 operator-(P2 a, P2 b) { return mkp(__fadd_rn(a.v.x, -b.v.x), __fadd_rn(a.v.y, -b.v.y)); }
+__device__ __forceinline__ P2 operator*(P2 a, P2 b) { return mkp(__fmul_rn(a.v.x, b.v.x), __fmul_rn(a.v.y, b.v.y)); }
+__device__ __forceinline__ P2 operator*(P2 a, float c) { return mkp(__fmul_rn(a.v.x, c), __fmul_rn(a.v.y, c)); }
 __device__ __forceinline__ P2 operator*(float c, P2 a) { return a * c; }
-__device__ __forceinline__ P2 operator+(P2 a, float c) { P2 r; r.v = __fadd2_rn(a.v, make_float2(c, c)); return r; }
+__device__ __forceinline__ P2 operator+(P2 a, float c) { return mkp(__fadd_rn(a.v.x, c), __fadd_rn(a.v.y, c)); }
 __device__ __forceinline__ P2 operator+(float c, P2 a) { return a + c; }
 __device__ __forceinline__ P2 operator-(P2 a, float c) { return a + (-c); }
 __device__ __forceinline__ P2 operator-(float c, P2 a) { return (-a) + c; }
@@ -32,11 +31,11 @@ __device__ __forceinline__ P2& operator+=(P2& a, P2 b) { a = a + b; return a; }
 
 // a * b + c
 __device__ __forceinline__ float fma_(float a, float b, float c) { return fmaf(a, b, c); }
-__device__ __forceinline__ P2 fma_(P2 a, P2 b, P2 c) { P2 r; r.v = __ffma2_rn(a.v, b.v, c.v); return r; }
-__device__ __forceinline__ P2 fma_(P2 a, float b, P2 c) { P2 r; r.v = __ffma2_rn(a.v, make_float2(b, b), c.v); return r; }
+__device__ __forceinline__ P2 fma_(P2 a, P2 b, P2 c) { return mkp(fmaf(a.v.x, b.v.x, c.v.x), fmaf(a.v.y, b.v.y, c.v.y)); }
+__device__ __forceinline__ P2 fma_(P2 a, float b, P2 c) { return mkp(fmaf(a.v.x, b, c.v.x), fmaf(a.v.y, b, c.v.y)); }
 __device__ __forceinline__ P2 fma_(float a, P2 b, P2 c) { return fma_(b, a, c); }
-__device__ __forceinline__ P2 fma_(P2 a, P2 b, float c) { P2 r; r.v = __ffma2_rn(a.v, b.v, make_float2(c, c)); return r; }
-__device__ __forceinline__ P2 fma_(P2 a, float b, float c) { P2 r; r.v = __ffma2_rn(a.v, make_float2(b, b), make_float2(c, c)); return r; }
+__device__ __forceinline__ P2 fma_(P2 a, P2 b, float c) { return mkp(fmaf(a.v.x, b.v.x, c), fmaf(a.v.y, b.v.y, c)); }
+__device__ __forceinline__ P2 fma_(P2 a, float b, float c) { return mkp(fmaf(a.v.x, b, c), fmaf(a.v.y, b, c)); }
 
 template <class F> __device__ __forceinline__ F bcast(float c);
 template <> __device__ __forceinline__ float bcast<float>(float c) { return c; }

@@ -28,7 +28,7 @@ __device__ __forceinline__ V3 mulT(const M3& m, V3 v) {
 
 // sin / cos with a two-term Cody-Waite reduction and the Cephes minimax polynomials on [-pi/4, pi/4]: max error 9e-8 for
 // |x| < 3000 rad (checked against float64), ~25 instructions and NO slow path.  CUDA's sincosf carries a Payne-Hanek
-// fallback whose code, registers and convergence barriers cost 11 % of this kernel (profiles/r1_rollout_tuning.md).
+// fallback whose code, registers and convergence barriers this kernel does not need.
 __device__ __forceinline__ void sincos_cw(float x, float* s_out, float* c_out) {
     const float k = rintf(x * 0.63661975f);
     float r = fmaf(-k, 1.5707964f, x);

@@ -146,7 +146,7 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, fl
         for (int e = e4; e < P4; e += 64) {
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             int c = cg;
-            for (; c + 60 < G; c += 64) {        // 16 independent 128-bit loads in flight: 148 CTA rows are two to three L2 round trips
+            for (; c + 60 < G; c += 64) {        // 16 independent 128-bit loads in flight: 132 CTA rows are two to three L2 round trips
                 float4 v[16];
 #pragma unroll
                 for (int u = 0; u < 16; ++u) v[u] = __ldcg(reinterpret_cast<const float4*>(scratch + (size_t)(c + 4 * u) * PP) + e);
@@ -358,7 +358,7 @@ mppib_reduce_kernel(const __grid_constant__ MppibParams p, const __grid_constant
 // consumer warps each own WHOLE tiles end to end -- S_k, minimum, weights, weighted row sums, online merge into the warp's own
 // running (beta, eta, W) in registers -- so nothing inside the streaming loop is CTA-wide: no __syncthreads, the only
 // synchronisation is the full / empty mbarrier pair of a ring stage (the first version above runs three block barriers per
-// tile; ncu: barrier stall 2.0 per issued instruction at K = 262 144, profiles/r1_reduce_v2.md).
+// tile, and its warps wait on them).
 //   tile i of this CTA -> ring stage i % NSTAGE, consumer i % NCONS;  full[s]: TMA complete_tx;  empty[s]: the consumer's arrive
 //   per tile and warp: phase A lane = sample (S_k = sum_t gamma^t c[t][k] + sum_r g[r] x[r][k], conflict-free column reads),
 //                      phase B warp shuffles (min, exp, sum), weights to a 32-float per-warp strip,
@@ -736,7 +736,7 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
         return launch_reduce_ws_t<16>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
     }
     // wide tiles once every SM has one; narrow tiles keep all SMs busy at small K
-    bool wide = c->params.K >= 64 * c->num_sms && reduce_smem_bytes<64, 3>(T, nu) <= 226 * 1024;   // tools/tune_reduce.py: 12.5 -> 11.7 us at K = 10 000
+    bool wide = c->params.K >= 64 * c->num_sms && reduce_smem_bytes<64, 3>(T, nu) <= 226 * 1024;   // A/B: tools/tune_reduce.py
     if (const char* e = getenv("MPPIB_K3_WIDE")) wide = atoi(e) != 0 && reduce_smem_bytes<64, 3>(T, nu) <= 226 * 1024;   // tuning knob
     if (const char* e = getenv("MPPIB_K3_VARIANT")) {          // tuning knob: "64x3" | "64x1" | "32x4" | "32x2"
         if (!strcmp(e, "64x1")) return launch_reduce_t<64, 1, 2>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);

@@ -9,7 +9,7 @@
 //   * per-body working set of a rollout lives in SHARED MEMORY as [slot][lane] (bank = lane: conflict free), so
 //     the three ABA sweeps are ROLLED loops over bodies.  The first version of this kernel unrolled everything
 //     into registers: 7.6k SASS instructions (122 KB) per substep body, far beyond the 32 KB L1.5 instruction
-//     cache, and ncu showed 41 % of all issue cycles stalled on `no_instruction` (profiles/r1_rollout_v1.md);
+//     cache, so issue stalled on instruction fetch;
 //   * serial chains (point robot, heijn, panda) carry the parent transform / articulated inertia / acceleration
 //     in registers from one body to the next (template CHAIN); general trees (gripper fingers) keep them in
 //     shared memory and index the parent at run time;
@@ -30,7 +30,7 @@
 // After the last substep of a model step the observed rows are written to obs[R][T][K].
 #include "common.cuh"
 
-// tuning knobs (profiles/r1_rollout_tuning.md records what each one bought)
+// tuning knobs (A/B builds: tools/tune_rollout.py)
 #ifndef ROLL_UNROLL_S1
 #define ROLL_UNROLL_S1 1      // unroll factor of sweep 1 (kinematics / inertia: bodies are independent apart from the frame recursion)
 #endif
@@ -568,12 +568,11 @@ int launch_t(MppibContext* c, const float* state0, const float* root0, float* st
 }  // namespace
 
 // Which kernel runs a scene.  Serial chains without contacts: one body per lane (rollout_lanes.cu).  Everything else the team kernel
-// can take (trees of up to 16 bodies in depth-first order, with or without contacts): a team of lanes per rollout (rollout_team.cu) --
-// 1.4 - 4.5x the thread-per-rollout kernel on contact-free trees, 2.0 - 2.4x on the contact scenes of robots with up to 8 joints at the
-// shard sizes of BASELINE C3 / C4 (1.4x at K = 16 000), 1.17x on the K = 8 192 shard of the 9-joint panda_pick scene (BASELINE C5) and
-// 0.99x at its full K = 65 536 (profiles/r2_team.md).  The choice does not depend on K, so a shard of a multi-GPU job runs the same
-// arithmetic as the single-GPU job (bit-identical rollouts, tests/test_gpu_sizes.py).  The thread-per-rollout kernel below remains for
-// scenes the team kernel does not take and as the A/B reference: MPPIB_K2_LANES=0 / MPPIB_K2_TEAM=0|1 force a mapping.
+// can take (trees of up to 16 bodies in depth-first order, with or without contacts): a team of lanes per rollout (rollout_team.cu),
+// which spreads a rollout over many lanes where this kernel gives it one thread.  The choice does not depend on K, so a shard of a
+// multi-GPU job runs the same arithmetic as the single-GPU job (bit-identical rollouts, tests/test_gpu_sizes.py).  The
+// thread-per-rollout kernel below remains for scenes the team kernel does not take and as the A/B reference:
+// MPPIB_K2_LANES=0 / MPPIB_K2_TEAM=0|1 force a mapping.
 int rollout_mapping(const MppibContext* c) {
     const MppibModel& m = c->model;
     if (c->k2_lanes && rollout_lanes_eligible(m)) return MPPIB_MAPPING_LANES;

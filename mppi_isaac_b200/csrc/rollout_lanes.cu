@@ -4,9 +4,9 @@
 // implement the same substep (same drive model, same saturation re-solve, same integration) and are tested against the same
 // oracle.
 //
-// Why a second mapping.  rollout.cu gives every rollout one thread; at the headline K = 10 000 that is 313 warps for the 592
-// warp schedulers of a B200, each walking a serial recursion of ~5 400 instructions per substep: the kernel time is the
-// latency of ONE warp and 47 % of the schedulers have no warp at all (profiles/r1_rollout_v3.md).  Here a rollout is spread
+// Why a second mapping.  rollout.cu gives every rollout one thread; at the headline K = 10 000 that is 313 warps for the 528
+// warp schedulers of an H100 (132 SMs x 4), each walking a serial recursion of ~5 400 instructions per substep: the kernel
+// time is the latency of ONE warp and 41 % of the schedulers have no warp at all.  Here a rollout is spread
 // over G = 8 lanes, so K = 10 000 becomes 2 500 warps of ~1 000 instructions per substep, and a shard of a strong-scaled plan
 // (K / 8 per GPU) still occupies every scheduler.
 //
@@ -24,9 +24,8 @@
 //   7. integrate     semi-implicit Euler, velocity and position limits (lane-local)
 // All exchanges are __shfl_*_sync with width G: no shared memory, no barriers.
 //
-// Scalar type F (lanes_math.cuh): float = one rollout per lane group; P2 = two rollouts per lane group with every arithmetic
-// instruction a packed FFMA2 / FMUL2 / FADD2 (1.4x the fp32 rate per issue slot, control / address instructions shared by the
-// pair); measured slower than the float instantiation on B200 and therefore opt-in (MPPIB_K2_PAIRS=1), see launch_rollout_lanes.
+// Scalar type F (lanes_math.cuh): float = one rollout per lane group; P2 = two rollouts per lane group (two independent fp32
+// instruction streams, control / address instructions shared by the pair); opt-in (MPPIB_K2_PAIRS=1), see launch_rollout_lanes.
 #include "common.cuh"
 #include "lanes_math.cuh"
 
@@ -35,10 +34,10 @@ namespace {
 using namespace lm;
 
 #ifndef LANES_MIN_CTAS
-#define LANES_MIN_CTAS 18      // resident 1-warp CTAs per SM the register allocation of the float kernel must allow (K = 10 000 -> 17 per SM at G = 8)
+#define LANES_MIN_CTAS 19      // resident 1-warp CTAs per SM the register allocation of the float kernel must allow (K = 10 000 -> 19 per SM at G = 8 on 132 SMs)
 #endif
 #ifndef LANES_MIN_CTAS_P2
-#define LANES_MIN_CTAS_P2 9    // the packed kernel: K = 10 000 -> 1 250 warps = 8.4 per SM
+#define LANES_MIN_CTAS_P2 10   // the pair kernel: K = 10 000 -> 1 250 warps = 9.5 per SM
 #endif
 
 template <class F> __device__ __forceinline__ F dot6(const V6T<F>& a, const V6T<F>& b) {
@@ -441,10 +440,8 @@ bool rollout_lanes_eligible(const MppibModel& m) {
 }
 
 int launch_rollout_lanes(MppibContext* c, const float* state0, float* state, const float* actions, int t0, int nsteps, float* obs, cudaStream_t s) {
-    // One rollout per lane group by default.  The packed instantiation (two rollouts per group, FFMA2 / FMUL2 / FADD2) halves the
-    // arithmetic instruction count per rollout but measured SLOWER at every K on B200 (K = 10 000: 258 vs 218 us, K = 65 536: 1188 vs
-    // 1124 us, profiles/r2_rollout_lanes.md): register-pair moves, doubled address arithmetic and 168 registers with spills eat the
-    // gain.  It stays selectable (MPPIB_K2_PAIRS=1) for re-measurement.
+    // One rollout per lane group by default.  The pair instantiation (two rollouts per group) shares the control and address
+    // instructions of the pair but needs about twice the registers per lane; it stays selectable (MPPIB_K2_PAIRS=1) for A/B runs.
     bool packed = c->k2_pairs > 0;
     if (packed) return launch_lanes_f<lm::P2>(c, state0, state, actions, t0, nsteps, obs, s);
     return launch_lanes_f<float>(c, state0, state, actions, t0, nsteps, obs, s);

@@ -3,11 +3,11 @@
 // not cover: panda + gripper, omnipanda, the planar differential-drive bases (boxer, albert, jackal), and BASELINE C3 / C4 / C5
 // (boxer_push, heijn_push, panda_pick).  Same spec as rollout.cu + contact.cuh (the thread-per-rollout kernel, kept for scenes outside
 // this kernel's limits and as the A/B reference: MPPIB_K2_TEAM=0) and as oracle/oracle.cpp; tested against the same oracle under
-// both mappings (tests/test_gpu_mappings.py).  Measurements and ncu: profiles/r2_team.md.
+// both mappings (tests/test_gpu_mappings.py).
 //
 // Why.  The thread-per-rollout contact kernels are ONE warp per SM walking a data-dependent stream of 23 - 32 k instructions per
-// (sub)step at CPI 3.7 (profiles/r2_contact.md): at the BASELINE shard sizes every CTA is resident at once, so their time is the
-// latency of a single warp, and 98 % of the machine idles.  Here:
+// (sub)step: at the BASELINE shard sizes every CTA is resident at once, so their time is the latency of a single warp, and most of
+// the machine idles.  Here:
 //   * ARTICULATION PHASE, G = 8 / 16 lanes per rollout, one body per lane: the composite-rigid-body / joint-space LDL^T formulation of
 //     rollout_lanes.cu generalised to trees (ancestor sums by pointer jumping, subtree sums as differences of suffix sums in depth-first
 //     order, leaves-first elimination so that the pivots are the articulated-body diagonals D_j);
@@ -54,7 +54,8 @@ enum : int { SH_R = 0, SH_C = 9, SH_HALF = 12, SH_MU = 15, SH_RAD = 16, SHN = 17
 // Two layouts of the per-rollout block.  ROOMY (robots of up to 8 joints): 20-float contact records, contact rows as one float4 per
 // coordinate -- one LDS.128 per coordinate slot and visit; these kernels run latency-bound with every CTA resident.  COMPACT (9 - 16
 // joints, e.g. panda_pick: 15 coordinates x 24 contacts of rows): 16-float records, rows as three planes of floats -- 20 % less shared
-// memory per rollout = 7 instead of 5 resident CTAs per SM, worth 1.25x there and a loss of 12 % on the small robots.
+// memory per rollout = 7 instead of 5 resident CTAs per SM; the roomy layout is the faster one per CTA for the small robots, which take
+// the compact one only where it saves a wave of CTAs (launch_team_contact).
 enum : int { CT_LN = 0, CT_LT1 = 1, CT_LT2 = 2, CT_MU = 3, CT_D = 4, CT_KN = 5, CT_KT1 = 6, CT_KT2 = 7, CT_P = 8, CT_IDS = 11, CT_N = 12, CT_T1 = 16 };
 enum : int { JB_R = 0, JB_O = 9, JB_SN = 12, JB_SF = 15, JB_VP = 18, JB_INVD = 19, JBN = 20 };
 constexpr float K_ROW_MIN = 1e-9f;     // contact rows with a smaller effective inverse mass [1/kg] are dropped (contact.cuh, oracle.cpp)
@@ -141,8 +142,7 @@ __device__ __forceinline__ uint32_t partner_mask(const MppibModel& m, int a) {
 // The teams of a warp see different numbers of contacts, but the control flow of the contact phase is kept WARP-UNIFORM: loops run to the
 // largest trip count among the teams of the warp and a team past its own count is predicated off.  (The teams of a warp wait for each
 // other at the next full-warp shuffle anyway; with team-divergent loops every shuffle would need the team's lane mask in a register,
-// which costs a MATCH / REDUX / VOTE convergence check per shuffle group -- 8 of the 83 instructions of a Gauss-Seidel visit, and
-// 11 % of its stall samples, profiles/r2_team.md.)
+// which costs a MATCH / REDUX / VOTE convergence check per shuffle group -- 8 of the 83 instructions of a Gauss-Seidel visit.)
 template <int G> __device__ __forceinline__ float team_sum(float v) {
 #pragma unroll
     for (int o = G / 2; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o, G);
@@ -230,8 +230,8 @@ __device__ __forceinline__ void kinematics(const BodyConst& bc, const Tree<R>& t
 // RPW = 32 / GC rollouts; with GC < G (the 9-joint panda_pick scene: G = 16, GC = 8) the articulation runs in G / GC passes over them --
 // it is a few per cent of the work -- so that the Gauss-Seidel sweeps, which are 3/4 of the work and whose cost per visit hardly depends
 // on the team width, serve four rollouts per warp instead of two.  The two phases talk through the joint block in shared memory.
-template <int G, int NB, bool CONTACT, int NCS, int GC>
-__global__ void __launch_bounds__(32, (CONTACT && G > 8) ? 8 : 12)   // compact-layout contact kernels: shared memory allows 7 CTAs per SM -> up to 255 registers, no spills (5 % there)
+template <int G, int NB, bool CONTACT, int NCS, int GC, bool COMPACT>
+__global__ void __launch_bounds__(32, (CONTACT && G > 8) ? 8 : 12)   // 9 - 16 joint contact kernels: shared memory allows 7 CTAs per SM -> up to 255 registers, no spills
 mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_constant__ MppibParams p,
                           const float* __restrict__ state0, const float* __restrict__ root0, float* __restrict__ state,
                           const float* __restrict__ actions, int t0, int nsteps, float* __restrict__ obs) {
@@ -250,7 +250,6 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     const int team = lane / G;
     const int k_first = (int)blockIdx.x * RPW;
     if (k_first >= K) return;
-    constexpr bool COMPACT = G > 8;                             // layout of the per-rollout block (see CT_*)
     constexpr int CTN = COMPACT ? 16 : 20;
     const TLayout L(nb, m.nfree, m.nshapes, m.max_contacts, GC, COMPACT);
     const int xstride = team_stride(L.total, GC);
@@ -1077,39 +1076,79 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     }
 }
 
-template <int G, int NB, bool CONTACT, int NCS, int GC>
-int launch_team_t(MppibContext* c, const float* state0, const float* root0, float* state, const float* actions, int t0, int nsteps, float* obs, cudaStream_t s) {
-    const int K = c->params.K;
-    constexpr int RPW = 32 / GC;
-    const TLayout L(c->model.nb, c->model.nfree, c->model.nshapes, c->model.max_contacts, GC, G > 8);
-    const size_t smem = CONTACT ? sizeof(float) * (size_t)RPW * team_stride(L.total, GC) : 0;
+// dynamic shared memory of a team CTA; raises the kernel's limit on this device where it needs more than the default 48 KB
+template <int G, int NB, bool CONTACT, int NCS, int GC, bool COMPACT>
+int team_smem(MppibContext* c, size_t* smem_out) {
+    const TLayout L(c->model.nb, c->model.nfree, c->model.nshapes, c->model.max_contacts, GC, COMPACT);
+    const size_t smem = CONTACT ? sizeof(float) * (size_t)(32 / GC) * team_stride(L.total, GC) : 0;
     MPPIB_REQUIRE(smem <= 200 * 1024, "mppib_rollout: %zu bytes of shared memory per team CTA", smem);
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > 48 * 1024 && smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_rollout_team_kernel<G, NB, CONTACT, NCS, GC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_rollout_team_kernel<G, NB, CONTACT, NCS, GC, COMPACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
+    *smem_out = smem;
+    return 0;
+}
+
+template <int G, int NB, bool CONTACT, int NCS, int GC, bool COMPACT>
+int launch_team_t(MppibContext* c, const float* state0, const float* root0, float* state, const float* actions, int t0, int nsteps, float* obs, cudaStream_t s) {
+    const int K = c->params.K;
+    constexpr int RPW = 32 / GC;
+    size_t smem = 0;
+    if (int rc = team_smem<G, NB, CONTACT, NCS, GC, COMPACT>(c, &smem)) return rc;
     const int ctas = (K + RPW - 1) / RPW;
-    mppib_rollout_team_kernel<G, NB, CONTACT, NCS, GC><<<ctas, 32, smem, s>>>(c->model, c->params, state0, root0, state, actions, t0, nsteps, obs);
+    mppib_rollout_team_kernel<G, NB, CONTACT, NCS, GC, COMPACT><<<ctas, 32, smem, s>>>(c->model, c->params, state0, root0, state, actions, t0, nsteps, obs);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+// waves of resident CTAs a contact launch of this K needs on this device (CTAs per SM from shared memory and registers)
+template <int G, int NB, int NCS, int GC, bool COMPACT>
+int team_waves(MppibContext* c, int* waves) {
+    size_t smem = 0;
+    if (int rc = team_smem<G, NB, true, NCS, GC, COMPACT>(c, &smem)) return rc;
+    int per_sm = 0;
+    MPPIB_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mppib_rollout_team_kernel<G, NB, true, NCS, GC, COMPACT>, 32, smem));
+    MPPIB_REQUIRE(per_sm > 0, "mppib_rollout: a team CTA of %zu bytes of shared memory does not fit an SM", smem);
+    const long long ctas = (c->params.K + 32 / GC - 1) / (32 / GC), slots = (long long)per_sm * c->num_sms;
+    *waves = (int)((ctas + slots - 1) / slots);
+    return 0;
+}
+
+// Layout of the per-rollout block of a contact scene (see CT_*): 9 - 16 joints always take the compact one.  Up to 8 joints the roomy
+// one is faster per CTA, but its CTAs are larger: where it needs more waves of resident CTAs than the compact one at this K (BASELINE
+// C3, K = 4 000 on 132 SMs: 1 000 CTAs, 7 per SM roomy, 9 per SM compact), the compact one runs.  Both layouts hold the same values,
+// so the choice does not change the arithmetic.
+template <int G, int NB, int NCS, int GC>
+int launch_team_contact(MppibContext* c, const float* state0, const float* root0, float* state, const float* actions, int t0, int nsteps,
+                        float* obs, cudaStream_t s) {
+    if constexpr (G > 8) {
+        return launch_team_t<G, NB, true, NCS, GC, true>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+    } else {
+        int w_roomy = 0, w_compact = 0;
+        if (int rc = team_waves<G, NB, NCS, GC, false>(c, &w_roomy)) return rc;
+        if (int rc = team_waves<G, NB, NCS, GC, true>(c, &w_compact)) return rc;
+        if (w_compact < w_roomy) return launch_team_t<G, NB, true, NCS, GC, true>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+        return launch_team_t<G, NB, true, NCS, GC, false>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+    }
 }
 
 // contact scenes: 8 lanes per rollout in the contact phase; coordinate slots per lane (compile time) = ceil((nb + 6 nfree) / 8)
 template <int G, int NB>
 int launch_team_g(MppibContext* c, bool contact, const float* state0, const float* root0, float* state, const float* actions, int t0, int nsteps, float* obs,
                   cudaStream_t s) {
-    if (!contact) return launch_team_t<G, NB, false, 1, G>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+    if (!contact) return launch_team_t<G, NB, false, 1, G, (G > 8)>(c, state0, root0, state, actions, t0, nsteps, obs, s);
     constexpr int GC = 8;
     const int ncs = (c->model.nb + 6 * c->model.nfree + GC - 1) / GC;
     switch (ncs) {
-        case 1: return launch_team_t<G, NB, true, 1, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
-        case 2: return launch_team_t<G, NB, true, 2, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
-        case 3: return launch_team_t<G, NB, true, 3, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
-        case 4: return launch_team_t<G, NB, true, 4, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+        case 1: return launch_team_contact<G, NB, 1, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+        case 2: return launch_team_contact<G, NB, 2, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+        case 3: return launch_team_contact<G, NB, 3, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+        case 4: return launch_team_contact<G, NB, 4, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
         default: MPPIB_REQUIRE(ncs <= MAXS_ALL, "mppib_rollout: %d coordinate slots per lane", ncs);
-                 return launch_team_t<G, NB, true, 5, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
+                 return launch_team_contact<G, NB, 5, GC>(c, state0, root0, state, actions, t0, nsteps, obs, s);
     }
 }
 

@@ -2,8 +2,8 @@
 
 An Objective is user code: anything written with torch ops on the views ``RolloutSim`` hands out works.  The terms below
 are the ones the reference's example Objectives are made of, as single CUDA kernels of ``libmppib.so`` -- the pose-reach
-cost of ``examples/panda/planner.py:22-40`` costs ~28 element-wise torch launches (~57 us at K = 10 000, T = 30) and
-one launch (~3 us) here.  CPU tensors (the checker backend of the tests) take the torch formulation.
+cost of ``examples/panda/planner.py:22-40`` costs ~28 element-wise torch launches (~61 us at K = 10 000, T = 30 on an H100) and
+one launch (~4 us) here.  CPU tensors (the checker backend of the tests) take the torch formulation.
 """
 import ctypes as C
 

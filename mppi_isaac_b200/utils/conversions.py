@@ -8,7 +8,7 @@ keeps pytorch3d's real-first convention so that the literal arithmetic of those 
 
 Provenance: ``quaternion_to_matrix``, ``_angle_from_tan`` and ``matrix_to_euler_angles`` follow the public formulas of
 pytorch3d's ``transforms/rotation_conversions.py`` (Meta Platforms, BSD licence) -- third-party code the reference depends on,
-not code of ``/root/reference``; they have to reproduce that library's numbers exactly, so their structure is the library's.
+not code of the reference repository; they have to reproduce that library's numbers exactly, so their structure is the library's.
 """
 import torch
 

@@ -4,7 +4,7 @@
 // load this library; the product package never imports it (it fails loudly without CUDA).
 //
 // PARITY UNPINNED: the arithmetic of this path lives in two third-party engines that are not
-// in /root/reference and cannot be installed here -- mppi_torch @75e17e87 (pyproject.toml:20,
+// in the reference repository and cannot be installed with it -- mppi_torch @75e17e87 (pyproject.toml:20,
 // poetry.lock:1273-1293) and IsaacGym 1.0rc4 / PhysX (pyproject.toml:16, thirdparty/README.md:3).
 // The reference ships no golden vectors for them (SURVEY.md section 4).  This file therefore
 // restates the *pipeline* the reference source does pin, function by function:

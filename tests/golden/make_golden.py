@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""Generates the golden fixtures in this directory (run in the build container).
+"""Generates the golden fixtures in this directory:  python tests/golden/make_golden.py <path to an mppi-isaac checkout>
 
 * savgol_w9_o2.json : scipy.signal.savgol_filter(window_length=9, polyorder=2, mode='interp', axis=0) on seeded
   random (T, 7) sequences -- the filter mppi_torch applies when filter_u is set (SURVEY.md Appendix C).
 * fk_reference_urdf.json : forward-kinematics known answers computed straight from the reference URDFs
-  (/root/reference/assets/urdf/**) by an independent 4x4 homogeneous-transform walk (no model compiler).
+  (<checkout>/assets/urdf/**) by an independent 4x4 homogeneous-transform walk (no model compiler).
 """
 import json
 import math
 import os
+import sys
 import xml.etree.ElementTree as ET
 
 import numpy as np
@@ -78,7 +79,7 @@ def urdf_fk(path, qmap, base=np.eye(4)):
 
 
 def fk():
-    A = "/root/reference/assets/urdf/"
+    A = os.path.join(sys.argv[1], "assets", "urdf") + os.sep
     rng = np.random.default_rng(7)
     cases = []
     specs = [
@@ -99,7 +100,7 @@ def fk():
             cases.append(dict(urdf=rel, base_pos=list(base_p), q=q.tolist(),
                               links={k: dict(p=v[:3, 3].tolist(), R=v[:3, :3].tolist()) for k, v in Ts.items()}))
     with open(os.path.join(HERE, "fk_reference_urdf.json"), "w") as fh:
-        json.dump(dict(source="independent homogeneous-transform FK over /root/reference/assets/urdf", cases=cases), fh)
+        json.dump(dict(source="independent homogeneous-transform FK over the reference's assets/urdf", cases=cases), fh)
 
 
 if __name__ == "__main__":

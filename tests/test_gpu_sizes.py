@@ -106,7 +106,7 @@ def _pick_scene(K, T):
 
 
 def test_c5_panda_pick_shard_size_lockstep(oracle):
-    """BASELINE C5 on one of its 8 GPUs: panda_pick, K = 8 192, T = 30 (two waves of 222 KB CTAs on 148 SMs): the gripper closes on
+    """BASELINE C5 on one of its 8 GPUs: panda_pick, K = 8 192, T = 30 (two waves of 222 KB CTAs on 132 SMs): the gripper closes on
     the block while the arm moves; every fifth step of the horizon in lock-step."""
     K, T = 8192, 30
     sc, p, s0 = _pick_scene(K, T)
@@ -136,6 +136,26 @@ def test_c5_full_size_determinism_and_shard_invariance():
     o8 = torch.zeros((R, T, 8192), device=DEV)
     be8.rollout(s0_d, None, dev(a[:, :, 3 * 8192:4 * 8192]), 0, T, o8, root0=root_d)
     assert torch.equal(o8, o1[:, :, 3 * 8192:4 * 8192])
+
+
+def test_c3_shard_invariance_across_team_layouts():
+    """BASELINE C3 at K = 4 000: the whole launch and a 512-sample shard of it (k_offset keys the per-rollout randomisation) are
+    bit-identical, also where the two launches take different shared-memory layouts of the team kernel (on 132 SMs the 4 000-sample
+    launch takes the compact one, which fits its 1 000 CTAs in one wave, and the shard the roomy one)."""
+    K, T, KS, off = 4000, 20, 512, 1024
+    sc, p, s0 = boxer_setup(K=K, T=T)
+    be = gpu_backend(sc, p)
+    rng = np.random.default_rng(12)
+    a = np.stack([rng.uniform(0.3, 1.2, (T, K)), rng.uniform(-1.0, 1.0, (T, K))], axis=1).astype(np.float32)
+    a_d, root_d, s0_d = dev(a), dev(sc.root_state0), dev(s0)
+    R = be.obs_size()
+    o = torch.zeros((R, T, K), device=DEV)
+    be.rollout(s0_d, None, a_d, 0, T, o, root0=root_d)
+    ps = copy.copy(p); ps.K, ps.k_offset = KS, off
+    bs = gpu_backend(sc, ps)
+    o_s = torch.zeros((R, T, KS), device=DEV)
+    bs.rollout(s0_d, None, dev(a[:, :, off:off + KS]), 0, T, o_s, root0=root_d)
+    assert torch.isfinite(o).all() and torch.equal(o_s, o[:, :, off:off + KS])
 
 
 @pytest.mark.parametrize("which,K", [("gripper", 65536), ("point", 65536), ("panda", 131072), ("gripper", 8192)])

@@ -1,18 +1,20 @@
 """URDF -> model-constants compiler: pinned against forward kinematics computed straight from the reference URDFs by
 an independent homogeneous-transform walk (tests/golden/fk_reference_urdf.json, made by make_golden.py), the
-known answers of SURVEY.md Appendix B, and -- in the build container only -- a re-compile from /root/reference."""
+known answers of SURVEY.md Appendix B, and a re-compile of the reference's URDFs and example scenes
+(tests/golden/reference_configs.json, made by make_reference_configs.py)."""
+import glob
 import json
 import os
 
 import numpy as np
 import pytest
 
-from conftest import REFERENCE, has_reference
 from mppi_isaac_b200.model.blob import compiled_path, build_scene
-from mppi_isaac_b200.model.urdf import (compile_urdf, forward_kinematics, load_compiled, mesh_inertia, quat_xyzw_to_R)
+from mppi_isaac_b200.model.urdf import (forward_kinematics, load_compiled, mesh_inertia, quat_xyzw_to_R)
 from mppi_isaac_b200.utils.config_store import load_actor_cfgs, load_config, load_isaacgym_config
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+CONF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "mppi_isaac_b200", "conf")
 
 
 def test_fk_of_compiled_models_matches_reference_urdf_fk():
@@ -93,34 +95,36 @@ def test_config_loader_builtin_and_errors(tmp_path):
         load_config(str(f))
 
 
-@pytest.mark.skipif(not has_reference(), reason="reference checkout only exists in the build container")
 def test_reference_configs_and_urdfs_load_unchanged():
-    import glob
-    conf = [os.path.join(REFERENCE, "conf")]
-    tasks = sorted(glob.glob(os.path.join(REFERENCE, "examples", "*", "*.yaml")))
+    """Against what the package's loaders and URDF compiler made of the upstream mppi-isaac checkout (its example task YAMLs,
+    conf/ and assets/; tests/golden/reference_configs.json, made by make_reference_configs.py): the shipped pre-compiled models
+    equal a fresh compile of the upstream URDFs, and every example scene whose actors the package ships builds from the
+    package's own conf/ into the same articulation as from upstream's."""
+    with open(os.path.join(GOLD, "reference_configs.json")) as f:
+        gold = json.load(f)
+    tasks = gold["tasks"]
     assert len(tasks) >= 10
-    for t in tasks:
-        cfg = load_config(t, conf)
-        assert cfg.mppi.num_samples > 0 and len(cfg.actors) > 0
-    for rel in ("point_robot.urdf", "heijn/heijn.urdf", "panda_isaac/robots/franka_panda_stick.urdf"):
-        fresh = compile_urdf(os.path.join(REFERENCE, "assets", "urdf", rel))
+    assert all(t["num_samples"] > 0 and len(t["actors"]) > 0 for t in tasks.values())
+    for rel, fresh in gold["urdfs"].items():
         shipped = load_compiled(compiled_path(rel))
-        np.testing.assert_allclose(fresh.mass, shipped.mass, rtol=1e-12)
-        np.testing.assert_allclose(fresh.inertia_o, shipped.inertia_o, rtol=1e-9, atol=1e-12)
-        assert fresh.link_names == shipped.link_names and fresh.dof_names == shipped.dof_names
-    # every example scene of the reference builds from ITS conf/ and assets/ (anymal: legged floating base, out of scope)
-    built = {}
-    for t in tasks:
-        cfg = load_config(t, conf)
-        name = os.path.basename(os.path.dirname(t))
-        try:
-            sc = build_scene(load_actor_cfgs(cfg.actors, conf), assets_dirs=[os.path.join(REFERENCE, "assets")], substep=cfg.isaacgym.dt / cfg.isaacgym.substeps)
-            built[name] = (sc.model.nb, sc.nu)
-        except NotImplementedError as e:
-            built[name] = str(e)
+        np.testing.assert_allclose(fresh["mass"], shipped.mass, rtol=1e-12)
+        np.testing.assert_allclose(np.reshape(fresh["inertia_o"], np.shape(shipped.inertia_o)), shipped.inertia_o, rtol=1e-9, atol=1e-12)
+        assert fresh["link_names"] == list(shipped.link_names) and fresh["dof_names"] == list(shipped.dof_names)
+    # every example scene of the reference built from ITS conf/ and assets/ (anymal: legged floating base, out of scope)
+    built = {os.path.dirname(k): (tuple(t["scene"]) if isinstance(t["scene"], list) else t["scene"]) for k, t in tasks.items()}
     assert isinstance(built.pop("anymal"), str)
     assert all(isinstance(v, tuple) for v in built.values()), built
     assert built["albert"] == (12, 9) and built["omni_panda_pick"] == (12, 12) and built["panda_effort"] == (7, 7) and built["panda_stick_push"][0] == 7
-    a = load_actor_cfgs(["panda_stick", "goal"], conf)
+    shipped_actors = {os.path.splitext(os.path.basename(p))[0] for p in glob.glob(os.path.join(CONF, "actors", "*.yaml"))}
+    rebuilt = 0
+    for k, t in tasks.items():
+        if not isinstance(t["scene"], list) or not set(t["actors"]) <= shipped_actors:
+            continue
+        sc = build_scene(load_actor_cfgs(t["actors"]), substep=t["dt"] / t["substeps"])
+        assert [sc.model.nb, sc.nu] == t["scene"], k
+        rebuilt += 1
+    assert rebuilt >= 8
     b = load_actor_cfgs(["panda_stick", "goal"])
-    assert a[0].urdf_file == b[0].urdf_file and a[0].init_joint_pose == b[0].init_joint_pose and a[1].init_pos == b[1].init_pos
+    a = gold["actors"]
+    assert a["panda_stick"]["urdf_file"] == b[0].urdf_file and a["panda_stick"]["init_joint_pose"] == list(b[0].init_joint_pose)
+    assert a["goal"]["init_pos"] == list(b[1].init_pos)

@@ -1,9 +1,8 @@
 #!/usr/bin/env python
 """Pre-compile the hot-path robots into mppi_isaac_b200/models_compiled/*.json.
 
-The GPU boxes have no /root/reference, so the constant blocks derived from the reference's
-URDF + collision meshes (assets/urdf/**, 96 MB, not copied) are generated here once and
-committed.  Usage:  python tools/compile_models.py [/root/reference/assets]
+The reference's URDF + collision meshes (assets/urdf/**, 96 MB) are not part of this repository, so the constant blocks
+derived from them are generated once and committed.  Usage:  python tools/compile_models.py <mppi-isaac checkout>/assets
 """
 import os
 import sys
@@ -25,7 +24,7 @@ ROOT_MASS = {"jackal/jackal.urdf": 40.0}                              # ActorWra
 
 
 def main():
-    assets = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/assets"
+    assets = sys.argv[1]
     for rel in ROBOTS:
         model = compile_urdf(os.path.join(assets, "urdf", rel), fixed_base=True)
         out = compiled_path(rel)

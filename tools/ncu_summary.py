@@ -2,7 +2,7 @@
 """Key numbers of an ncu report (`ncu --set full ... -o report`), read here without a GPU:
     python tools/ncu_summary.py report.ncu-rep [report2.ncu-rep ...]
 duration, launch shape, registers, shared memory, executed warp instructions, issue-slot utilisation, stall reasons per issued
-instruction, pipe utilisation, DRAM bytes (traffic) -- the table that goes into profiles/*.md."""
+instruction, pipe utilisation, DRAM bytes (traffic)."""
 import csv
 import subprocess
 import sys

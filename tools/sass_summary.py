@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Opcode histogram per kernel from `cuobjdump -sass` (static instruction counts; evidence for profiles/*_sass_summary.txt).
+"""Opcode histogram per kernel from `cuobjdump -sass` (static instruction counts).
 
     python tools/sass_summary.py [path/to/lib.so | file.o] [--filter substring] [--top N]
 
-Prints, per kernel: total SASS instructions, the share of FP32 (FFMA / FMUL / FADD / FFMA2 ...), shuffles, shared- and global-memory
+Prints, per kernel: total SASS instructions, the share of FP32 (FFMA / FMUL / FADD), shuffles, shared- and global-memory
 instructions, and the TMA / mbarrier / cp.async mnemonics that prove which hardware paths a kernel uses (UTMALDG = TMA load,
-SYNCS = mbarrier, LDGSTS = cp.async, UTC*MMA = tcgen05 -- none expected here: the path has no dense contraction).
+SYNCS = mbarrier, LDGSTS = cp.async, HGMMA = wgmma -- none expected here: the path has no dense contraction).
 """
 import argparse
 import collections
@@ -41,7 +41,7 @@ def histogram(path):
 
 
 GROUPS = [
-    ("fp32", ("FFMA", "FMUL", "FADD", "FFMA2", "FMUL2", "FADD2")),
+    ("fp32", ("FFMA", "FMUL", "FADD")),
     ("mufu", ("MUFU",)),
     ("shfl", ("SHFL",)),
     ("lds/sts", ("LDS", "STS", "LDSM")),
@@ -51,7 +51,7 @@ GROUPS = [
     ("mbarrier", ("SYNCS",)),
     ("cp.async", ("LDGSTS",)),
     ("bar", ("BAR",)),
-    ("tcgen05", ("UTCHMMA", "UTCQMMA", "UTCIMMA", "UTCOMMA", "LDTM", "STTM")),
+    ("wgmma", ("HGMMA", "IGMMA", "QGMMA", "BGMMA")),
 ]
 
 

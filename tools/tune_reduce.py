@@ -10,11 +10,11 @@ Ks = [int(a) for a in sys.argv[1:]] or [10000, 65536]
 code = ("import sys; sys.path.insert(0, %r); import bench, torch, numpy as np\n"
         "from mppi_isaac_b200 import MPPIisaacPlanner\nfrom mppi_isaac_b200.objectives import PandaReachObjective\n"
         "p = MPPIisaacPlanner(bench.panda_cfg(10000, 'cuda:0'), PandaReachObjective(), use_cuda_graph=False)\n"
-        "r = bench.k3_roofline(p, 6486.5, 'x', %r)\n"
+        "r = bench.k3_roofline(p, 3350.0, 'x', %r)\n"
         "print('RES', ' '.join('%%d:%%.2f' %% (e['K'], e['us']) for e in r))\n") % (ROOT, Ks)
 res = {}
-CASES = [{}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "296"}, {"MPPIB_K3_VARIANT": "64x1", "MPPIB_K3_GRID": "296"},
-         {"MPPIB_K3_VARIANT": "32x4"}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "148"}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "444"}]
+CASES = [{}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "264"}, {"MPPIB_K3_VARIANT": "64x1", "MPPIB_K3_GRID": "264"},
+         {"MPPIB_K3_VARIANT": "32x4"}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "132"}, {"MPPIB_K3_VARIANT": "32x2", "MPPIB_K3_GRID": "396"}]
 for case in CASES:
     env = dict(os.environ, **case)
     out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True)

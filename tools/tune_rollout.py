@@ -24,7 +24,7 @@ if sys.argv[1] == "build":
     csrc = os.path.join(ROOT, "mppi_isaac_b200", "csrc")
     for name, flags in VARIANTS.items():
         so = os.path.join(OUT, f"libmppib_{name}.so")
-        cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
+        cmd = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
                "-diag-suppress", "177", *flags, "-o", so] + [os.path.join(csrc, f) for f in ("api.cu", "sample.cu", "rollout.cu", "reduce.cu", "cost.cu")]
         subprocess.check_call(cmd)
         print("built", so)
