@@ -288,10 +288,11 @@ int32_t mppib_cost_pose(int64_t n, const float* a, int64_t a_si, int64_t a_sr, c
  * lets the model compiler size `max_contacts` to what fits an SM (226 KB usable) before a handle exists.                     */
 int64_t mppib_rollout_smem_bytes(const MppibModel* model_h);
 
-/* Which rollout kernel mppib_rollout launches for this handle's model and K (diagnostics / benchmark reporting; the result of the
+/* Which rollout kernel mppib_rollout launches for this handle's model (diagnostics / benchmark reporting; the result of the
  * rollout does not depend on it beyond float32 rounding -- every mapping is tested against the same oracle):
  * one thread per rollout, one articulation body per lane (serial chains without contacts), or a team of lanes per rollout
- * (trees; contact scenes of small robots).  Environment MPPIB_K2_LANES=0, MPPIB_K2_TEAM=0|1 force a mapping.               */
+ * (trees; contact scenes of small robots).  The choice depends on the scene, never on K.  Environment MPPIB_K2_LANES=0 /
+ * MPPIB_K2_TEAM=0 switch the lanes / team mapping off (the scene then falls to the next one, down to one thread per rollout). */
 #define MPPIB_MAPPING_THREAD 0
 #define MPPIB_MAPPING_LANES  1
 #define MPPIB_MAPPING_TEAM   2

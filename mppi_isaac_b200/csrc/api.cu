@@ -73,12 +73,13 @@ extern "C" {
 int32_t mppib_abi_version(void) { return MPPIB_ABI_VERSION; }
 const char* mppib_last_error(void) { return g_err; }
 
-// the K2 mapping knobs of the environment (A/B runs): MPPIB_K2_LANES=0, MPPIB_K2_TEAM=0|1
+// the K2 mapping switches of the environment: MPPIB_K2_LANES=0 / MPPIB_K2_TEAM=0 turn a mapping off (the thread-per-rollout
+// kernel as the reference of the other two)
 static void read_mapping_knobs(MppibContext* c) {
-    c->k2_lanes = 1;
+    c->k2_lanes = true;
     if (const char* e = getenv("MPPIB_K2_LANES")) c->k2_lanes = atoi(e) != 0;
-    c->k2_team = -1;
-    if (const char* e = getenv("MPPIB_K2_TEAM")) c->k2_team = atoi(e) < 0 ? -1 : (atoi(e) != 0);
+    c->k2_team = true;
+    if (const char* e = getenv("MPPIB_K2_TEAM")) c->k2_team = atoi(e) != 0;
 }
 
 int32_t mppib_create(const MppibModel* model_h, const MppibParams* params_h, int32_t device, MppibHandle* out) {
@@ -99,9 +100,6 @@ int32_t mppib_create(const MppibModel* model_h, const MppibParams* params_h, int
     c->params = *params_h;
     c->num_sms = prop.multiProcessorCount;
     read_mapping_knobs(c);                                                      // read once per handle, not per launch
-    c->k2_pairs = -1;
-    if (const char* e = getenv("MPPIB_K2_PAIRS")) c->k2_pairs = atoi(e) != 0;
-    c->k3_variant = (getenv("MPPIB_K3_VARIANT") || getenv("MPPIB_K3_WIDE") || getenv("MPPIB_K3_GRID")) ? 1 : 0;
     derive(c);
     if (int rc = alloc_scratch(c)) { delete c; return rc; }
     *out = c;

@@ -45,11 +45,9 @@ struct MppibContext {
     void* peer_win[MPPIB_MAX_PEERS];           // window base of every rank (own entry = local allocation)
     unsigned long long peer_timeout_ns;
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
-    int k3_variant;                            // 0 = warp-specialised K3 (default), 1 = block-synchronous K3 (MPPIB_K3_VARIANT / _WIDE / _GRID knobs)
-    int k2_pairs;                              // lanes kernel: -1 = choose by K (default), 0 / 1 = force one / two rollouts per lane group (MPPIB_K2_PAIRS)
-    int k2_team;                               // K2 mapping for trees / contact scenes: 1 = a team of lanes per rollout (rollout_team.cu), 0 = one thread per
-                                               // rollout, -1 = choose by scene and K (default; rollout_mapping())
-    int k2_lanes;                              // K2 mapping for eligible scenes: 1 = one body per lane (default), 0 = one thread per rollout
+    // K2 mappings the handle may use (rollout_mapping() picks by scene, never by K); both default to true
+    bool k2_team;                              // a team of lanes per rollout for trees / contact scenes (rollout_team.cu); MPPIB_K2_TEAM=0 turns it off
+    bool k2_lanes;                             // one body per lane for serial chains (rollout_lanes.cu); MPPIB_K2_LANES=0 turns it off
 };
 
 // Every C-ABI entry that touches the device runs on the handle's device, whatever the calling thread's current device is (an

@@ -5,9 +5,9 @@
 // spec SURVEY.md 8(a) M5/M6 and 8(e)).
 //
 // K3 data flow (HBM-bound; every input byte is read from HBM exactly once):
-//   * persistent CTAs (one per SM), each walks tiles of W samples: tile = x[T*nu][W] + cost[T][W]
-//   * tiles arrive by TMA (cp.async.bulk.tensor.2d, one elected thread, mbarrier complete_tx) into an NS-deep
-//     shared-memory ring, so NS-1 tiles (~90 KB / SM) are always in flight while the CTA computes
+//   * persistent CTAs (one per SM), each walks tiles of 32 samples: tile = x[T*nu][32] + cost[T][32]
+//   * tiles arrive by TMA (cp.async.bulk.tensor.2d, one elected thread, mbarrier complete_tx) into a shared-memory
+//     ring of up to 8 stages, so several tiles are always in flight while the CTA computes
 //   * per tile:  S_k = sum_t gamma^t cost[t][k]  (+ sum_r g[r] x[r][k],  g = lambda Sigma^-1 U,  SIMPLE mode)
 //                b = min_k S_k ; w_k = exp(-(S_k - b)/lambda) ; eta = sum_k w_k ; W[r] = sum_k w_k x[r][k]
 //     and an online log-sum-exp merge into the CTA's running (beta, eta, W) -- no second pass for the minimum
@@ -20,7 +20,6 @@
 namespace {
 
 constexpr int NT = 256;         // threads per CTA
-constexpr int RPT = 2;          // rows of W per thread (T*nu <= 512)
 constexpr int MAX_GRID = 512;   // persistent CTAs (<= scratch rows)
 
 __device__ __forceinline__ float warp_min(float v) {
@@ -116,8 +115,8 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
 }
 
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
-// every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = at least MAX_GRID + 4 * (P + 3)
-// floats of idle shared memory, `misc` = 8 floats.
+// every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
+// at least, `misc` = 8 floats.
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda) {
@@ -198,175 +197,39 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, fl
     }
 }
 
-template <int W, int NS, int MINB>
-__global__ void __launch_bounds__(NT, MINB)
-mppib_reduce_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
-              int nu, int xbox_rows, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
-              float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
-              float* __restrict__ fin_stats, float* __restrict__ fin_mirror) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    constexpr int KPL = W / 32;   // samples per lane
-    const int K = p.K, T = p.T, NR = T * nu;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const float inv_lambda = 1.0f / p.lambda_;
-    const bool simple = p.mode == MPPIB_MODE_SIMPLE;
-
-    const int tile_floats = (NR + T) * W;
-    float* tiles = reinterpret_cast<float*>(smem_raw);                       // [NS][(NR+T)*W], each stage 128-B aligned
-    const int stage_floats = (tile_floats + 31) & ~31;
-    float* g = tiles + (size_t)NS * stage_floats;                            // [NR]  lambda * Sigma^-1 U (SIMPLE)
-    float* gp = g + ((NR + 3) & ~3);                                         // [T]   gamma^t          (every array 16-B aligned:
-    float* red = gp + ((T + 3) & ~3);                                        // [8][W]                  wk is read as float4)
-    float* wk = red + 8 * W;                                                 // [W]
-    float* misc = wk + W;                                                    // [8]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + (((size_t)((misc + 8) - tiles) * 4 + 15) & ~(size_t)15));  // [NS] mbarriers
-
-    const int ntiles = (K + W - 1) / W;
-    const int my_tiles = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-    const uint32_t tile_bytes = (uint32_t)tile_floats * 4u;
-
-    auto issue = [&](int i) {   // elected thread: TMA the i-th tile of this CTA into ring slot i % NS
-        const int s = i % NS, k0 = ((int)blockIdx.x + i * (int)gridDim.x) * W;
-        float* dst = tiles + (size_t)s * stage_floats;
-        mbar_expect_tx(&full[s], tile_bytes);
-        for (int r0 = 0; r0 < NR; r0 += xbox_rows) tma_load_2d(dst + (size_t)r0 * W, &tm_x, k0, r0, &full[s]);
-        tma_load_2d(dst + (size_t)NR * W, &tm_c, k0, 0, &full[s]);
-    };
-
-    if (tid == 0) {
-        for (int s = 0; s < NS; ++s) mbar_init(&full[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        for (int i = 0; i < NS && i < my_tiles; ++i) issue(i);
-    }
-    for (int r = tid; r < NR; r += NT) {
-        float acc = 0.f;
-        if (simple) {
-            const int t = r / nu, i = r % nu;
-            for (int j = 0; j < nu; ++j) acc += p.sigma_inv[i * nu + j] * U[t * nu + j];
-            acc *= p.lambda_;
-        }
-        g[r] = acc;
-    }
-    for (int t = tid; t < T; t += NT) gp[t] = powf(p.gamma, (float)t);
-    __syncthreads();
-
-    float b_run = INFINITY, e_run = 0.f, w_run[RPT];
-#pragma unroll
-    for (int i = 0; i < RPT; ++i) w_run[i] = 0.f;
-
-    for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % NS;
-        const int k0 = ((int)blockIdx.x + i * (int)gridDim.x) * W;
-        const float* xs = tiles + (size_t)s * stage_floats;       // [NR][W]
-        const float* cs = xs + (size_t)NR * W;                    // [T][W]
-        mbar_wait(&full[s], (uint32_t)((i / NS) & 1));
-        // ---- S_k partial sums: warp w takes rows r = w, w+8, ...; lane = sample(s)
-        {
-            float acc[KPL];
-#pragma unroll
-            for (int q = 0; q < KPL; ++q) acc[q] = 0.f;
-            for (int t = warp; t < T; t += 8) {
-                const float gt = gp[t];
-#pragma unroll
-                for (int q = 0; q < KPL; ++q) acc[q] += gt * cs[t * W + lane + 32 * q];
-            }
-            if (simple) {
-                for (int r = warp; r < NR; r += 8) {
-                    const float gr = g[r];
-#pragma unroll
-                    for (int q = 0; q < KPL; ++q) acc[q] += gr * xs[r * W + lane + 32 * q];
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < KPL; ++q) red[warp * W + lane + 32 * q] = acc[q];
-        }
-        __syncthreads();
-        if (warp == 0) {
-            float S[KPL], bmin = INFINITY;
-#pragma unroll
-            for (int q = 0; q < KPL; ++q) {
-                const int kk = lane + 32 * q;
-                float sum = 0.f;
-#pragma unroll
-                for (int w8 = 0; w8 < 8; ++w8) sum += red[w8 * W + kk];
-                const bool valid = (k0 + kk < K) && isfinite(sum);
-                S[q] = valid ? sum : INFINITY;
-                bmin = fminf(bmin, S[q]);
-            }
-            bmin = warp_min(bmin);
-            float es = 0.f;
-#pragma unroll
-            for (int q = 0; q < KPL; ++q) {
-                const float w = (S[q] == INFINITY) ? 0.f : expf(-(S[q] - bmin) * inv_lambda);
-                wk[lane + 32 * q] = w;
-                es += w;
-            }
-            es = warp_sum(es);
-            if (lane == 0) { misc[0] = bmin; misc[1] = es; }
-        }
-        __syncthreads();
-        const float b_c = misc[0];
-        if (b_c != INFINITY) {
-            const float e_c = misc[1];
-            const float b_out = fminf(b_run, b_c);
-            const float s_old = (b_run == INFINITY) ? 0.f : expf(-(b_run - b_out) * inv_lambda);
-            const float s_new = expf(-(b_c - b_out) * inv_lambda);
-#pragma unroll
-            for (int rr = 0; rr < RPT; ++rr) {
-                const int r = tid + rr * NT;
-                if (r < NR) {
-                    float acc = 0.f;
-                    const float4* xr = reinterpret_cast<const float4*>(xs + (size_t)r * W);
-                    const float4* w4 = reinterpret_cast<const float4*>(wk);
-#pragma unroll
-                    for (int j = 0; j < W / 4; ++j) {
-                        const int jj = (j + r) & (W / 4 - 1);   // rotation => conflict-free LDS.128
-                        const float4 a = xr[jj], b = w4[jj];
-                        acc += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
-                    }
-                    w_run[rr] = w_run[rr] * s_old + acc * s_new;
-                }
-            }
-            e_run = e_run * s_old + e_c * s_new;
-            b_run = b_out;
-        }
-        __syncthreads();   // every thread is done with ring slot s and with red/wk/misc
-        if (tid == 0 && i + NS < my_tiles) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy reads before async-proxy writes
-            issue(i + NS);
-        }
-    }
-    // ---- per-CTA partial -> scratch ; last CTA folds all of them in parallel
-    const int P = 2 + NR;
-    float* mine = scratch + (size_t)blockIdx.x * (((P + 3) >> 2) << 2);   // rows padded to 16 bytes
-    if (tid == 0) { mine[0] = b_run; mine[1] = e_run; }
-#pragma unroll
-    for (int rr = 0; rr < RPT; ++rr) { const int r = tid + rr * NT; if (r < NR) mine[2 + r] = w_run[rr]; }
-    __threadfence();
-    __syncthreads();
-    __shared__ unsigned int s_last;
-    if (tid == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    fold_and_finish(p, nu, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda);
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // K3, warp-specialised (the default): ONE producer warp streams 32-sample tiles through an NSTAGE-deep ring with TMA, SEVEN
 // consumer warps each own WHOLE tiles end to end -- S_k, minimum, weights, weighted row sums, online merge into the warp's own
 // running (beta, eta, W) in registers -- so nothing inside the streaming loop is CTA-wide: no __syncthreads, the only
-// synchronisation is the full / empty mbarrier pair of a ring stage (the first version above runs three block barriers per
-// tile, and its warps wait on them).
+// synchronisation is the full / empty mbarrier pair of a ring stage.
 //   tile i of this CTA -> ring stage i % NSTAGE, consumer i % NCONS;  full[s]: TMA complete_tx;  empty[s]: the consumer's arrive
 //   per tile and warp: phase A lane = sample (S_k = sum_t gamma^t c[t][k] + sum_r g[r] x[r][k], conflict-free column reads),
 //                      phase B warp shuffles (min, exp, sum), weights to a 32-float per-warp strip,
 //                      phase C lane = row (r = lane, lane + 32, ...: W[r] += sum_k w_k x[r][k], rotated LDS.128, conflict-free)
 // After the loop the seven warp partials are merged once through shared memory; the per-CTA partial, the ticket and the
-// last-CTA fold / exchange / fused K4 are shared with the kernel above (fold_and_finish).
+// last-CTA fold / exchange / fused K4 follow (fold_and_finish).
 constexpr int WS_W = 32;          // samples per tile
 constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
+
+// Shared-memory layout of the kernel with `nstage` ring stages, used by the host for the size and by the kernel for its pointers.
+// Offsets in floats from the base, except `bar` (bytes).  The last CTA reuses the ring for the fold (fold_and_finish), so the ring
+// region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.
+struct WsLayout {
+    int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [NCONS][P4] warp partials | [8]
+    int bar;                      // full[nstage], then empty[nstage] mbarriers
+    int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
+    __host__ __device__ WsLayout(int T, int nu, int nstage) {
+        const int NR = T * nu, P4 = (2 + NR + 3) & ~3;
+        const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
+        g = ring > fold_floats ? ring : fold_floats;
+        gp = g + ((NR + 3) & ~3);
+        wk = gp + ((T + 3) & ~3);
+        cpart = wk + 8 * WS_W;
+        misc = cpart + WS_NCONS * P4;
+        bar = ((misc + 8) * 4 + 15) & ~15;
+        bytes = bar + 2 * 8 * nstage + 128;
+    }
+};
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -386,14 +249,15 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const int P = 2 + NR;
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
-    float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
-    float* g = tiles + (size_t)nstage * tile_floats;                          // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded
-    float* gp = g + NR4;                                                      // [T4]  gamma^t, zero padded
-    float* wk = gp + T4;                                                      // [8][32] weights of the tile a warp is working on
-    float* cpart = wk + 8 * WS_W;                                             // [NCONS][P4] warp partials (after the loop)
-    float* misc = cpart + WS_NCONS * P4;                                      // [8]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + (((size_t)((misc + 8) - tiles) * 4 + 15) & ~(size_t)15));   // [nstage]
+    const WsLayout L(T, nu, nstage);
+    float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
+    float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded
+    float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
+    float* wk = tiles + L.wk;                                                 // [8][32] weights of the tile a warp is working on
+    float* cpart = tiles + L.cpart;                                           // [NCONS][P4] warp partials (after the loop)
+    float* misc = tiles + L.misc;                                             // [8]
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + L.bar);           // [nstage]
     uint64_t* empty = full + nstage;                                          // [nstage]
 
     const int ntiles = (K + WS_W - 1) / WS_W;
@@ -592,16 +456,6 @@ __global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu
     if (threadIdx.x == 0 && plan_ctr) *plan_ctr += 1u;
 }
 
-template <int W, int NS>
-size_t reduce_smem_bytes(int T, int nu) {
-    const int NR = T * nu;
-    const size_t stage = ((size_t)(NR + T) * W + 31) & ~(size_t)31;
-    size_t ring = (size_t)NS * stage;
-    const size_t fold = MAX_GRID + 4 * (size_t)(2 + NR + 3);  // the last CTA reuses the ring for the fold
-    if (ring < fold) ring = (fold + 31) & ~(size_t)31;
-    return sizeof(float) * (ring + (NR + 3) + (T + 3) + 8 * W + W + 8) + 16 + sizeof(uint64_t) * NS + 128;
-}
-
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -640,47 +494,9 @@ static PeerArgs reduce_peers(const MppibContext* c) {
     return a;
 }
 
-template <int W, int NS, int MINB = 1>
-int launch_reduce_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
-                    float* fin_stats, cudaStream_t s) {
-    const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
-    const size_t smem = reduce_smem_bytes<W, NS>(T, nu);
-    MPPIB_REQUIRE(smem <= 226 * 1024, "mppib_reduce: ring of %zu bytes exceeds shared memory", smem);
-    static size_t smem_attr[64] = {0};              // per device: the attribute belongs to the function on ONE device
-    size_t& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_kernel<W, NS, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
-    }
-    // a TMA box has at most 256 rows: split the T*nu rows into equal boxes (largest divisor of T*nu that fits)
-    int xbox_rows = NR < 256 ? NR : 256;
-    while (NR % xbox_rows != 0) --xbox_rows;
-    CUtensorMap tm_x, tm_c;
-    if (int rc = make_map(&tm_x, x, NR, K, xbox_rows, W)) return rc;
-    if (int rc = make_map(&tm_c, cost, T, K, T, W)) return rc;
-    const int ntiles = (K + W - 1) / W;
-    int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
-    if (const char* e = getenv("MPPIB_K3_GRID")) { const int g = atoi(e); if (g >= 1 && g <= ntiles) grid = g; }   // tuning knob (tools/tune_reduce.py)
-    if (grid > MAX_GRID) grid = MAX_GRID;
-    MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
-    mppib_reduce_kernel<W, NS, MINB><<<grid, NT, smem, s>>>(c->params, tm_x, tm_c, nu, xbox_rows, U, c->reduce_scratch, c->reduce_ticket, partial, reduce_peers(c), fin_U, fin_action,
-                                                       fin_stats, fin_U ? c->action_mirror : nullptr);
-    MPPIB_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-
-// shared memory of the warp-specialised kernel with `nstage` ring stages
-static size_t reduce_ws_smem_bytes(int T, int nu, int nstage) {
-    const int NR = T * nu, P4 = (2 + NR + 3) & ~3;
-    size_t fl = (size_t)nstage * (size_t)(NR + T) * WS_W + ((NR + 3) & ~3) + ((T + 3) & ~3) + 8 * WS_W + (size_t)WS_NCONS * P4 + 8;
-    const size_t fold = MAX_GRID + 4 * (size_t)(2 + NR + 3) + 64;            // the last CTA reuses the ring for the fold
-    if ((size_t)nstage * (size_t)(NR + T) * WS_W < fold) fl += fold;
-    return sizeof(float) * fl + 16 + sizeof(uint64_t) * 2 * nstage + 128;
-}
 static int reduce_ws_stages(int T, int nu) {
     int ns = 8;
-    while (ns > 1 && reduce_ws_smem_bytes(T, nu, ns) > 224 * 1024) --ns;
+    while (ns > 1 && WsLayout(T, nu, ns).bytes > 224 * 1024) --ns;
     return ns;
 }
 
@@ -693,7 +509,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     const int nstage_max = reduce_ws_stages(T, nu);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = reduce_ws_smem_bytes(T, nu, nstage);
+    const size_t smem = WsLayout(T, nu, nstage).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
@@ -726,27 +542,13 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
                   float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(c->params.K >= 4 && c->params.K % 4 == 0, "mppib_reduce: K=%d must be a positive multiple of 4 (16-byte rows for TMA / 128-bit loads)", c->params.K);
-    MPPIB_REQUIRE(T * nu <= RPT * NT, "mppib_reduce: T*nu = %d exceeds %d", T * nu, RPT * NT);
+    MPPIB_REQUIRE(T * nu <= 32 * 16, "mppib_reduce: T*nu = %d exceeds %d", T * nu, 32 * 16);
     MPPIB_REQUIRE(T <= 256, "mppib_reduce: T = %d exceeds the 256-row TMA box", T);
-    // default: the warp-specialised kernel (two ring stages at least); MPPIB_K3_VARIANT=64x3|64x1|32x4|32x2 selects the block-synchronous one
-    if (c->k3_variant == 0 && reduce_ws_stages(T, nu) >= 2) {
-        const int NR = T * nu;
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    }
-    // wide tiles once every SM has one; narrow tiles keep all SMs busy at small K
-    bool wide = c->params.K >= 64 * c->num_sms && reduce_smem_bytes<64, 3>(T, nu) <= 226 * 1024;   // A/B: tools/tune_reduce.py
-    if (const char* e = getenv("MPPIB_K3_WIDE")) wide = atoi(e) != 0 && reduce_smem_bytes<64, 3>(T, nu) <= 226 * 1024;   // tuning knob
-    if (const char* e = getenv("MPPIB_K3_VARIANT")) {          // tuning knob: "64x3" | "64x1" | "32x4" | "32x2"
-        if (!strcmp(e, "64x1")) return launch_reduce_t<64, 1, 2>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (!strcmp(e, "32x2")) return launch_reduce_t<32, 2, 2>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (!strcmp(e, "32x4")) return launch_reduce_t<32, 4>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (!strcmp(e, "64x3")) return launch_reduce_t<64, 3>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    }
-    if (wide) return launch_reduce_t<64, 3>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    if (reduce_smem_bytes<32, 4>(T, nu) <= 226 * 1024) return launch_reduce_t<32, 4>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    return launch_reduce_t<32, 2>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    MPPIB_REQUIRE(reduce_ws_stages(T, nu) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
+    const int NR = T * nu;
+    if (NR <= 32 * 4) return launch_reduce_ws_t<4>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    if (NR <= 32 * 8) return launch_reduce_ws_t<8>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    return launch_reduce_ws_t<16>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
 }
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {

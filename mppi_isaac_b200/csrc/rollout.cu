@@ -30,23 +30,6 @@
 // After the last substep of a model step the observed rows are written to obs[R][T][K].
 #include "common.cuh"
 
-// tuning knobs (A/B builds: tools/tune_rollout.py)
-#ifndef ROLL_UNROLL_S1
-#define ROLL_UNROLL_S1 1      // unroll factor of sweep 1 (kinematics / inertia: bodies are independent apart from the frame recursion)
-#endif
-#ifndef ROLL_S1_PIPE
-#define ROLL_S1_PIPE 0        // software-pipelined sweep 1 for serial chains (kinematics of body i+1 with the dynamics terms of body i)
-#endif
-#ifndef ROLL_UNROLL_S2
-#define ROLL_UNROLL_S2 1      // unroll factor of sweep 2 (articulated inertias)
-#endif
-#ifndef ROLL_UNROLL_S3
-#define ROLL_UNROLL_S3 2      // unroll factor of sweep 3 (accelerations)
-#endif
-#define MPPIB_STR2(x) #x
-#define MPPIB_STR(x) MPPIB_STR2(x)
-#define MPPIB_UNROLL(n) _Pragma(MPPIB_STR(unroll n))
-
 #include "rbd_math.cuh"
 
 namespace {
@@ -360,44 +343,7 @@ mppib_rollout_kernel(const __grid_constant__ MppibModel m, const __grid_constant
             {
                 const bool obs_now = sub == 0 && pending >= 0;   // this sweep's kinematics ARE the observation of the previous step
                 Frame par = base; Quat qp = bq;
-#if ROLL_S1_PIPE
-                if (CHAIN && !CONTACT) {
-                    // software-pipelined: the kinematics of body i+1 (the frame recursion) and the inertia / bias terms of body i are
-                    // independent and sit in ONE basic block, so the scheduler can interleave them (the last iteration recomputes
-                    // the kinematics of body nb-1, discarded)
-                    auto head = [&](int j, const Frame& pf, Frame& f, V6& S, float& qdj) {
-                        const float qj = SM(j, F_Q);
-                        qdj = SM(j, F_QD);
-                        body_kinematics(m, j, qj, qdj, pf, f, S);
-                        return qj;
-                    };
-                    auto obs_head = [&](int j, float qj, const Frame& f) {
-                        const Quat qt = {m.tree_quat[j][0], m.tree_quat[j][1], m.tree_quat[j][2], m.tree_quat[j][3]};
-                        Quat r = qmul(qp, qt);
-                        if (m.jtype[j] == MPPIB_JOINT_REVOLUTE) {
-                            float sh, ch; sincos_cw(0.5f * qj, &sh, &ch);
-                            const Quat qz = {0.f, 0.f, sh, ch};
-                            r = qmul(r, qz);
-                        }
-                        stM3(sm, j * NSLOT + F_OR, lane, f.R); st3(sm, j * NSLOT + F_OO, lane, f.o); st6(sm, j * NSLOT + F_OV, lane, f.V);
-                        SM(j, F_OQ) = r.x; SM(j, F_OQ + 1) = r.y; SM(j, F_OQ + 2) = r.z; SM(j, F_OQ + 3) = r.w;
-                        qp = r;
-                    };
-                    Frame fc; V6 Sc; float qdc;
-                    { const float q0 = head(0, base, fc, Sc, qdc); if (obs_now) obs_head(0, q0, fc); }
 #pragma unroll 1
-                    for (int i = 0; i < nb; ++i) {
-                        const int j = i + 1 < nb ? i + 1 : nb - 1;
-                        Frame fn; V6 Sn; float qdn;
-                        const float qj = head(j, fc, fn, Sn, qdn);
-                        s1_dynamics<NSLOT>(m, sm, lane, i, fc, Sc, qdc);
-                        SM(i, F_SAT) = 0.f;
-                        if (obs_now && i + 1 < nb) obs_head(j, qj, fn);
-                        fc = fn; Sc = Sn; qdc = qdn;
-                    }
-                } else
-#endif
-                MPPIB_UNROLL(ROLL_UNROLL_S1)
                 for (int i = 0; i < nb; ++i) {
                     if (!CHAIN) {
                         const int pi = m.parent[i];
@@ -440,7 +386,7 @@ mppib_rollout_kernel(const __grid_constant__ MppibModel m, const __grid_constant
                 }
                 SpI Ic; V6 pc;   // contribution of the child (serial chains)
                 bool have_child = false;
-                MPPIB_UNROLL(ROLL_UNROLL_S2)
+#pragma unroll 1
                 for (int i = nb - 1; i >= 0; --i) {
                     const V6 S = ld6(sm, i * NSLOT + F_S, lane);
                     SpI IA; V6 pA;
@@ -485,7 +431,7 @@ mppib_rollout_kernel(const __grid_constant__ MppibModel m, const __grid_constant
                 // -------------------------------------------------------------- sweep 3: root -> leaves
                 V6 ap = a0;
                 bool any = false;
-                MPPIB_UNROLL(ROLL_UNROLL_S3)
+#pragma unroll 2
                 for (int i = 0; i < nb; ++i) {
                     if (!CHAIN) { const int pi = m.parent[i]; ap = pi >= 0 ? ld6(sm, pi * NSLOT + F_ACC, lane) : a0; }
                     const V6 S = ld6(sm, i * NSLOT + F_S, lane), c = ld6(sm, i * NSLOT + F_C, lane), U = ld6(sm, i * NSLOT + F_U, lane);
@@ -571,14 +517,12 @@ int launch_t(MppibContext* c, const float* state0, const float* root0, float* st
 // can take (trees of up to 16 bodies in depth-first order, with or without contacts): a team of lanes per rollout (rollout_team.cu),
 // which spreads a rollout over many lanes where this kernel gives it one thread.  The choice does not depend on K, so a shard of a
 // multi-GPU job runs the same arithmetic as the single-GPU job (bit-identical rollouts, tests/test_gpu_sizes.py).  The
-// thread-per-rollout kernel below remains for scenes the team kernel does not take and as the A/B reference:
-// MPPIB_K2_LANES=0 / MPPIB_K2_TEAM=0|1 force a mapping.
+// thread-per-rollout kernel below remains for scenes the team kernel does not take and as the reference of the other two:
+// MPPIB_K2_LANES=0 / MPPIB_K2_TEAM=0 switch the lanes / team mapping off.
 int rollout_mapping(const MppibContext* c) {
     const MppibModel& m = c->model;
     if (c->k2_lanes && rollout_lanes_eligible(m)) return MPPIB_MAPPING_LANES;
-    if (c->k2_team != 0 && rollout_team_eligible(m)) {
-        return MPPIB_MAPPING_TEAM;
-    }
+    if (c->k2_team && rollout_team_eligible(m)) return MPPIB_MAPPING_TEAM;
     return MPPIB_MAPPING_THREAD;
 }
 

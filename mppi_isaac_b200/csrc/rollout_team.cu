@@ -25,13 +25,8 @@
 namespace {
 
 using namespace lm;
-typedef V3T<float> V3;
-typedef M3T<float> M3;
-typedef S3T<float> S3;
-typedef QT<float> Quat;
-typedef V6T<float> V6;
 
-__device__ __forceinline__ V3 mk(float x, float y, float z) { return mk3<float>(x, y, z); }
+__device__ __forceinline__ V3 mk(float x, float y, float z) { return mk3(x, y, z); }
 __device__ __forceinline__ float dot6(const V6& a, const V6& b) { return dot(a.n, b.n) + dot(a.f, b.f); }
 __device__ __forceinline__ V3 mulM(const M3& m, V3 v) { return mulc(m, v.x, v.y, v.z); }
 __device__ __forceinline__ V3 mulMT(const M3& m, V3 v) {

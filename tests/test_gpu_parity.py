@@ -420,13 +420,24 @@ def test_halton_spline_plan_through_planner_api():
     assert gpu.mppi._graph is not None
 
 
-@pytest.mark.parametrize("setup,T", [(point_setup, 12), (point_setup, 25), (point_setup, 9), (gripper_setup, 30), (gripper_setup, 11), (gripper_setup, 29)])
+def point_nu1_setup(K, T):
+    """The point robot driven through one input: both command maps point at input 0 (nu = 1)."""
+    sc, p, state0 = point_setup(K=K, T=T)
+    sc.model.nu = 1
+    for i in range(sc.model.nb):
+        sc.model.cmd_i0[i] = sc.model.cmd_i1[i] = 0
+    return sc, p, state0
+
+
+@pytest.mark.parametrize("setup,T", [(point_setup, 12), (point_setup, 25), (point_setup, 9), (gripper_setup, 30), (gripper_setup, 11), (gripper_setup, 29),
+                                     (point_nu1_setup, 1)])
 def test_k3_shapes_and_alignment(oracle, setup, T):
-    """K3 across (T, nu) shapes: T*nu = 27..270 rows, odd row counts, two TMA boxes for T*nu > 256 (270 = 2 x 135) and three for 261 = 3 x 87."""
+    """K3 across (T, nu) shapes: T*nu = 27..270 rows, odd row counts, two TMA boxes for T*nu > 256 (270 = 2 x 135) and three for 261 = 3 x 87;
+    T = nu = 1, where the last CTA's fold needs more shared memory than the ring stages hold."""
     K = 1000
     sc, p, _ = setup(K=K, T=T) if setup is not gripper_setup else setup(K=K, T=T, filter_u=False)
     p.filter_u = 0
-    nu = sc.nu
+    nu = sc.model.nu
     be = gpu_backend(sc, p)
     rng = np.random.default_rng(T)
     U = rng.uniform(-0.1, 0.1, (T, nu)).astype(np.float32)

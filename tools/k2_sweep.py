@@ -21,13 +21,9 @@ from mppi_isaac_b200.objectives import PandaReachObjective  # noqa: E402
 KS = [int(a) for a in sys.argv[1:]] or [1252, 2500, 5000, 10000, 20000, 40000, 65536, 131072]
 
 
-def time_rollout(K, lanes, pairs=None):
+def time_rollout(K, lanes):
     os.environ["MPPIB_K2_LANES"] = "1" if lanes else "0"      # read by mppib_create
     os.environ["MPPIB_K2_TEAM"] = "0"                         # (a chain is also a tree: without this the team kernel would take it)
-    if pairs is None:
-        os.environ.pop("MPPIB_K2_PAIRS", None)
-    else:
-        os.environ["MPPIB_K2_PAIRS"] = "1" if pairs else "0"
     planner = MPPIisaacPlanner(bench.panda_cfg(K, "cuda:0"), PandaReachObjective(), use_cuda_graph=False)
     q0, goal = bench.synthetic_state()
     planner.sim.set_actor_position_by_name(goal, "goal")
@@ -41,17 +37,15 @@ def time_rollout(K, lanes, pairs=None):
 
 
 rows = []
-print("| K | lanes, 1 rollout / group (us) | lanes, 2 rollouts / group, packed f32x2 (us) | thread-per-rollout (us) | best lanes vs thread | rollout-steps/s (best) | max abs obs diff (1 vs thread, 2 vs thread) |")
-print("|---|---|---|---|---|---|---|")
+print("| K | lanes (us) | thread-per-rollout (us) | lanes vs thread | rollout-steps/s (lanes) | max abs obs diff |")
+print("|---|---|---|---|---|---|")
 for K in KS:
     K = (K // 4) * 4
-    a, oa = time_rollout(K, True, False)
-    a2, oa2 = time_rollout(K, True, True)
+    a, oa = time_rollout(K, True)
     b, ob = time_rollout(K, False)
-    diff, diff2 = float((oa - ob).abs().max()), float((oa2 - ob).abs().max())
-    best = min(a, a2)
-    rows.append({"K": K, "lanes_us": a, "lanes_packed_us": a2, "thread_us": b, "max_abs_obs_diff": diff, "max_abs_obs_diff_packed": diff2})
-    print(f"| {K} | {a:.1f} | {a2:.1f} | {b:.1f} | {b / best:.2f}x | {K * 30 / (best * 1e-6):.3e} | {diff:.2e}, {diff2:.2e} |", flush=True)
+    diff = float((oa - ob).abs().max())
+    rows.append({"K": K, "lanes_us": a, "thread_us": b, "max_abs_obs_diff": diff})
+    print(f"| {K} | {a:.1f} | {b:.1f} | {b / a:.2f}x | {K * 30 / (a * 1e-6):.3e} | {diff:.2e} |", flush=True)
     torch.cuda.empty_cache()
 print()
 print(json.dumps(rows))

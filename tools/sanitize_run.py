@@ -2,7 +2,7 @@
 """Small, complete pass over every kernel of libmppib.so for compute-sanitizer (tools/sanitize.sh): K1 (Gaussian and Halton-spline
 library), K2 (lanes-per-rollout chain kernel, team kernel on contact scenes of small and large robots, thread-per-rollout chain / tree /
 contact kernels), fused cost, K3 (warp-specialised
-ring, ragged last tile, and the block-synchronous variant), K4, shift, and whole plans (eager and CUDA-graph replay).  Sizes are
+ring, ragged last tile), K4, shift, and whole plans (eager and CUDA-graph replay).  Sizes are
 small: the sanitizer serialises the GPU.  With WORLD_SIZE > 1 (torchrun) the plans also run the peer-memory exchange."""
 import os
 import sys
@@ -45,9 +45,6 @@ for name, mk, obj, q in CASES:
     if rank == 0:
         print("ok:", name, flush=True)
 if world == 1:
-    os.environ["MPPIB_K3_VARIANT"] = "auto"           # the block-synchronous K3 (read by mppib_create)
-    pl = MPPIisaacPlanner(panda_cfg(K=4100, T=30, device=dev), PandaReachObjective(), use_cuda_graph=False)
-    pl.compute_action([0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0], [0.0] * 7)
     os.environ["MPPIB_K2_LANES"] = "0"                # a serial chain on the contact-free TEAM kernel (a chain is a tree)
     pl = MPPIisaacPlanner(panda_cfg(K=512, T=10, device=dev), PandaReachObjective(), use_cuda_graph=False)
     pl.compute_action([0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0], [0.0] * 7)
@@ -61,7 +58,7 @@ if world == 1:
         pl.compute_action(q, [0.0] * len(q))
         del pl
     del os.environ["MPPIB_K2_TEAM"]
-    print("ok: block-synchronous K3, thread-per-rollout chain / contact K2", flush=True)
+    print("ok: team and thread-per-rollout chain K2, thread-per-rollout contact K2", flush=True)
 torch.cuda.synchronize()
 if world > 1:
     dist.barrier()
