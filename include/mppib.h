@@ -32,7 +32,9 @@
  *                               rows 0..ndof-1 = q, ndof..2ndof-1 = qdot, then free bodies
  *   obs      [R][T][K]          observed rows per step, R = mppib_obs_size()
  *   cost     [T][K]             per-step running cost from Objective.compute_cost
- *   partial  [2 + T*nu]         (beta_g, eta_g, W_g[T][nu]) of one shard
+ *   partial  [2 + T*nu]         (beta_g, eta_g, W_g[T][nu]) of one shard;
+ *            [2 + 2*T*nu]       (beta_g, eta_g, W_g, M2_g[T][nu]) with update_cov and a registered distribution
+ *   dist     [1 + nu]           (lambda, cov[nu]) live sampling distribution of adaptive MPPI (mppib_set_distribution)
  */
 #ifndef MPPIB_H
 #define MPPIB_H
@@ -43,7 +45,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 13
+#define MPPIB_ABI_VERSION 14
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -191,6 +193,15 @@ typedef struct MppibParams {
     uint32_t rand_seed;        /* seed of the per-rollout size / mass / friction draws              */
     int32_t nobs;
     MppibObsItem obs[MPPIB_MAX_OBS];
+    /* adaptive MPPI (mppi_torch update_cov / update_lambda): they act only once a distribution buffer is registered
+       (mppib_set_distribution); lambda_ above is then the initial temperature lambda0 and the clamp centre             */
+    int32_t update_cov;        /* K1 draws sqrt(cov) z, K3 adds the second-moment row, K4 updates cov (diagonal Sigma)  */
+    int32_t update_lambda;     /* K4 adapts lambda to the weight sum eta                                               */
+    float   eta_u_bound;       /* eta > bound: lambda *= 1 - lambda_mult                                                */
+    float   eta_l_bound;       /* eta < bound: lambda *= 1 + lambda_mult; lambda stays in [1e-3, 1e3] * lambda0      */
+    float   step_size_cov;     /* cov <- (1 - s) cov + s mean_t var_t + kappa                                          */
+    float   kappa;
+    float   lambda_mult;
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -240,6 +251,8 @@ int32_t mppib_rollout(MppibHandle h, const float* state0, const float* root0, fl
 /* K3: S_k = sum_t gamma^t cost[t][k] (+ lambda sum_t U_t^T Sigma^-1 noise_k,t in SIMPLE mode),
  * beta_g = min_k S_k, w_k = exp(-(S_k - beta_g)/lambda), eta_g = sum w_k,
  * W_g[t][j] = sum_k w_k x[t][j][k] with x = noise (SIMPLE) or actions (MEAN).
+ * With a registered distribution lambda (and, with update_cov, Sigma^-1 = diag(1/cov)) come from it, and update_cov appends
+ * M2_g[t][j] = sum_k w_k (x[t][j][k] - c[t][j])^2, c = U (MEAN) or 0 (SIMPLE).
  * Single pass over HBM; the last CTA to finish folds the per-CTA partials.                  */
 int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const float* U,
                      float* partial, void* stream);
@@ -306,6 +319,14 @@ int32_t mppib_rollout_mapping_for_model(const MppibModel* model_h);
  * PINNED host memory (device-addressable under unified addressing), so the caller of the reference's compute_action* only
  * waits for the stream instead of issuing a device->host copy.  NULL switches it off.                                      */
 int32_t mppib_set_action_mirror(MppibHandle h, float* mirror);
+
+/* Adaptive MPPI: register the device buffer dist[1 + nu] = (lambda, cov[nu]) (float32, caller-owned, initialised by the caller).
+ * Once set, K1 draws noise_j = sqrt(cov_j) z_j (update_cov; mppib_noise_library then builds a WHITE library that
+ * mppib_sample_library scales per plan), K3 weights with the buffer's lambda (and diag(1/cov)), and K4 updates the buffer in
+ * place after the U update: cov (update_cov, needs the [2 + 2*T*nu] partial rows) and lambda (update_lambda); dist is left
+ * as it is when no sample is valid.  Because the buffer lives in device memory, a captured plan graph follows it.  NULL
+ * switches it off: every launch then runs the fixed-distribution kernels.                                                   */
+int32_t mppib_set_distribution(MppibHandle h, float* dist);
 
 /* shift U by one step: U[t] <- U[t+1], U[T-1] <- u_init (mppi_torch command() prologue);
  * increments *plan_ctr (device, nullable) by one.                                            */

@@ -24,6 +24,7 @@ SYMBOLS = [
     "mppib_set_model", "mppib_state_size", "mppib_obs_size", "mppib_sample", "mppib_rollout",
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
+    "mppib_set_distribution",
 ]
 
 
@@ -82,6 +83,7 @@ class CudaBackend:
         self.model = None
         self.params = None
         self._mirror_keepalive = None
+        self._dist_keepalive = None
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -97,6 +99,8 @@ class CudaBackend:
         self._finalizer = weakref.finalize(self, _destroy_handle, self.lib, self.handle.value)   # also runs at interpreter exit
         if self._mirror_keepalive is not None:           # a re-created handle keeps writing the action to the same pinned mirror
             self.set_action_mirror(self._mirror_keepalive)
+        if self._dist_keepalive is not None:             # ... and keeps following the planner's adaptive distribution
+            self.set_distribution(self._dist_keepalive)
 
     def destroy(self):
         if self.handle:
@@ -172,6 +176,11 @@ class CudaBackend:
         """K4 also stores the action into this PINNED host tensor (None switches it off)."""
         self._mirror_keepalive = pinned_host_tensor
         self._check(self.lib.mppib_set_action_mirror(self.handle, _ptr(pinned_host_tensor)), "mppib_set_action_mirror")
+
+    def set_distribution(self, dist):
+        """Adaptive MPPI: register the device tensor (lambda, cov[nu]) that K1 / K3 read and K4 updates (None switches it off)."""
+        self._dist_keepalive = dist
+        self._check(self.lib.mppib_set_distribution(self.handle, _ptr(dist)), "mppib_set_distribution")
 
     def reduce(self, cost, x, U, partial):
         self.launches += 1

@@ -39,6 +39,9 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     MPPIB_REQUIRE(p->lambda_ > 0.f, "lambda must be positive");
     MPPIB_REQUIRE(!(p->filter_u && p->T < 9), "filter_u needs T >= 9");
     MPPIB_REQUIRE(p->nobs >= 0 && p->nobs <= MPPIB_MAX_OBS, "nobs out of range");
+    if (p->update_cov || p->update_lambda)
+        MPPIB_REQUIRE(p->step_size_cov >= 0.f && p->step_size_cov <= 1.f && p->kappa >= 0.f && p->lambda_mult >= 0.f && p->lambda_mult < 1.f,
+                      "adaptive MPPI: step_size_cov %g, kappa %g or lambda_mult %g out of range", p->step_size_cov, p->kappa, p->lambda_mult);
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -59,7 +62,7 @@ static void derive(MppibContext* c) {
 static int alloc_scratch(MppibContext* c) {
     if (c->reduce_scratch) { cudaFree(c->reduce_scratch); c->reduce_scratch = nullptr; }
     c->reduce_max_ctas = c->num_sms * 4;
-    const size_t P = (2 + (size_t)c->params.T * c->model.nu + 3) & ~(size_t)3;   // rows padded to 16 bytes
+    const size_t P = ((size_t)partial_row_capacity(c->params, c->model.nu) + 3) & ~(size_t)3;   // rows padded to 16 bytes
     MPPIB_CHECK_CUDA(cudaMalloc(&c->reduce_scratch, sizeof(float) * P * c->reduce_max_ctas));
     if (!c->reduce_ticket) {
         MPPIB_CHECK_CUDA(cudaMalloc(&c->reduce_ticket, sizeof(unsigned int)));
@@ -128,7 +131,7 @@ int32_t mppib_peer_alloc(MppibHandle h, int32_t world, int32_t rank, unsigned ch
     static_assert(sizeof(cudaIpcMemHandle_t) == MPPIB_IPC_HANDLE_BYTES, "IPC handle size");
     mppib_peer_close(h);
     MPPIB_ON_DEVICE(h);
-    const int P = 2 + h->params.T * h->model.nu;
+    const int P = partial_row_capacity(h->params, h->model.nu);
     const int pcap = ((P + 3) >> 2) << 2;
     void* win = nullptr;
     MPPIB_CHECK_CUDA(cudaMalloc(&win, peer_window_bytes(world, pcap)));
@@ -173,8 +176,8 @@ int32_t mppib_destroy(MppibHandle h) {
 int32_t mppib_set_params(MppibHandle h, const MppibParams* params_h) {
     MPPIB_REQUIRE(h != nullptr, "null handle");
     if (int rc = validate(&h->model, params_h)) return rc;
-    const bool resize = params_h->T != h->params.T;
-    MPPIB_REQUIRE(h->peer_world <= 1 || 2 + params_h->T * h->model.nu <= h->peer_pcap, "mppib_set_params: T*nu outgrows the open peer window; close and re-open the peers");
+    const bool resize = partial_row_capacity(*params_h, h->model.nu) != partial_row_capacity(h->params, h->model.nu);
+    MPPIB_REQUIRE(h->peer_world <= 1 || partial_row_capacity(*params_h, h->model.nu) <= h->peer_pcap, "mppib_set_params: T*nu outgrows the open peer window; close and re-open the peers");
     h->params = *params_h;
     derive(h);
     if (resize) { MPPIB_ON_DEVICE(h); return alloc_scratch(h); }
@@ -185,7 +188,7 @@ int32_t mppib_set_model(MppibHandle h, const MppibModel* model_h) {
     MPPIB_REQUIRE(h != nullptr, "null handle");
     if (int rc = validate(model_h, &h->params)) return rc;
     const bool resize = model_h->nu != h->model.nu;
-    MPPIB_REQUIRE(h->peer_world <= 1 || 2 + h->params.T * model_h->nu <= h->peer_pcap, "mppib_set_model: T*nu outgrows the open peer window; close and re-open the peers");
+    MPPIB_REQUIRE(h->peer_world <= 1 || partial_row_capacity(h->params, model_h->nu) <= h->peer_pcap, "mppib_set_model: T*nu outgrows the open peer window; close and re-open the peers");
     h->model = *model_h;
     derive(h);
     if (resize) { MPPIB_ON_DEVICE(h); return alloc_scratch(h); }
@@ -276,6 +279,12 @@ int64_t mppib_rollout_smem_bytes(const MppibModel* model_h) {
 int32_t mppib_set_action_mirror(MppibHandle h, float* mirror) {
     MPPIB_REQUIRE(h != nullptr, "null handle");
     h->action_mirror = mirror;
+    return 0;
+}
+
+int32_t mppib_set_distribution(MppibHandle h, float* dist) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    h->dist = dist;
     return 0;
 }
 

@@ -37,14 +37,15 @@ struct MppibContext {
     int state_rows;          // NS
     int num_sms;
     // K3 scratch: per-CTA partials + ticket counter (device memory owned by the handle)
-    float* reduce_scratch;   // [max_ctas][2 + T*nu]
+    float* reduce_scratch;   // [max_ctas][partial_row_floats(), padded to 4]
     unsigned int* reduce_ticket;
     int reduce_max_ctas;
     // peer window (multi-GPU exchange over NVLink peer memory), see include/mppib.h
-    int peer_world, peer_rank, peer_pcap;      // pcap: floats per row (>= 2 + T*nu, multiple of 4)
+    int peer_world, peer_rank, peer_pcap;      // pcap: floats per row (>= partial_row_floats(), multiple of 4)
     void* peer_win[MPPIB_MAX_PEERS];           // window base of every rank (own entry = local allocation)
     unsigned long long peer_timeout_ns;
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
+    float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) read by K1 / K3, updated by K4 (nullable)
     // K2 mappings the handle may use (rollout_mapping() picks by scene, never by K); both default to true
     bool k2_team;                              // a team of lanes per rollout for trees / contact scenes (rollout_team.cu); MPPIB_K2_TEAM=0 turns it off
     bool k2_lanes;                             // one body per lane for serial chains (rollout_lanes.cu); MPPIB_K2_LANES=0 turns it off
@@ -67,6 +68,11 @@ struct DeviceGuard {
 #define MPPIB_ON_DEVICE(h)                                                                   \
     DeviceGuard _guard((h)->device);                                                        \
     MPPIB_CHECK_CUDA(_guard.err)
+
+// Floats of one shard row (beta, eta, W[T*nu] and, with update_cov, M2[T*nu]).  Buffers are sized by the flag alone, so that
+// registering a distribution never needs a reallocation; the kernels append M2 only when a distribution is registered too.
+static inline int partial_row_capacity(const MppibParams& p, int nu) { return 2 + p.T * nu * (p.update_cov ? 2 : 1); }
+static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 
 // device view of the peer windows, passed by value to K3 / K4
 struct PeerArgs {

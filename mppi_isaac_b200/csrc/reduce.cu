@@ -65,12 +65,24 @@ __constant__ float c_sg_edge[4][9] = {{763.f, 441.f, 189.f, 7.f, -105.f, -147.f,
                                       {7.f, 136.5f, 223.5f, 268.f, 270.f, 229.5f, 146.5f, 21.f, -147.f}};
 
 // combine G rows (beta_g, eta_g, W_g) of stride P, update U (+ Savitzky-Golay, clamp), first action, statistics; one CTA of 256
-// threads, `un` = [T*nu + G] floats of shared memory
+// threads, `un` = [T*nu + G] floats of shared memory (+ T*nu with update_cov).
+// ADAPT (a distribution is registered): lambda comes from dist[0]; after the U update the CTA updates dist in place --
+//   update_cov:    the rows carry M2_g after W_g; m1 = W/eta - c, m2 = M2/eta, d = U_new - U_old (before Savitzky-Golay),
+//                  var = max(m2 - 2 d m1 + d^2, 0), cov_j <- (1 - s) cov_j + s mean_t var[t][j] + kappa
+//   update_lambda: lambda *= 1 - lambda_mult (eta > eta_u_bound) or 1 + lambda_mult (eta < eta_l_bound), kept in [1e-3, 1e3] lambda0
+// and leaves it as it is when no sample is valid.  The mean over t runs serially in t order on one thread per j, so every rank of a
+// multi-GPU plan, which combines the same rows in the same order, writes bit-identical values.  Every thread reads dist[0] at entry and
+// dist[1 + j] is read and written by thread j only; the writes come after the __syncthreads below, so nothing reads a value written here.
+template <bool ADAPT>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
-                                              float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un) {
+                                              float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
+                                              float* __restrict__ dist) {
     const int T = p.T, NR = T * nu;
     float* sg = un + NR;
-    const float inv_lambda = 1.0f / p.lambda_;
+    const float lam = ADAPT ? dist[0] : p.lambda_;
+    const float inv_lambda = 1.0f / lam;
+    const bool cov = ADAPT && p.update_cov;
+    float* var = sg + G;                                                      // [NR] per-element variance (update_cov)
     float b = INFINITY;
     for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
     for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
@@ -85,6 +97,13 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
         for (int gidx = 0; gidx < G; ++gidx) w += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + r]);
         const float wm = e > 0.f ? w / e : (p.mode == MPPIB_MODE_SIMPLE ? 0.f : U[r]);   // no valid sample: keep U
         un[r] = p.mode == MPPIB_MODE_SIMPLE ? U[r] + wm : (1.0f - p.step_size_mean) * U[r] + p.step_size_mean * wm;
+        if (cov && e > 0.f) {
+            float m2 = 0.f;
+            for (int gidx = 0; gidx < G; ++gidx) m2 += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + NR + r]);
+            const float c0 = p.mode == MPPIB_MODE_SIMPLE ? 0.f : U[r];
+            const float m1 = w / e - c0, d = un[r] - U[r];
+            var[r] = fmaxf(m2 / e - 2.0f * d * m1 + d * d, 0.f);
+        }
     }
     __syncthreads();
     for (int r = threadIdx.x; r < NR; r += blockDim.x) {
@@ -112,16 +131,32 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
         if (r < nu) { action_out[r] = out; if (action_mirror) action_mirror[r] = out; }
     }
     if (threadIdx.x == 0 && stats) { stats[0] = b; stats[1] = e; }
+    if (ADAPT && e > 0.f) {
+        if (cov) {
+            for (int j = threadIdx.x; j < nu; j += blockDim.x) {
+                float acc = 0.f;
+                for (int t = 0; t < T; ++t) acc += var[t * nu + j];
+                dist[1 + j] = (1.0f - p.step_size_cov) * dist[1 + j] + p.step_size_cov * (acc / (float)T) + p.kappa;
+            }
+        }
+        if (p.update_lambda && threadIdx.x == 0) {
+            float l = lam;
+            if (e > p.eta_u_bound) l = lam * (1.0f - p.lambda_mult);
+            else if (e < p.eta_l_bound) l = lam * (1.0f + p.lambda_mult);
+            dist[0] = fminf(fmaxf(l, 1e-3f * p.lambda_), 1e3f * p.lambda_);
+        }
+    }
 }
 
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
 // at least, `misc` = 8 floats.
-__device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
+template <bool ADAPT>
+__device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
-                                                float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda) {
+                                                float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
+                                                float* __restrict__ dist) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int NR = p.T * nu, P = 2 + NR;
     const int G = (int)gridDim.x;
     float* sc = tiles;                   // [MAX_GRID] scale of every CTA partial (the ring is idle now)
     float* fold = tiles + MAX_GRID;      // [4][PP]
@@ -189,10 +224,11 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, fl
         if (tid == 0) *ticket = 0u;
         if (fin_U != nullptr) {
             // single-GPU plans: this CTA is the last one alive and holds the shard row -> do K4's work here (U update, savgol,
-            // first action) instead of launching another kernel.  Every CTA read U in its prologue, long before this point.
+            // first action) instead of launching another kernel.  Every CTA read U -- and, with a registered distribution, lambda and
+            // cov -- in its prologue, before it took its ticket, so this CTA is the only reader left when it updates them.
             __threadfence();
             __syncthreads();
-            finalize_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles);
+            finalize_rows<ADAPT>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
         }
     }
 }
@@ -218,8 +254,8 @@ struct WsLayout {
     int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [NCONS][P4] warp partials | [8]
     int bar;                      // full[nstage], then empty[nstage] mbarriers
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
-    __host__ __device__ WsLayout(int T, int nu, int nstage) {
-        const int NR = T * nu, P4 = (2 + NR + 3) & ~3;
+    __host__ __device__ WsLayout(int T, int nu, int nstage, bool m2 = false) {   // m2: the shard row carries M2 (2 + 2 T*nu floats)
+        const int NR = T * nu, P4 = (2 + NR * (m2 ? 2 : 1) + 3) & ~3;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
         gp = g + ((NR + 3) & ~3);
@@ -235,22 +271,27 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-template <int RPL>   // rows of W per lane: T*nu <= 32 * RPL
+// ADAPT (a distribution is registered): lambda comes from dist[0]; with update_cov the SIMPLE-mode Sigma^-1 is diag(1 / dist[1 + j])
+// and phase C keeps a second running sum per row, M2[r] = sum_k w_k (x[r][k] - c[r])^2 with c = U (MEAN) or 0 (SIMPLE), rescaled
+// online like W; the shard row becomes (beta, eta, W[T*nu], M2[T*nu]).  The bytes read from HBM are the same.
+template <int RPL, bool ADAPT>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
-                       float* __restrict__ fin_stats, float* __restrict__ fin_mirror) {
+                       float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const float inv_lambda = 1.0f / p.lambda_;
+    const float lam = ADAPT ? dist[0] : p.lambda_;
+    const float inv_lambda = 1.0f / lam;
     const bool simple = p.mode == MPPIB_MODE_SIMPLE;
-    const int P = 2 + NR;
+    const bool m2 = ADAPT && p.update_cov;
+    const int P = 2 + (m2 ? 2 : 1) * NR;
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
-    const WsLayout L(T, nu, nstage);
+    const WsLayout L(T, nu, nstage, m2);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -282,8 +323,10 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         float acc = 0.f;
         if (simple && r < NR) {
             const int t = r / nu, i = r % nu;
-            for (int j = 0; j < nu; ++j) acc += p.sigma_inv[i * nu + j] * U[t * nu + j];
-            acc *= p.lambda_;
+            if (m2) acc = (1.0f / dist[1 + i]) * U[r];
+            else
+                for (int j = 0; j < nu; ++j) acc += p.sigma_inv[i * nu + j] * U[t * nu + j];
+            acc *= lam;
         }
         g[r] = acc;
     }
@@ -309,8 +352,17 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         const int c = warp - 1;
         float* wme = wk + warp * WS_W;
         float b_run = INFINITY, e_run = 0.f, w_run[RPL];
+        float m2_run[ADAPT ? RPL : 1], c_row[ADAPT ? RPL : 1];               // second moment and its centre per row (update_cov)
 #pragma unroll
         for (int i = 0; i < RPL; ++i) w_run[i] = 0.f;
+        if (ADAPT) {
+#pragma unroll
+            for (int i = 0; i < RPL; ++i) {
+                const int r = lane + 32 * i;
+                m2_run[i] = 0.f;
+                c_row[i] = (m2 && !simple && r < NR) ? U[r] : 0.f;
+            }
+        }
         for (int i = c; i < my_tiles; i += ncons) {
             const int s = i % nstage;
             const int k0 = ((int)blockIdx.x + i * (int)gridDim.x) * WS_W;
@@ -357,11 +409,25 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                     if (r < NR) {
                         const float4* xr = reinterpret_cast<const float4*>(xs + (size_t)r * WS_W);
                         float acc = 0.f;
+                        if (ADAPT && m2) {
+                            const float cr = c_row[ADAPT ? rr : 0];
+                            float acc2 = 0.f;
 #pragma unroll
-                        for (int j = 0; j < WS_W / 4; ++j) {
-                            const int jj = (j + lane) & (WS_W / 4 - 1);       // rotation => conflict-free LDS.128
-                            const float4 a = xr[jj], b = w4[jj];
-                            acc += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+                            for (int j = 0; j < WS_W / 4; ++j) {
+                                const int jj = (j + lane) & (WS_W / 4 - 1);
+                                const float4 a = xr[jj], b = w4[jj];
+                                acc += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+                                const float dx = a.x - cr, dy = a.y - cr, dz = a.z - cr, dw = a.w - cr;
+                                acc2 += b.x * dx * dx + b.y * dy * dy + b.z * dz * dz + b.w * dw * dw;
+                            }
+                            m2_run[ADAPT ? rr : 0] = m2_run[ADAPT ? rr : 0] * s_old + acc2 * s_new;
+                        } else {
+#pragma unroll
+                            for (int j = 0; j < WS_W / 4; ++j) {
+                                const int jj = (j + lane) & (WS_W / 4 - 1);   // rotation => conflict-free LDS.128
+                                const float4 a = xr[jj], b = w4[jj];
+                                acc += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+                            }
                         }
                         w_run[rr] = w_run[rr] * s_old + acc * s_new;
                     }
@@ -377,11 +443,15 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         if (lane == 0) { mine[0] = b_run; mine[1] = e_run; }
 #pragma unroll
         for (int rr = 0; rr < RPL; ++rr) { const int r = lane + 32 * rr; if (r < NR) mine[2 + r] = w_run[rr]; }
+        if (ADAPT && m2) {
+#pragma unroll
+            for (int rr = 0; rr < RPL; ++rr) { const int r = lane + 32 * rr; if (r < NR) mine[2 + NR + r] = m2_run[ADAPT ? rr : 0]; }
+        }
     } else {
         // spare warp (fewer ring stages than warps): an empty partial
         float* mine = cpart + (size_t)(warp - 1) * P4;
         if (lane == 0) { mine[0] = INFINITY; mine[1] = 0.f; }
-        for (int r = lane; r < NR; r += 32) mine[2 + r] = 0.f;
+        for (int r = lane; r < P - 2; r += 32) mine[2 + r] = 0.f;
     }
     __syncthreads();
     // ---- merge the warp partials into the CTA partial (global scratch), then ticket -> the last CTA folds all of them
@@ -407,17 +477,19 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __syncthreads();
     if (!s_last_ws) return;
     __threadfence();
-    fold_and_finish(p, nu, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda);
+    fold_and_finish<ADAPT>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist);
 }
 
-// K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out.
+// K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
+// distribution update of finalize_rows.
+template <bool ADAPT>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
-                float* __restrict__ action_mirror) {
-    extern __shared__ float un[];   // [T*nu] then [G] scales
+                float* __restrict__ action_mirror, float* __restrict__ dist) {
+    extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov)
     const int T = p.T, NR = T * nu;
-    int P = 2 + NR;                 // row stride of the partials
+    int P = 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
     const float* partials = partials_in;
     uint32_t seq = 0;
     if (partials_in == nullptr) {
@@ -443,7 +515,7 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
         partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
         P = peers.pcap;
     }
-    finalize_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un);
+    finalize_rows<ADAPT>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
 }
 
@@ -494,26 +566,27 @@ static PeerArgs reduce_peers(const MppibContext* c) {
     return a;
 }
 
-static int reduce_ws_stages(int T, int nu) {
+static int reduce_ws_stages(int T, int nu, bool m2) {
     int ns = 8;
-    while (ns > 1 && WsLayout(T, nu, ns).bytes > 224 * 1024) --ns;
+    while (ns > 1 && WsLayout(T, nu, ns, m2).bytes > 224 * 1024) --ns;
     return ns;
 }
 
-template <int RPL>
+template <int RPL, bool ADAPT>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
-    const int nstage_max = reduce_ws_stages(T, nu);
+    const bool m2 = ADAPT && c->params.update_cov;
+    const int nstage_max = reduce_ws_stages(T, nu, m2);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = WsLayout(T, nu, nstage).bytes;
+    const size_t smem = WsLayout(T, nu, nstage, m2).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -530,8 +603,8 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
     if (grid > MAX_GRID) grid = MAX_GRID;
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
-    mppib_reduce_ws_kernel<RPL><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch, c->reduce_ticket, partial,
-                                                      reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr);
+    mppib_reduce_ws_kernel<RPL, ADAPT><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch, c->reduce_ticket,
+                                                             partial, reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -544,16 +617,29 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     MPPIB_REQUIRE(c->params.K >= 4 && c->params.K % 4 == 0, "mppib_reduce: K=%d must be a positive multiple of 4 (16-byte rows for TMA / 128-bit loads)", c->params.K);
     MPPIB_REQUIRE(T * nu <= 32 * 16, "mppib_reduce: T*nu = %d exceeds %d", T * nu, 32 * 16);
     MPPIB_REQUIRE(T <= 256, "mppib_reduce: T = %d exceeds the 256-row TMA box", T);
-    MPPIB_REQUIRE(reduce_ws_stages(T, nu) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
+    MPPIB_REQUIRE(reduce_ws_stages(T, nu, false) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
+    MPPIB_REQUIRE(!adaptive_cov(c) || reduce_ws_stages(T, nu, true) >= 2,
+                  "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the second-moment row of update_cov", T, nu);
     const int NR = T * nu;
-    if (NR <= 32 * 4) return launch_reduce_ws_t<4>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    if (NR <= 32 * 8) return launch_reduce_ws_t<8>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    return launch_reduce_ws_t<16>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    if (c->dist) {
+        if (NR <= 32 * 4) return launch_reduce_ws_t<4, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        if (NR <= 32 * 8) return launch_reduce_ws_t<8, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        return launch_reduce_ws_t<16, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
+    if (NR <= 32 * 4) return launch_reduce_ws_t<4, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    if (NR <= 32 * 8) return launch_reduce_ws_t<8, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    return launch_reduce_ws_t<16, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
 }
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    mppib_finalize_kernel<<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror);
+    if (c->dist) {
+        const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
+        mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist);
+    } else {
+        mppib_finalize_kernel<false><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
+                                                                              c->action_mirror, nullptr);
+    }
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

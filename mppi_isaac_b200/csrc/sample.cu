@@ -32,10 +32,13 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
     z0 = r * c; z1 = r * s;
 }
 
+// DIAG (adaptive MPPI with update_cov): noise_j = sqrt(cov_j) z_j with cov = dist[1..nu], the live diagonal covariance; the Philox
+// counters, clamping and the null / prior rows are those of the fixed-Sigma kernel.
+template <bool DIAG>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
               const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
-              float* __restrict__ actions, float* __restrict__ noise) {
+              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
     const int K = p.K;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int t = blockIdx.y;
@@ -58,9 +61,13 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
     for (int j = 0; j < MPPIB_MAX_NU; ++j) {
         if (j >= nu) break;
         float n = 0.f;
+        if (DIAG) {
+            n = sqrtf(dist[1 + j]) * z[j];
+        } else {
 #pragma unroll
-        for (int i = 0; i < MPPIB_MAX_NU; ++i)
-            if (i <= j) n += p.sigma_chol[j * nu + i] * z[i];
+            for (int i = 0; i < MPPIB_MAX_NU; ++i)
+                if (i <= j) n += p.sigma_chol[j * nu + i] * z[i];
+        }
         const float u = U[t * nu + j];
         float a = u + n;
         if (is_null) a = 0.f;
@@ -87,7 +94,9 @@ __device__ __forceinline__ float halton(uint32_t index, uint32_t base, uint32_t 
 
 constexpr int MAX_KNOTS = 32;
 
-// one thread per sample k: Gaussian knots (n_knots x nu) -> coloured -> spline-interpolated to T points
+// one thread per sample k: Gaussian knots (n_knots x nu) -> coloured -> spline-interpolated to T points.  WHITE (adaptive MPPI with
+// update_cov): identity colour, the library sampler scales by the live sqrt(cov) on every plan.
+template <bool WHITE>
 __global__ void __launch_bounds__(128)
 mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total,
                            const int32_t* __restrict__ tab, const float* __restrict__ B, int n_knots, float* __restrict__ Z) {
@@ -102,10 +111,11 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
         float cn[MAX_KNOTS];
         for (int n = 0; n < n_knots; ++n) {
             float acc = 0.f;
-            for (int i = 0; i <= j; ++i) {
+            for (int i = WHITE ? j : 0; i <= j; ++i) {
                 const int d = n * nu + i;
                 const float u = halton(kg + 1u, (uint32_t)tab[d], (uint32_t)tab[nd + d]);
-                acc += p.sigma_chol[j * nu + i] * (1.41421356237f * erfinvf(2.0f * u - 1.0f));
+                const float zn = 1.41421356237f * erfinvf(2.0f * u - 1.0f);
+                acc += WHITE ? zn : p.sigma_chol[j * nu + i] * zn;
             }
             cn[n] = acc;
         }
@@ -117,10 +127,12 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     }
 }
 
+// DIAG (adaptive MPPI with update_cov): Z is the white library, scaled by the live sqrt(cov_j) = sqrt(dist[1 + j]).
+template <bool DIAG>
 __global__ void __launch_bounds__(128)
 mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
                             const float* __restrict__ prior_row, const float* __restrict__ Z, float* __restrict__ actions,
-                            float* __restrict__ noise) {
+                            float* __restrict__ noise, const float* __restrict__ dist) {
     const int K = p.K;
     const int k = blockIdx.x * blockDim.x + threadIdx.x, t = blockIdx.y;
     if (k >= K) return;
@@ -130,7 +142,7 @@ mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     for (int j = 0; j < nu; ++j) {
         const size_t idx = ((size_t)t * nu + j) * K + k;
         const float u = U[t * nu + j];
-        float a = u + Z[idx];
+        float a = u + (DIAG ? sqrtf(dist[1 + j]) * Z[idx] : Z[idx]);
         if (is_null) a = 0.f;
         a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
         if (is_prior) a = prior_row[t * nu + j];
@@ -145,7 +157,10 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
                          float* Z, cudaStream_t s) {
     MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
-    mppib_noise_library_kernel<<<(K + 127) / 128, 128, 0, s>>>(c->params, c->model.nu, k_offset, k_total, halton_tab, B, n_knots, Z);
+    if (adaptive_cov(c))
+        mppib_noise_library_kernel<true><<<(K + 127) / 128, 128, 0, s>>>(c->params, c->model.nu, k_offset, k_total, halton_tab, B, n_knots, Z);
+    else
+        mppib_noise_library_kernel<false><<<(K + 127) / 128, 128, 0, s>>>(c->params, c->model.nu, k_offset, k_total, halton_tab, B, n_knots, Z);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -154,7 +169,10 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
                           float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
-    mppib_sample_library_kernel<<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise);
+    if (adaptive_cov(c))
+        mppib_sample_library_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
+    else
+        mppib_sample_library_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -163,7 +181,12 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
-    mppib_sample_kernel<<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U, prior_row, actions, noise);
+    if (adaptive_cov(c))
+        mppib_sample_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
+                                                         prior_row, actions, noise, c->dist);
+    else
+        mppib_sample_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
+                                                          prior_row, actions, noise, nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 
@@ -71,6 +71,8 @@ class MppibParams(C.Structure):
         ("sigma_chol", f32 * (MAX_NU * MAX_NU)), ("sigma_inv", f32 * (MAX_NU * MAX_NU)),
         ("k_offset", C.c_uint32), ("rand_seed", C.c_uint32),
         ("nobs", i32), ("obs", MppibObsItem * MAX_OBS),
+        ("update_cov", i32), ("update_lambda", i32), ("eta_u_bound", f32), ("eta_l_bound", f32),
+        ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32),
     ]
 
 
@@ -379,6 +381,12 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         raise ValueError(f"unknown mppi_mode {mode}")
     p.lambda_ = float(mppi_cfg.lambda_)
     p.step_size_mean = 0.98
+    # adaptive MPPI (DESIGN.md section 2): the two flags and the eta bounds are config keys, the step sizes are constants
+    p.update_cov = int(bool(getattr(mppi_cfg, "update_cov", False)))
+    p.update_lambda = int(bool(getattr(mppi_cfg, "update_lambda", False)))
+    p.eta_u_bound = float(getattr(mppi_cfg, "eta_u_bound", 10.0))
+    p.eta_l_bound = float(getattr(mppi_cfg, "eta_l_bound", 5.0))
+    p.step_size_cov, p.kappa, p.lambda_mult = 0.7, 0.005, 0.1
     p.u_scale = float(mppi_cfg.u_scale)
     p.sample_null_action = int(bool(mppi_cfg.sample_null_action))
     p.filter_u = int(bool(mppi_cfg.filter_u))

@@ -121,9 +121,19 @@ class MPPIPlanner:
         if str(cfg.sampling_method) not in ("random", "halton"):
             raise ValueError(f"unknown sampling_method {cfg.sampling_method}")
         self.use_library = str(cfg.sampling_method) == "halton"     # Halton-spline noise library, drawn once (SURVEY 8(a) M4)
-        if getattr(cfg, "update_cov", False) or getattr(cfg, "update_lambda", False):
-            raise NotImplementedError("update_cov / update_lambda are False in every shipped config and not provided")
+        # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
+        # captured plan graph follows it without re-capture
+        self.update_cov = bool(getattr(cfg, "update_cov", False))
+        self.update_lambda = bool(getattr(cfg, "update_lambda", False))
+        self.adaptive = self.update_cov or self.update_lambda
+        if self.update_cov:
+            import numpy as np
+            sigma = np.asarray(cfg.noise_sigma, np.float64).reshape(self.nu, self.nu)
+            if np.any(sigma != np.diag(np.diag(sigma))):
+                raise ValueError("update_cov adapts a diagonal covariance: noise_sigma must be diagonal")
         self.backend = sim.backend
+        if self.adaptive and not hasattr(self.backend, "set_distribution"):
+            raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
         self._peer_exchange = False
         self._peer_capable = (self.world > 1 and getattr(self.backend, "name", "") == "cuda"
                               and os.environ.get("MPPIB_EXCHANGE", "peer") == "peer")
@@ -197,7 +207,7 @@ class MPPIPlanner:
         self.actions = torch.zeros((T, nu, K), **f32)       # [T][nu][K]
         self.noise = torch.zeros((T, nu, K), **f32)
         self.cost = torch.zeros((T, K), **f32)
-        P = 2 + T * nu
+        P = 2 + T * nu * (2 if self.update_cov else 1)      # (beta, eta, W[T*nu]) + M2[T*nu] with update_cov
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
@@ -210,6 +220,15 @@ class MPPIPlanner:
         self.stats = torch.zeros((2,), **f32)                # (beta, eta)
         self.plan_ctr = torch.zeros((1,), dtype=torch.int32, device=dev)
         self._prior_rows = torch.zeros((T, nu), **f32) if self.use_priors else None
+        # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma); registered before the noise library is built
+        # (update_cov makes it white)
+        self.dist = None
+        if not self.adaptive and hasattr(self.backend, "set_distribution"):
+            self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
+        if self.adaptive:
+            sigma = torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)
+            self.dist = torch.cat([torch.tensor([self.lambda_], dtype=torch.float64), torch.diagonal(sigma)]).to(**f32)
+            self.backend.set_distribution(self.dist)
         self._graph = None
         self._graph_failed = False
         self._graph_epoch = -1
@@ -240,6 +259,18 @@ class MPPIPlanner:
     @property
     def mean_action(self):
         return self.U
+
+    @property
+    def cov_action(self):
+        """(nu,) device view of the diagonal sampling covariance of adaptive MPPI: adapted with update_cov, the constant diag(Sigma)
+        with update_lambda alone, None with both flags off.  ``lambda_`` stays the configured float; the live temperature is
+        ``current_lambda``."""
+        return None if self.dist is None else self.dist[1:]
+
+    @property
+    def current_lambda(self):
+        """0-d device view of the live temperature of adaptive MPPI (None without update_cov / update_lambda)."""
+        return None if self.dist is None else self.dist[0]
 
     @property
     def perturbed_action(self):
@@ -328,6 +359,7 @@ class MPPIPlanner:
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             u_keep, ctr_keep = self.U.clone(), self.plan_ctr.clone()
+            dist_keep = None if self.dist is None else self.dist.clone()      # the warm-up plans adapt the distribution too
             with torch.cuda.stream(side):
                 for _ in range(2):                       # warm-up outside capture (allocator, lazy init)
                     self._plan_batched()
@@ -338,6 +370,8 @@ class MPPIPlanner:
                 self._plan_batched()
             self.U.copy_(u_keep)
             self.plan_ctr.copy_(ctr_keep)
+            if dist_keep is not None:
+                self.dist.copy_(dist_keep)
             self._graph = g
             self._graph_epoch = getattr(self.sim, "model_epoch", 0)
         except Exception as e:  # capture is an optimisation; the eager path is the same kernels

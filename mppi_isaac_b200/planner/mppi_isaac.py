@@ -76,6 +76,8 @@ class MPPIisaacPlanner(object):
         self._sim_build = self.sim.build_epoch         # MPPIPlanner.__init__ re-configures the sim (one more handle)
         if old is not None and old.U.shape == self.mppi.U.shape:
             self.mppi.U.copy_(old.U)           # the warm start survives a rebuilt simulator, as in the reference (mppi is not rebuilt there)
+            if old.dist is not None and self.mppi.dist is not None and old.dist.shape == self.mppi.dist.shape:
+                self.mppi.dist.copy_(old.dist)         # and so does the adapted (lambda, cov) of adaptive MPPI
 
     def _make_mppi(self):
         return MPPIPlanner(
