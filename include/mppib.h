@@ -34,7 +34,10 @@
  *   cost     [T][K]             per-step running cost from Objective.compute_cost
  *   partial  [2 + T*nu]         (beta_g, eta_g, W_g[T][nu]) of one shard;
  *            [2 + 2*T*nu]       (beta_g, eta_g, W_g, M2_g[T][nu]) with update_cov and a registered distribution
- *   dist     [1 + nu]           (lambda, cov[nu]) live sampling distribution of adaptive MPPI (mppib_set_distribution)
+ *            [2 + T*nu + nu(nu+1)/2]  (beta_g, eta_g, W_g, C_g[lower triangle of nu x nu]) with update_cov, cov_full and a
+ *                               registered distribution
+ *   dist     [1 + nu]           (lambda, cov[nu]) live sampling distribution of adaptive MPPI (mppib_set_distribution);
+ *            [1 + 3*nu*nu]      (lambda, Sigma[nu][nu], L[nu][nu], Sigma^-1[nu][nu]) with cov_full, all row-major, L lower
  */
 #ifndef MPPIB_H
 #define MPPIB_H
@@ -45,7 +48,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 14
+#define MPPIB_ABI_VERSION 15
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -202,6 +205,7 @@ typedef struct MppibParams {
     float   step_size_cov;     /* cov <- (1 - s) cov + s mean_t var_t + kappa                                          */
     float   kappa;
     float   lambda_mult;
+    int32_t cov_full;          /* with update_cov: adapt a full Sigma (K1 draws L z, K3 appends C, K4 updates Sigma, L, Sigma^-1) */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -252,7 +256,9 @@ int32_t mppib_rollout(MppibHandle h, const float* state0, const float* root0, fl
  * beta_g = min_k S_k, w_k = exp(-(S_k - beta_g)/lambda), eta_g = sum w_k,
  * W_g[t][j] = sum_k w_k x[t][j][k] with x = noise (SIMPLE) or actions (MEAN).
  * With a registered distribution lambda (and, with update_cov, Sigma^-1 = diag(1/cov)) come from it, and update_cov appends
- * M2_g[t][j] = sum_k w_k (x[t][j][k] - c[t][j])^2, c = U (MEAN) or 0 (SIMPLE).
+ * M2_g[t][j] = sum_k w_k (x[t][j][k] - c[t][j])^2, c = U (MEAN) or 0 (SIMPLE).  With cov_full too, Sigma^-1 is the full one of
+ * the buffer and the row carries C_g = sum_t sum_k w_k (x_tk - c_t)(x_tk - c_t)^T instead of M2_g, packed as its lower triangle
+ * (i >= j, row-major, nu(nu+1)/2 floats); row length 2 + T*nu + nu(nu+1)/2.
  * Single pass over HBM; the last CTA to finish folds the per-CTA partials.                  */
 int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const float* U,
                      float* partial, void* stream);
@@ -272,7 +278,8 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
 /* multi-GPU exchange over peer memory (one process per GPU, one box) -----------------------------
  * Replaces the all-gather between K3 and K4 (the reference has no multi-GPU path; this is the
  * multi-GPU scale-out of its single-GPU mppi_torch reduction, SURVEY.md 8(e)).  Every rank owns a small
- * WINDOW in its HBM: [2 parities][world] rows of 2 + T*nu floats plus one arrival flag per row.
+ * WINDOW in its HBM: [2 parities][world] rows of 2 + T*nu floats (2 + 2*T*nu with update_cov, 2 + T*nu + nu(nu+1)/2 with
+ * update_cov and cov_full; rounded up to a multiple of 4) plus one arrival flag per row.
  * With peers open, the last CTA of mppib_reduce stores this rank's (beta, eta, W) row straight
  * into the window of EVERY rank over NVLink (st.global + fence.sys + st.release.sys of the flag),
  * and mppib_finalize (called with partials == NULL) spins on its own window's flags
@@ -325,7 +332,12 @@ int32_t mppib_set_action_mirror(MppibHandle h, float* mirror);
  * mppib_sample_library scales per plan), K3 weights with the buffer's lambda (and diag(1/cov)), and K4 updates the buffer in
  * place after the U update: cov (update_cov, needs the [2 + 2*T*nu] partial rows) and lambda (update_lambda); dist is left
  * as it is when no sample is valid.  Because the buffer lives in device memory, a captured plan graph follows it.  NULL
- * switches it off: every launch then runs the fixed-distribution kernels.                                                   */
+ * switches it off: every launch then runs the fixed-distribution kernels.
+ * With update_cov and cov_full the buffer is dist[1 + 3*nu*nu] = (lambda, Sigma[nu][nu], L[nu][nu], Sigma^-1[nu][nu]), row-major,
+ * L the lower Cholesky factor of Sigma (zero above the diagonal), all three consistent at registration.  K1 draws noise = L z
+ * (the library sampler colours the white library by L), K3 uses the full Sigma^-1 in SIMPLE mode and appends C, and K4 updates
+ * Sigma, then L and Sigma^-1 on the device; a non-positive-definite update leaves the three as they were.  The partial rows
+ * are [2 + T*nu + nu(nu+1)/2].                                                                                              */
 int32_t mppib_set_distribution(MppibHandle h, float* dist);
 
 /* shift U by one step: U[t] <- U[t+1], U[T-1] <- u_init (mppi_torch command() prologue);

@@ -177,22 +177,44 @@ class CudaBackend:
         self._mirror_keepalive = pinned_host_tensor
         self._check(self.lib.mppib_set_action_mirror(self.handle, _ptr(pinned_host_tensor)), "mppib_set_action_mirror")
 
+    def _cov_full(self):
+        return bool(self.params.update_cov) and bool(self.params.cov_full)
+
+    def partial_row_floats(self) -> int:
+        """Floats of one shard row K3 writes with a registered distribution: 2 + T*nu, + T*nu with update_cov, or + nu(nu+1)/2
+        with update_cov and cov_full."""
+        T, nu = int(self.params.T), int(self.model.nu)
+        if self._cov_full():
+            return 2 + T * nu + nu * (nu + 1) // 2
+        return 2 + T * nu * (2 if self.params.update_cov else 1)
+
+    def _check_row(self, rows, what):
+        if self._cov_full() and self._dist_keepalive is not None and rows is not None and rows.shape[-1] != self.partial_row_floats():
+            raise RuntimeError(f"{what}: cov_full shard rows hold {self.partial_row_floats()} floats, got {rows.shape[-1]}")
+
     def set_distribution(self, dist):
-        """Adaptive MPPI: register the device tensor (lambda, cov[nu]) that K1 / K3 read and K4 updates (None switches it off)."""
+        """Adaptive MPPI: register the device tensor (lambda, cov[nu]) -- with cov_full (lambda, Sigma, L, Sigma^-1), 1 + 3 nu^2
+        floats -- that K1 / K3 read and K4 updates (None switches it off)."""
+        if dist is not None and self._cov_full() and dist.numel() != 1 + 3 * self.model.nu ** 2:
+            raise RuntimeError(f"mppib_set_distribution: cov_full needs (lambda, Sigma, L, Sigma^-1) = {1 + 3 * self.model.nu ** 2} floats, "
+                               f"got {dist.numel()}")
         self._dist_keepalive = dist
         self._check(self.lib.mppib_set_distribution(self.handle, _ptr(dist)), "mppib_set_distribution")
 
     def reduce(self, cost, x, U, partial):
+        self._check_row(partial, "mppib_reduce")
         self.launches += 1
         self._check(self.lib.mppib_reduce(self.handle, _ptr(cost), _ptr(x), _ptr(U), _ptr(partial), self._stream()), "mppib_reduce")
 
     def reduce_finalize(self, cost, x, U, partial, action_out, stats):
         """K3 + K4 in one launch (single-GPU plans)."""
+        self._check_row(partial, "mppib_reduce_finalize")
         self.launches += 1
         self._check(self.lib.mppib_reduce_finalize(self.handle, _ptr(cost), _ptr(x), _ptr(U), _ptr(partial), _ptr(action_out), _ptr(stats), self._stream()),
                     "mppib_reduce_finalize")
 
     def finalize(self, partials, G, U, action_out, stats):
+        self._check_row(partials, "mppib_finalize")
         self.launches += 1
         self._check(self.lib.mppib_finalize(self.handle, _ptr(partials), C.c_int32(G), _ptr(U), _ptr(action_out), _ptr(stats), self._stream()), "mppib_finalize")
 

@@ -42,6 +42,7 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     if (p->update_cov || p->update_lambda)
         MPPIB_REQUIRE(p->step_size_cov >= 0.f && p->step_size_cov <= 1.f && p->kappa >= 0.f && p->lambda_mult >= 0.f && p->lambda_mult < 1.f,
                       "adaptive MPPI: step_size_cov %g, kappa %g or lambda_mult %g out of range", p->step_size_cov, p->kappa, p->lambda_mult);
+    MPPIB_REQUIRE(!p->cov_full || p->update_cov, "cov_full selects the update rule of update_cov and needs update_cov");
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);

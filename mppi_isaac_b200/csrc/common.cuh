@@ -45,7 +45,8 @@ struct MppibContext {
     void* peer_win[MPPIB_MAX_PEERS];           // window base of every rank (own entry = local allocation)
     unsigned long long peer_timeout_ns;
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
-    float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) read by K1 / K3, updated by K4 (nullable)
+    float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) or, with cov_full, (lambda, Sigma, L, Sigma^-1)
+                                               // read by K1 / K3, updated by K4 (nullable)
     // K2 mappings the handle may use (rollout_mapping() picks by scene, never by K); both default to true
     bool k2_team;                              // a team of lanes per rollout for trees / contact scenes (rollout_team.cu); MPPIB_K2_TEAM=0 turns it off
     bool k2_lanes;                             // one body per lane for serial chains (rollout_lanes.cu); MPPIB_K2_LANES=0 turns it off
@@ -69,10 +70,15 @@ struct DeviceGuard {
     DeviceGuard _guard((h)->device);                                                        \
     MPPIB_CHECK_CUDA(_guard.err)
 
-// Floats of one shard row (beta, eta, W[T*nu] and, with update_cov, M2[T*nu]).  Buffers are sized by the flag alone, so that
-// registering a distribution never needs a reallocation; the kernels append M2 only when a distribution is registered too.
-static inline int partial_row_capacity(const MppibParams& p, int nu) { return 2 + p.T * nu * (p.update_cov ? 2 : 1); }
+// Floats of one shard row (beta, eta, W[T*nu] and, with update_cov, M2[T*nu], or with cov_full too C[nu(nu+1)/2]).  Buffers are
+// sized by the flags alone, so that registering a distribution never needs a reallocation; the kernels append M2 / C only when a
+// distribution is registered too.
+static inline int partial_row_capacity(const MppibParams& p, int nu) {
+    if (p.update_cov && p.cov_full) return 2 + p.T * nu + nu * (nu + 1) / 2;
+    return 2 + p.T * nu * (p.update_cov ? 2 : 1);
+}
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
+static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
 
 // device view of the peer windows, passed by value to K3 / K4
 struct PeerArgs {

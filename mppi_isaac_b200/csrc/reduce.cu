@@ -21,6 +21,15 @@ namespace {
 
 constexpr int NT = 256;         // threads per CTA
 constexpr int MAX_GRID = 512;   // persistent CTAs (<= scratch rows)
+constexpr int MAX_PAIRS = MPPIB_MAX_NU * (MPPIB_MAX_NU + 1) / 2;   // lower triangle of a full nu x nu covariance
+
+// what a shard row carries after (beta, eta, W[T*nu]): nothing, M2[T*nu] (update_cov) or C[nu(nu+1)/2] (update_cov with cov_full)
+enum RowKind { ROW_W = 0, ROW_M2 = 1, ROW_C = 2 };
+__host__ __device__ __forceinline__ int row_floats(int T, int nu, int kind) {
+    return 2 + T * nu + (kind == ROW_M2 ? T * nu : kind == ROW_C ? nu * (nu + 1) / 2 : 0);
+}
+// shared floats finalize_rows<true, true> needs after un[T*nu] and the G scales: m1[T*nu], d[T*nu], C[nu(nu+1)/2], Sigma, L, L^-1
+__host__ __device__ __forceinline__ int full_fin_floats(int T, int nu) { return 2 * T * nu + nu * (nu + 1) / 2 + 3 * nu * nu; }
 
 __device__ __forceinline__ float warp_min(float v) {
 #pragma unroll
@@ -73,7 +82,12 @@ __constant__ float c_sg_edge[4][9] = {{763.f, 441.f, 189.f, 7.f, -105.f, -147.f,
 // and leaves it as it is when no sample is valid.  The mean over t runs serially in t order on one thread per j, so every rank of a
 // multi-GPU plan, which combines the same rows in the same order, writes bit-identical values.  Every thread reads dist[0] at entry and
 // dist[1 + j] is read and written by thread j only; the writes come after the __syncthreads below, so nothing reads a value written here.
-template <bool ADAPT>
+// FULL (update_cov with cov_full; dist = (lambda, Sigma, L, Sigma^-1)): the rows carry C_g[nu(nu+1)/2] after W_g.  With m1 = W/eta - c and
+// d = U_new - U_old per (t, j):  V = C/eta - sum_t (m1_t d_t^T + d_t m1_t^T - d_t d_t^T),  Sigma <- (1 - s) Sigma + (s/T) V + kappa I,
+// one thread per lower-triangle entry (t in order), written to both halves; then warp 0 computes L = chol(Sigma) (left-looking, lane =
+// row) and Sigma^-1 = L^-T L^-1 (lane = column of L^-1) in a fixed order.  A pivot that is not finite and positive leaves Sigma, L and
+// Sigma^-1 as they were.  The diagonal equals the diagonal rule above without its clamp at 0.
+template <bool ADAPT, bool FULL = false>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
                                               float* __restrict__ dist) {
@@ -81,8 +95,15 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
     float* sg = un + NR;
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
-    const bool cov = ADAPT && p.update_cov;
+    const bool cov = ADAPT && !FULL && p.update_cov;
     float* var = sg + G;                                                      // [NR] per-element variance (update_cov)
+    const int npairs = nu * (nu + 1) / 2;
+    float* m1s = sg + G;                                                      // FULL: [NR] m1, [NR] d, [npairs] C, [nu*nu] Sigma, L, L^-1
+    float* dds = m1s + NR;
+    float* cc = dds + NR;
+    float* sn = cc + npairs;
+    float* Lm = sn + nu * nu;
+    float* Mi = Lm + nu * nu;
     float b = INFINITY;
     for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
     for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
@@ -103,6 +124,17 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
             const float c0 = p.mode == MPPIB_MODE_SIMPLE ? 0.f : U[r];
             const float m1 = w / e - c0, d = un[r] - U[r];
             var[r] = fmaxf(m2 / e - 2.0f * d * m1 + d * d, 0.f);
+        }
+        if (FULL && e > 0.f) {
+            m1s[r] = w / e - (p.mode == MPPIB_MODE_SIMPLE ? 0.f : U[r]);
+            dds[r] = un[r] - U[r];
+        }
+    }
+    if (FULL && e > 0.f) {
+        for (int q = threadIdx.x; q < npairs; q += blockDim.x) {
+            float cq = 0.f;
+            for (int gidx = 0; gidx < G; ++gidx) cq += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + NR + q]);
+            cc[q] = cq;
         }
     }
     __syncthreads();
@@ -131,6 +163,68 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
         if (r < nu) { action_out[r] = out; if (action_mirror) action_mirror[r] = out; }
     }
     if (threadIdx.x == 0 && stats) { stats[0] = b; stats[1] = e; }
+    if (FULL && e > 0.f) {
+        const float* Sig = dist + 1;
+        for (int q = threadIdx.x; q < npairs; q += blockDim.x) {
+            int i = 0;
+            while ((i + 1) * (i + 2) / 2 <= q) ++i;
+            const int j = q - i * (i + 1) / 2;
+            float acc = 0.f;
+            for (int t = 0; t < T; ++t) {
+                const float mi = m1s[t * nu + i], mj = m1s[t * nu + j], di = dds[t * nu + i], dj = dds[t * nu + j];
+                acc += mi * dj + di * mj - di * dj;
+            }
+            const float v = cc[q] / e - acc;
+            const float sij = (1.0f - p.step_size_cov) * Sig[i * nu + j] + (p.step_size_cov / (float)T) * v + (i == j ? p.kappa : 0.f);
+            sn[i * nu + j] = sij;
+            sn[j * nu + i] = sij;
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            const int l = threadIdx.x;
+            for (int q = l; q < nu * nu; q += 32) { Lm[q] = 0.f; Mi[q] = 0.f; }
+            __syncwarp();
+            bool ok = true;
+            for (int k = 0; k < nu && ok; ++k) {                         // every lane computes the same pivot in the same order
+                float dk = sn[k * nu + k];
+                for (int m = 0; m < k; ++m) dk -= Lm[k * nu + m] * Lm[k * nu + m];
+                ok = isfinite(dk) && dk > 0.f;
+                if (ok) {
+                    const float lkk = sqrtf(dk);
+                    if (l > k && l < nu) {
+                        float a = sn[l * nu + k];
+                        for (int m = 0; m < k; ++m) a -= Lm[l * nu + m] * Lm[k * nu + m];
+                        Lm[l * nu + k] = a / lkk;
+                    }
+                    if (l == k) Lm[k * nu + k] = lkk;
+                }
+                __syncwarp();
+            }
+            if (ok) {
+                if (l < nu) {                                             // column l of L^-1 by forward substitution
+                    for (int i = l; i < nu; ++i) {
+                        float a = i == l ? 1.0f : 0.f;
+                        for (int m = l; m < i; ++m) a -= Lm[i * nu + m] * Mi[m * nu + l];
+                        Mi[i * nu + l] = a / Lm[i * nu + i];
+                    }
+                }
+                __syncwarp();
+                float* dS = dist + 1;
+                float* dL = dS + nu * nu;
+                float* dI = dL + nu * nu;
+                for (int q = l; q < npairs; q += 32) {                   // Sigma^-1 = L^-T L^-1, lower triangle, written to both halves
+                    int i = 0;
+                    while ((i + 1) * (i + 2) / 2 <= q) ++i;
+                    const int j = q - i * (i + 1) / 2;
+                    float a = 0.f;
+                    for (int m = i; m < nu; ++m) a += Mi[m * nu + i] * Mi[m * nu + j];
+                    dI[i * nu + j] = a;
+                    dI[j * nu + i] = a;
+                }
+                for (int q = l; q < nu * nu; q += 32) { dS[q] = sn[q]; dL[q] = Lm[q]; }
+            }
+        }
+    }
     if (ADAPT && e > 0.f) {
         if (cov) {
             for (int j = threadIdx.x; j < nu; j += blockDim.x) {
@@ -151,7 +245,7 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
 // at least, `misc` = 8 floats.
-template <bool ADAPT>
+template <bool ADAPT, bool FULL = false>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
@@ -228,7 +322,7 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             // cov -- in its prologue, before it took its ticket, so this CTA is the only reader left when it updates them.
             __threadfence();
             __syncthreads();
-            finalize_rows<ADAPT>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            finalize_rows<ADAPT, FULL>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
         }
     }
 }
@@ -249,15 +343,17 @@ constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
 
 // Shared-memory layout of the kernel with `nstage` ring stages, used by the host for the size and by the kernel for its pointers.
 // Offsets in floats from the base, except `bar` (bytes).  The last CTA reuses the ring for the fold (fold_and_finish), so the ring
-// region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.
+// region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.  With the C row (ROW_C)
+// the fused K4 also keeps its covariance scratch there (full_fin_floats), which the ring stages of every accepted shape exceed.
 struct WsLayout {
     int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [NCONS][P4] warp partials | [8]
     int bar;                      // full[nstage], then empty[nstage] mbarriers
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
-    __host__ __device__ WsLayout(int T, int nu, int nstage, bool m2 = false) {   // m2: the shard row carries M2 (2 + 2 T*nu floats)
-        const int NR = T * nu, P4 = (2 + NR * (m2 ? 2 : 1) + 3) & ~3;
+    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W) {   // kind: what the shard row carries after W (RowKind)
+        const int NR = T * nu, P4 = (row_floats(T, nu, kind) + 3) & ~3;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
+        if (kind == ROW_C && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
         gp = g + ((NR + 3) & ~3);
         wk = gp + ((T + 3) & ~3);
         cpart = wk + 8 * WS_W;
@@ -274,7 +370,11 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // ADAPT (a distribution is registered): lambda comes from dist[0]; with update_cov the SIMPLE-mode Sigma^-1 is diag(1 / dist[1 + j])
 // and phase C keeps a second running sum per row, M2[r] = sum_k w_k (x[r][k] - c[r])^2 with c = U (MEAN) or 0 (SIMPLE), rescaled
 // online like W; the shard row becomes (beta, eta, W[T*nu], M2[T*nu]).  The bytes read from HBM are the same.
-template <int RPL, bool ADAPT>   // rows of W per lane: T*nu <= 32 * RPL
+// FULL (update_cov with cov_full): the SIMPLE-mode Sigma^-1 is the full one of dist, and instead of M2 every consumer lane keeps the
+// lower triangle of sum_t w_k (x_tk - c_t)(x_tk - c_t)^T of its own sample k across tiles (lane = sample: column reads of the tile,
+// conflict-free like phase A; c = U staged in g in MEAN mode), rescaled online like W and summed over the warp once after the loop;
+// the shard row becomes (beta, eta, W[T*nu], C[nu(nu+1)/2]).
+template <int RPL, bool ADAPT, bool FULL = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
@@ -286,14 +386,15 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
     const bool simple = p.mode == MPPIB_MODE_SIMPLE;
-    const bool m2 = ADAPT && p.update_cov;
-    const int P = 2 + (m2 ? 2 : 1) * NR;
+    const bool m2 = ADAPT && !FULL && p.update_cov;
+    const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
+    const int P = 2 + (m2 ? 2 : 1) * NR + npairs;
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
-    const WsLayout L(T, nu, nstage, m2);
+    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
-    float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded
+    float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
     float* wk = tiles + L.wk;                                                 // [8][32] weights of the tile a warp is working on
     float* cpart = tiles + L.cpart;                                           // [NCONS][P4] warp partials (after the loop)
@@ -323,11 +424,15 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         float acc = 0.f;
         if (simple && r < NR) {
             const int t = r / nu, i = r % nu;
-            if (m2) acc = (1.0f / dist[1 + i]) * U[r];
+            if (FULL) {
+                const float* sinv = dist + 1 + 2 * nu * nu;
+                for (int j = 0; j < nu; ++j) acc += sinv[i * nu + j] * U[t * nu + j];
+            } else if (m2) acc = (1.0f / dist[1 + i]) * U[r];
             else
                 for (int j = 0; j < nu; ++j) acc += p.sigma_inv[i * nu + j] * U[t * nu + j];
             acc *= lam;
         }
+        if (FULL && !simple && r < NR) acc = U[r];                            // phase A reads g in SIMPLE mode only
         g[r] = acc;
     }
     {
@@ -353,6 +458,9 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         float* wme = wk + warp * WS_W;
         float b_run = INFINITY, e_run = 0.f, w_run[RPL];
         float m2_run[ADAPT ? RPL : 1], c_row[ADAPT ? RPL : 1];               // second moment and its centre per row (update_cov)
+        float c_run[FULL ? MAX_PAIRS : 1];                                    // FULL: this lane's lower triangle of C
+#pragma unroll
+        for (int q = 0; q < (FULL ? MAX_PAIRS : 1); ++q) c_run[q] = 0.f;
 #pragma unroll
         for (int i = 0; i < RPL; ++i) w_run[i] = 0.f;
         if (ADAPT) {
@@ -432,6 +540,24 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                         w_run[rr] = w_run[rr] * s_old + acc * s_new;
                     }
                 }
+                if constexpr (FULL) {
+                    // ---- C of this lane's sample: lane = sample, column reads (conflict-free), weight rescaled to b_out
+                    const float ws = w * s_new;
+#pragma unroll
+                    for (int q = 0; q < MAX_PAIRS; ++q) if (q < npairs) c_run[q] *= s_old;
+                    for (int t = 0; t < T; ++t) {
+                        float dx[MPPIB_MAX_NU];
+#pragma unroll
+                        for (int i = 0; i < MPPIB_MAX_NU; ++i) dx[i] = i < nu ? xs[(t * nu + i) * WS_W + lane] - (simple ? 0.f : g[t * nu + i]) : 0.f;
+#pragma unroll
+                        for (int i = 0; i < MPPIB_MAX_NU; ++i) {
+                            if (i >= nu) break;
+                            const float wd = ws * dx[i];
+#pragma unroll
+                            for (int j = 0; j <= i; ++j) c_run[i * (i + 1) / 2 + j] = fmaf(wd, dx[j], c_run[i * (i + 1) / 2 + j]);
+                        }
+                    }
+                }
                 e_run = e_run * s_old + e_c * s_new;
                 b_run = b_out;
             }
@@ -446,6 +572,14 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         if (ADAPT && m2) {
 #pragma unroll
             for (int rr = 0; rr < RPL; ++rr) { const int r = lane + 32 * rr; if (r < NR) mine[2 + NR + r] = m2_run[ADAPT ? rr : 0]; }
+        }
+        if constexpr (FULL) {
+#pragma unroll
+            for (int q = 0; q < MAX_PAIRS; ++q) {
+                if (q >= npairs) break;
+                const float v = warp_sum(c_run[q]);
+                if (lane == 0) mine[2 + NR + q] = v;
+            }
         }
     } else {
         // spare warp (fewer ring stages than warps): an empty partial
@@ -477,19 +611,19 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __syncthreads();
     if (!s_last_ws) return;
     __threadfence();
-    fold_and_finish<ADAPT>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist);
+    fold_and_finish<ADAPT, FULL>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
-// distribution update of finalize_rows.
-template <bool ADAPT>
+// distribution update of finalize_rows (FULL: of the full covariance).
+template <bool ADAPT, bool FULL = false>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
                 float* __restrict__ action_mirror, float* __restrict__ dist) {
-    extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov)
+    extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const int T = p.T, NR = T * nu;
-    int P = 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
+    int P = FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
     const float* partials = partials_in;
     uint32_t seq = 0;
     if (partials_in == nullptr) {
@@ -515,7 +649,7 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
         partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
         P = peers.pcap;
     }
-    finalize_rows<ADAPT>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
+    finalize_rows<ADAPT, FULL>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
 }
 
@@ -566,27 +700,27 @@ static PeerArgs reduce_peers(const MppibContext* c) {
     return a;
 }
 
-static int reduce_ws_stages(int T, int nu, bool m2) {
+static int reduce_ws_stages(int T, int nu, int kind) {
     int ns = 8;
-    while (ns > 1 && WsLayout(T, nu, ns, m2).bytes > 224 * 1024) --ns;
+    while (ns > 1 && WsLayout(T, nu, ns, kind).bytes > 224 * 1024) --ns;
     return ns;
 }
 
-template <int RPL, bool ADAPT>
+template <int RPL, bool ADAPT, bool FULL = false>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
-    const bool m2 = ADAPT && c->params.update_cov;
-    const int nstage_max = reduce_ws_stages(T, nu, m2);
+    const int kind = FULL ? ROW_C : (ADAPT && c->params.update_cov) ? ROW_M2 : ROW_W;
+    const int nstage_max = reduce_ws_stages(T, nu, kind);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = WsLayout(T, nu, nstage, m2).bytes;
+    const size_t smem = WsLayout(T, nu, nstage, kind).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -603,7 +737,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
     if (grid > MAX_GRID) grid = MAX_GRID;
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
-    mppib_reduce_ws_kernel<RPL, ADAPT><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch, c->reduce_ticket,
+    mppib_reduce_ws_kernel<RPL, ADAPT, FULL><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch, c->reduce_ticket,
                                                              partial, reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -617,10 +751,17 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     MPPIB_REQUIRE(c->params.K >= 4 && c->params.K % 4 == 0, "mppib_reduce: K=%d must be a positive multiple of 4 (16-byte rows for TMA / 128-bit loads)", c->params.K);
     MPPIB_REQUIRE(T * nu <= 32 * 16, "mppib_reduce: T*nu = %d exceeds %d", T * nu, 32 * 16);
     MPPIB_REQUIRE(T <= 256, "mppib_reduce: T = %d exceeds the 256-row TMA box", T);
-    MPPIB_REQUIRE(reduce_ws_stages(T, nu, false) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
-    MPPIB_REQUIRE(!adaptive_cov(c) || reduce_ws_stages(T, nu, true) >= 2,
+    MPPIB_REQUIRE(reduce_ws_stages(T, nu, ROW_W) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
+    MPPIB_REQUIRE(!adaptive_cov(c) || adaptive_full(c) || reduce_ws_stages(T, nu, ROW_M2) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the second-moment row of update_cov", T, nu);
+    MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(T, nu, ROW_C) >= 2,
+                  "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the covariance row of cov_full", T, nu);
     const int NR = T * nu;
+    if (adaptive_full(c)) {
+        if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        return launch_reduce_ws_t<16, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
     if (c->dist) {
         if (NR <= 32 * 4) return launch_reduce_ws_t<4, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
         if (NR <= 32 * 8) return launch_reduce_ws_t<8, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
@@ -633,7 +774,10 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    if (c->dist) {
+    if (adaptive_full(c)) {
+        const size_t smem = (NR + G + full_fin_floats(c->params.T, c->model.nu)) * sizeof(float);
+        mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist);
+    } else if (c->dist) {
         const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
         mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist);
     } else {

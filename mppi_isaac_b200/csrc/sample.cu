@@ -34,7 +34,9 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
 
 // DIAG (adaptive MPPI with update_cov): noise_j = sqrt(cov_j) z_j with cov = dist[1..nu], the live diagonal covariance; the Philox
 // counters, clamping and the null / prior rows are those of the fixed-Sigma kernel.
-template <bool DIAG>
+// FULL (update_cov with cov_full): noise = L z with L = dist[1 + nu*nu ..], the live lower Cholesky factor, summed in the order of the
+// fixed-Sigma kernel.
+template <bool DIAG, bool FULL = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
               const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
@@ -63,6 +65,11 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
         float n = 0.f;
         if (DIAG) {
             n = sqrtf(dist[1 + j]) * z[j];
+        } else if (FULL) {
+            const float* Ld = dist + 1 + nu * nu;
+#pragma unroll
+            for (int i = 0; i < MPPIB_MAX_NU; ++i)
+                if (i <= j) n += Ld[j * nu + i] * z[i];
         } else {
 #pragma unroll
             for (int i = 0; i < MPPIB_MAX_NU; ++i)
@@ -95,7 +102,7 @@ __device__ __forceinline__ float halton(uint32_t index, uint32_t base, uint32_t 
 constexpr int MAX_KNOTS = 32;
 
 // one thread per sample k: Gaussian knots (n_knots x nu) -> coloured -> spline-interpolated to T points.  WHITE (adaptive MPPI with
-// update_cov): identity colour, the library sampler scales by the live sqrt(cov) on every plan.
+// update_cov): identity colour, the library sampler scales by the live sqrt(cov) (or colours by the live L, cov_full) on every plan.
 template <bool WHITE>
 __global__ void __launch_bounds__(128)
 mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total,
@@ -128,7 +135,8 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
 }
 
 // DIAG (adaptive MPPI with update_cov): Z is the white library, scaled by the live sqrt(cov_j) = sqrt(dist[1 + j]).
-template <bool DIAG>
+// FULL (update_cov with cov_full): Z is the white library, coloured by the live L = dist[1 + nu*nu ..]: a = clamp(U + L Z[t][:, k]).
+template <bool DIAG, bool FULL = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
                             const float* __restrict__ prior_row, const float* __restrict__ Z, float* __restrict__ actions,
@@ -139,15 +147,38 @@ mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const uint32_t kg = k_offset + (uint32_t)k;
     const bool is_null = p.sample_null_action && kg == k_total - 1;
     const bool is_prior = prior_row != nullptr && kg == k_total - 2;
-    for (int j = 0; j < nu; ++j) {
-        const size_t idx = ((size_t)t * nu + j) * K + k;
-        const float u = U[t * nu + j];
-        float a = u + (DIAG ? sqrtf(dist[1 + j]) * Z[idx] : Z[idx]);
-        if (is_null) a = 0.f;
-        a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-        if (is_prior) a = prior_row[t * nu + j];
-        actions[idx] = a;
-        if (noise) noise[idx] = a - u;
+    if constexpr (FULL) {
+        const float* Ld = dist + 1 + nu * nu;
+        float zc[MPPIB_MAX_NU];
+#pragma unroll
+        for (int i = 0; i < MPPIB_MAX_NU; ++i) zc[i] = i < nu ? Z[((size_t)t * nu + i) * K + k] : 0.f;
+#pragma unroll
+        for (int j = 0; j < MPPIB_MAX_NU; ++j) {
+            if (j >= nu) break;
+            float n = 0.f;
+#pragma unroll
+            for (int i = 0; i < MPPIB_MAX_NU; ++i)
+                if (i <= j) n += Ld[j * nu + i] * zc[i];
+            const size_t idx = ((size_t)t * nu + j) * K + k;
+            const float u = U[t * nu + j];
+            float a = u + n;
+            if (is_null) a = 0.f;
+            a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+            if (is_prior) a = prior_row[t * nu + j];
+            actions[idx] = a;
+            if (noise) noise[idx] = a - u;
+        }
+    } else {
+        for (int j = 0; j < nu; ++j) {
+            const size_t idx = ((size_t)t * nu + j) * K + k;
+            const float u = U[t * nu + j];
+            float a = u + (DIAG ? sqrtf(dist[1 + j]) * Z[idx] : Z[idx]);
+            if (is_null) a = 0.f;
+            a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+            if (is_prior) a = prior_row[t * nu + j];
+            actions[idx] = a;
+            if (noise) noise[idx] = a - u;
+        }
     }
 }
 
@@ -169,7 +200,9 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
                           float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
-    if (adaptive_cov(c))
+    if (adaptive_full(c))
+        mppib_sample_library_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
+    else if (adaptive_cov(c))
         mppib_sample_library_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
     else
         mppib_sample_library_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, nullptr);
@@ -181,7 +214,10 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
-    if (adaptive_cov(c))
+    if (adaptive_full(c))
+        mppib_sample_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset,
+                                                                k_total, U, prior_row, actions, noise, c->dist);
+    else if (adaptive_cov(c))
         mppib_sample_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
                                                          prior_row, actions, noise, c->dist);
     else

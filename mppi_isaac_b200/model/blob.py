@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 
@@ -72,7 +72,7 @@ class MppibParams(C.Structure):
         ("k_offset", C.c_uint32), ("rand_seed", C.c_uint32),
         ("nobs", i32), ("obs", MppibObsItem * MAX_OBS),
         ("update_cov", i32), ("update_lambda", i32), ("eta_u_bound", f32), ("eta_l_bound", f32),
-        ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32),
+        ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32), ("cov_full", i32),
     ]
 
 
@@ -387,6 +387,12 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     p.eta_u_bound = float(getattr(mppi_cfg, "eta_u_bound", 10.0))
     p.eta_l_bound = float(getattr(mppi_cfg, "eta_l_bound", 5.0))
     p.step_size_cov, p.kappa, p.lambda_mult = 0.7, 0.005, 0.1
+    cov_type = str(getattr(mppi_cfg, "cov_type", "diag"))
+    if cov_type not in ("diag", "full"):
+        raise ValueError(f"unknown cov_type {cov_type!r} (diag | full)")
+    if cov_type == "full" and not p.update_cov:
+        raise ValueError("cov_type: full selects the update rule of update_cov and needs update_cov: true")
+    p.cov_full = int(cov_type == "full")
     p.u_scale = float(mppi_cfg.u_scale)
     p.sample_null_action = int(bool(mppi_cfg.sample_null_action))
     p.filter_u = int(bool(mppi_cfg.filter_u))
@@ -403,6 +409,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     umin, umax = bc(mppi_cfg.u_min, -1e30), bc(mppi_cfg.u_max, 1e30)
     uinit = bc(mppi_cfg.u_init, 0.0)
     sigma = np.asarray(mppi_cfg.noise_sigma, np.float64).reshape(nu, nu)
+    if p.cov_full and (np.any(sigma != sigma.T) or np.any(np.linalg.eigvalsh(sigma) <= 0)):
+        raise ValueError("cov_type: full needs a symmetric positive-definite noise_sigma")
     chol = np.linalg.cholesky(sigma)
     sinv = np.linalg.inv(sigma)
     for j in range(nu):

@@ -126,7 +126,10 @@ class MPPIPlanner:
         self.update_cov = bool(getattr(cfg, "update_cov", False))
         self.update_lambda = bool(getattr(cfg, "update_lambda", False))
         self.adaptive = self.update_cov or self.update_lambda
-        if self.update_cov:
+        # cov_type chooses the update rule of update_cov: "diag" adapts diag(Sigma), "full" the whole Sigma with its Cholesky factor
+        # and inverse (DESIGN.md section 2); make_params rejects other values, full without update_cov and a Sigma that is not SPD
+        self.cov_full = self.update_cov and str(getattr(cfg, "cov_type", "diag")) == "full"
+        if self.update_cov and not self.cov_full:
             import numpy as np
             sigma = np.asarray(cfg.noise_sigma, np.float64).reshape(self.nu, self.nu)
             if np.any(sigma != np.diag(np.diag(sigma))):
@@ -208,6 +211,8 @@ class MPPIPlanner:
         self.noise = torch.zeros((T, nu, K), **f32)
         self.cost = torch.zeros((T, K), **f32)
         P = 2 + T * nu * (2 if self.update_cov else 1)      # (beta, eta, W[T*nu]) + M2[T*nu] with update_cov
+        if self.cov_full:
+            P = 2 + T * nu + nu * (nu + 1) // 2               # (beta, eta, W[T*nu]) + C[lower triangle] with cov_type full
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
@@ -220,14 +225,19 @@ class MPPIPlanner:
         self.stats = torch.zeros((2,), **f32)                # (beta, eta)
         self.plan_ctr = torch.zeros((1,), dtype=torch.int32, device=dev)
         self._prior_rows = torch.zeros((T, nu), **f32) if self.use_priors else None
-        # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma); registered before the noise library is built
-        # (update_cov makes it white)
+        # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma), or with cov_type full (lambda, Sigma, L, Sigma^-1)
+        # computed in float64 and rounded; registered before the noise library is built (update_cov makes it white)
         self.dist = None
         if not self.adaptive and hasattr(self.backend, "set_distribution"):
             self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
         if self.adaptive:
             sigma = torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)
-            self.dist = torch.cat([torch.tensor([self.lambda_], dtype=torch.float64), torch.diagonal(sigma)]).to(**f32)
+            if self.cov_full:
+                chol = torch.linalg.cholesky(sigma)
+                parts = [sigma.reshape(-1), chol.reshape(-1), torch.cholesky_inverse(chol).reshape(-1)]
+            else:
+                parts = [torch.diagonal(sigma)]
+            self.dist = torch.cat([torch.tensor([self.lambda_], dtype=torch.float64), *parts]).to(**f32)
             self.backend.set_distribution(self.dist)
         self._graph = None
         self._graph_failed = False
@@ -263,9 +273,13 @@ class MPPIPlanner:
     @property
     def cov_action(self):
         """(nu,) device view of the diagonal sampling covariance of adaptive MPPI: adapted with update_cov, the constant diag(Sigma)
-        with update_lambda alone, None with both flags off.  ``lambda_`` stays the configured float; the live temperature is
-        ``current_lambda``."""
-        return None if self.dist is None else self.dist[1:]
+        with update_lambda alone, None with both flags off; with cov_type full the (nu, nu) view of the adapted Sigma.  ``lambda_``
+        stays the configured float; the live temperature is ``current_lambda``."""
+        if self.dist is None:
+            return None
+        if self.cov_full:
+            return self.dist[1:1 + self.nu * self.nu].view(self.nu, self.nu)
+        return self.dist[1:]
 
     @property
     def current_lambda(self):

@@ -36,6 +36,7 @@ class MPPIConfig:
     lambda_: float = 1.0
     update_lambda: bool = False
     update_cov: bool = False
+    cov_type: str = "diag"               # update rule of update_cov: diag | full (DESIGN.md section 2)
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0

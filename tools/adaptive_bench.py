@@ -1,12 +1,14 @@
 """Cost of adaptive MPPI (update_cov / update_lambda) on the device.
 
-1. K3 alone with and without the second-moment row (a registered distribution with update_cov), cold L2: inputs rotated over more
-   than twice the L2 size as bench.py's roofline sweep does, both variants alternated round by round in one process.
-2. The panda reach plan (config_panda_b200: K = 10 000, T = 30) with both flags on against both flags off, plans of the two planners
-   alternated in blocks, L2 flushed before every plan, CUDA-graph replay as in production.
+1. K3 alone without and with the second-moment row (a registered distribution with update_cov), and with the covariance row of
+   cov_type full, cold L2: inputs rotated over more than twice the L2 size as bench.py's roofline sweep does, the variants alternated
+   round by round in one process.  Panda (T = 30, nu = 7) and omnipanda (T = 30, nu = 12).
+2. The panda reach plan (config_panda_b200: K = 10 000, T = 30) with both flags off, with both flags on (diagonal rule) and with both
+   flags on and cov_type full, plans of the planners alternated in blocks, L2 flushed before every plan, CUDA-graph replay as in
+   production.
 
 Prints the card name and its power limit (read through NVML, nothing is changed) next to the numbers.
-    python tools/adaptive_bench.py [--ks 10000,65536,262144] [--rounds 5] [--plans 200]
+    python tools/adaptive_bench.py [--ks 10000,65536,262144] [--rounds 5] [--plans 200] [--scenes panda,omnipanda]
 """
 import argparse
 import json
@@ -53,22 +55,31 @@ def graph_time_us(fn, reps, replays=3):
     return best
 
 
-def k3_sweep(ks, rounds):
+def k3_sweep(ks, rounds, actors=("panda_stick", "goal")):
     from mppi_isaac_b200.backend import CudaBackend
     from mppi_isaac_b200.model.blob import OBS_DOF_STATE, build_scene, make_params
     from mppi_isaac_b200.utils.config_store import load_actor_cfgs, load_isaacgym_config
     cfg = load_isaacgym_config("config_panda_b200")
-    sc = build_scene(load_actor_cfgs(["panda_stick", "goal"]))
+    sc = build_scene(load_actor_cfgs(list(actors)))
     T, nu = int(cfg.mppi.horizon), sc.nu
     res = []
     for K in ks:
         bes = {}
-        for name, adaptive in (("fixed", False), ("second_moment", True)):
+        for name, adaptive in (("fixed", False), ("second_moment", True), ("full", True)):
             cfg.mppi.update_cov = cfg.mppi.update_lambda = adaptive
+            cfg.mppi.cov_type = "full" if name == "full" else "diag"
+            if np.asarray(cfg.mppi.noise_sigma).shape != (nu, nu):                # a scene other than the config's robot
+                cfg.mppi.noise_sigma = (0.1 * np.eye(nu)).tolist()
             p = make_params(cfg.mppi, cfg.isaacgym, nu, K, [(OBS_DOF_STATE, 0)])
             be = CudaBackend("cuda:0")
             be.create(sc.model, p)
-            if adaptive:
+            if name == "full":
+                L = 0.3 * np.eye(nu)
+                dist = torch.tensor(np.concatenate([[p.lambda_], (L @ L.T).ravel(), L.ravel(), np.linalg.inv(L @ L.T).ravel()]),
+                                    dtype=torch.float32, device="cuda:0")
+                be.set_distribution(dist)
+                bes[name] = (be, torch.zeros(be.partial_row_floats(), device="cuda:0"), dist)
+            elif adaptive:
                 dist = torch.tensor([p.lambda_] + [0.1] * nu, device="cuda:0")
                 be.set_distribution(dist)
                 bes[name] = (be, torch.zeros(2 + 2 * T * nu, device="cuda:0"), dist)
@@ -102,9 +113,10 @@ def plan_ab(plans, block=20):
     import copy
     q0 = [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]
     pls = {}
-    for name, on in (("flags_off", False), ("flags_on", True)):
+    for name, on in (("flags_off", False), ("flags_on", True), ("flags_on_full", True)):
         cfg = copy.deepcopy(load_isaacgym_config("config_panda_b200"))
         cfg.mppi.device, cfg.mppi.update_cov, cfg.mppi.update_lambda = "cuda:0", on, on
+        cfg.mppi.cov_type = "full" if name == "flags_on_full" else "diag"
         pl = MPPIisaacPlanner(cfg, PandaReachObjective(), use_cuda_graph=True)
         for _ in range(5):
             pl.compute_action(q0, [0.0] * 7)
@@ -124,6 +136,7 @@ def plan_ab(plans, block=20):
     out["graph_captured"] = {n: pl.mppi._graph is not None for n, pl in pls.items()}
     out["lambda_after"] = float(pls["flags_on"].mppi.current_lambda)
     out["cov_after"] = pls["flags_on"].mppi.cov_action.cpu().tolist()
+    out["sigma_after_full"] = pls["flags_on_full"].mppi.cov_action.cpu().tolist()
     return out
 
 
@@ -132,9 +145,12 @@ def main():
     ap.add_argument("--ks", default="10000,65536,262144")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--plans", type=int, default=200)
+    ap.add_argument("--scenes", default="panda,omnipanda")
     a = ap.parse_args()
     import __graft_entry__  # noqa: F401  (repository root on the path)
-    out = {"card": card(), "k3": k3_sweep([int(k) for k in a.ks.split(",")], a.rounds), "plan_c2": plan_ab(a.plans)}
+    scenes = {"panda": ("panda_stick", "goal"), "omnipanda": ("omnipanda", "goal")}
+    ks = [int(k) for k in a.ks.split(",")]
+    out = {"card": card(), "k3": [r for s in a.scenes.split(",") for r in k3_sweep(ks, a.rounds, scenes[s])], "plan_c2": plan_ab(a.plans)}
     print(json.dumps(out, indent=1))
 
 
