@@ -45,18 +45,33 @@ def _f(v):
     return " ".join(f"{x:.9g}" for x in np.atleast_1d(v))
 
 
-def robot_urdf(seed, nb, topology):
+def _collision(rng, kind):
+    """One <collision> element of the given kind (box / sphere / cylinder) at a random offset and rotation in its link frame."""
+    if kind == "box":
+        geom = f'<box size="{_f(rng.uniform(0.06, 0.2, 3))}"/>'
+    elif kind == "sphere":
+        geom = f'<sphere radius="{rng.uniform(0.04, 0.1):.9g}"/>'
+    else:
+        geom = f'<cylinder radius="{rng.uniform(0.03, 0.08):.9g}" length="{rng.uniform(0.08, 0.2):.9g}"/>'
+    return (f'<collision><origin xyz="{_f(rng.uniform(-0.05, 0.05, 3))}" rpy="{_f(rng.uniform(-np.pi, np.pi, 3))}"/>'
+            f'<geometry>{geom}</geometry></collision>')
+
+
+def robot_urdf(seed, nb, topology, collisions=None):
     """URDF text and the names of the fixed-joint link and the tip link.  Joint 1 is prismatic for even nb (the prismatic axis of a
     body on the base is rotated by the base pose), revolute for odd nb; the other joints are a random revolute / continuous /
-    prismatic mix."""
+    prismatic mix.  `collisions` ({link name: box | sphere | cylinder}) adds one collision primitive to each named link; its sizes
+    and poses come from an RNG stream of their own, so the rest of the URDF is the same with and without them."""
     assert topology in TOPOLOGIES and 1 <= nb <= 16 and (topology != "deep" or nb == 16)
     rng = np.random.default_rng([seed, nb, TOPOLOGIES.index(topology)])
+    col_rng = np.random.default_rng([seed, nb, TOPOLOGIES.index(topology), 2])
+    cols = {name: _collision(col_rng, kind) for name, kind in sorted((collisions or {}).items())}
     parents = _parents(rng, nb, topology)
     fixed_on = max(1, nb // 2)                   # link carrying the fixed-joint child "fx"; its child joints hang below "fx"
     light = max(1, nb - 1)                       # the light link (mass 1e-3)
     out = ['<robot name="synth">',
            f'<link name="l0"><inertial><origin xyz="{_f(rng.uniform(-0.05, 0.05, 3))}"/><mass value="3.0"/>'
-           '<inertia ixx="0.02" iyy="0.03" izz="0.04" ixy="0" ixz="0" iyz="0"/></inertial></link>']
+           f'<inertia ixx="0.02" iyy="0.03" izz="0.04" ixy="0" ixz="0" iyz="0"/></inertial>{cols.get("l0", "")}</link>']
 
     def inertial(m):
         d = rng.uniform(0.004, 0.04, 3) * m
@@ -65,7 +80,7 @@ def robot_urdf(seed, nb, topology):
 
     for i in range(1, nb + 1):
         m = 1e-3 if i == light else float(rng.uniform(0.3, 2.0))
-        out.append(f'<link name="l{i}">{inertial(m)}</link>')
+        out.append(f'<link name="l{i}">{inertial(m)}{cols.get(f"l{i}", "")}</link>')
         if i == 1:
             jt = "prismatic" if nb % 2 == 0 else "revolute"
         else:
@@ -79,7 +94,7 @@ def robot_urdf(seed, nb, topology):
         out.append(f'<joint name="j{i}" type="{jt}"><parent link="{par}"/><child link="l{i}"/>'
                    f'<origin xyz="{_f(rng.uniform(-0.15, 0.15, 3))}" rpy="{_f(rng.uniform(-np.pi, np.pi, 3))}"/><axis xyz="{_f(_unit(rng))}"/>'
                    f'{lim}<dynamics damping="{rng.uniform(0.05, 0.5):.9g}"/></joint>')
-    out.append(f'<link name="fx">{inertial(float(rng.uniform(0.2, 0.6)))}</link>')
+    out.append(f'<link name="fx">{inertial(float(rng.uniform(0.2, 0.6)))}{cols.get("fx", "")}</link>')
     out.append(f'<joint name="jfx" type="fixed"><parent link="l{fixed_on}"/><child link="fx"/>'
                f'<origin xyz="{_f(rng.uniform(-0.1, 0.1, 3))}" rpy="{_f(rng.uniform(-np.pi, np.pi, 3))}"/></joint>')
     out.append("</robot>")
@@ -87,12 +102,13 @@ def robot_urdf(seed, nb, topology):
 
 
 def make_robot(tmp_path, seed, nb, topology="chain", *, dof_mode="velocity", gravity=True, K=64, T=12, dt=0.02, substeps=1, u_lim=0.5,
-               base_pos=None, base_ori=None):
+               base_pos=None, base_ori=None, collisions=None, actors=(), obs=None):
     """Write the URDF to `tmp_path`, compile it into a one-robot scene and return (scene, params, state0).  The base pose is a random
     non-identity one unless given; state0 = (q, qd) with q inside the joint limits (a quarter of the range, at most 0.3, from a stop) and
-    small random qd."""
-    text, fixed_link, tip = robot_urdf(seed, nb, topology)
-    fn = f"synth_{topology}{nb}_s{seed}.urdf"
+    small random qd.  `collisions` (see robot_urdf) gives links collision geometry and builds the robot actor with collision on;
+    `actors` are further actors of the scene and `obs(scene)`, if given, returns the observation items instead of the default ones."""
+    text, fixed_link, tip = robot_urdf(seed, nb, topology, collisions)
+    fn = f"synth_{topology}{nb}_s{seed}{'_col' if collisions else ''}.urdf"
     with open(os.path.join(str(tmp_path), fn), "w") as f:
         f.write(text)
     rng = np.random.default_rng([seed, nb, TOPOLOGIES.index(topology), 1])
@@ -102,11 +118,14 @@ def make_robot(tmp_path, seed, nb, topology="chain", *, dof_mode="velocity", gra
         qb = rng.normal(size=4)
         base_ori = (np.sign(qb[3]) * qb / np.linalg.norm(qb)).tolist()
     actor = ActorWrapper(type="robot", name="synth", urdf_file=fn, fixed=True, init_pos=list(base_pos), init_ori=list(base_ori),
-                         dof_mode=dof_mode, gravity=gravity, collision=False)
-    sc = build_scene([actor], assets_dirs=[str(tmp_path)], substep=dt / substeps)
-    assert sc.ndof == nb and sc.model.nfree == 0 and sc.model.nshapes == 0
+                         dof_mode=dof_mode, gravity=gravity, collision=bool(collisions))
+    sc = build_scene([actor] + list(actors), assets_dirs=[str(tmp_path)], substep=dt / substeps)
+    assert sc.ndof == nb and (actors or (sc.model.nfree == 0 and sc.model.nshapes == 0))
     names = sc.robot.link_names
-    obs = [(OBS_LINK_STATE, names.index("l0")), (OBS_LINK_STATE, names.index(fixed_link)), (OBS_LINK_STATE, names.index(tip)), (OBS_DOF_STATE, 0)]
+    if obs is not None:
+        obs = obs(sc)
+    else:
+        obs = [(OBS_LINK_STATE, names.index("l0")), (OBS_LINK_STATE, names.index(fixed_link)), (OBS_LINK_STATE, names.index(tip)), (OBS_DOF_STATE, 0)]
     mc = MPPIConfig(num_samples=K, horizon=T, mppi_mode="simple", sampling_method="random", noise_sigma=(0.1 * np.eye(sc.nu)).tolist(),
                     u_min=[-u_lim], u_max=[u_lim], lambda_=0.05, sample_null_action=True)
     p = make_params(mc, IsaacGymConfig(dt=dt, substeps=substeps), sc.nu, K, obs)
