@@ -37,6 +37,7 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     MPPIB_REQUIRE(p->K >= 1, "K=%d must be positive", p->K);     // K % 4 == 0 is a requirement of the reduction only (checked there)
     MPPIB_REQUIRE(p->T >= 1 && p->substeps >= 1 && p->dt > 0.f, "bad T/substeps/dt");
     MPPIB_REQUIRE(p->lambda_ > 0.f, "lambda must be positive");
+    MPPIB_REQUIRE(isfinite(p->gamma) && p->gamma >= 0.f, "gamma = %g must be finite and >= 0 (rollout_var_discount)", p->gamma);
     MPPIB_REQUIRE(!(p->filter_u && p->T < 9), "filter_u needs T >= 9");
     MPPIB_REQUIRE(p->nobs >= 0 && p->nobs <= MPPIB_MAX_OBS, "nobs out of range");
     if (p->update_cov || p->update_lambda)

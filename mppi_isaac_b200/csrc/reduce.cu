@@ -436,8 +436,9 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         g[r] = acc;
     }
     {
+        // gamma^0 = 1 for every accepted gamma: log2f(0) * 0 would be NaN (validate refuses a negative or non-finite gamma)
         const float lg = log2f(p.gamma);
-        for (int t = tid; t < T4; t += NT) gp[t] = t < T ? exp2f(lg * (float)t) : 0.f;
+        for (int t = tid; t < T4; t += NT) gp[t] = t == 0 ? 1.f : t < T ? exp2f(lg * (float)t) : 0.f;
     }
     __syncthreads();
 

@@ -379,6 +379,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         p.mode, p.gamma = MODE_MEAN, float(mppi_cfg.rollout_var_discount)
     else:
         raise ValueError(f"unknown mppi_mode {mode}")
+    if not (math.isfinite(p.gamma) and p.gamma >= 0.0):     # gamma = 0 is legal: score only the first step
+        raise ValueError(f"rollout_var_discount = {p.gamma} must be finite and >= 0")
     p.lambda_ = float(mppi_cfg.lambda_)
     p.step_size_mean = 0.98
     # adaptive MPPI (DESIGN.md section 2): the two flags and the eta bounds are config keys, the step sizes are constants
