@@ -386,6 +386,25 @@ __device__ __forceinline__ uint32_t partner_mask(const MppibModel& m, int a) {
     return mask;
 }
 
+// Ground points of a free box (oracle.cpp ContactWorld::detect): bit c is set if corner c is among the 4 lowest of the 8 (ties by
+// corner index) and below the ground margin; z[c] is the same expression as the corner's pt.z.  With at most 4 corners below the
+// margin those are the answer (a corner below it has only corners below it beneath it): the ranks are needed only above h ~ 0.026 s.
+__device__ __forceinline__ uint32_t ground_corner_mask(const float (&z)[8], float margin) {
+    uint32_t below = 0;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) below |= (uint32_t)(z[c] < margin) << c;
+    if (__popc(below) <= 4) return below;
+    uint32_t keep = 0;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        int rank = 0;
+#pragma unroll
+        for (int o = 0; o < 8; ++o) rank += z[o] < z[c] || (z[o] == z[c] && o < c);
+        if (rank < 4) keep |= 1u << c;
+    }
+    return keep & below;
+}
+
 __device__ __forceinline__ int detect(const MppibModel& m, const Layout& L, float* xs, int lane, const uint32_t* __restrict__ bmask) {
     int nc = 0;
     const int ns = m.nshapes;
@@ -395,11 +414,18 @@ __device__ __forceinline__ int detect(const MppibModel& m, const Layout& L, floa
         if (m.ground_plane) {
             const M3 Ra = ldxM3(xs, sa + SH_R, lane); const V3 ca = ldx3(xs, sa + SH_C, lane), ha = ldx3(xs, sa + SH_HALF, lane);
             const float mu = 0.5f * (XS(sa + SH_MU) + m.ground_friction);
+            float z[8];                                               // at most the 4 lowest corners are ground points
+#pragma unroll
+            for (int idx = 0; idx < 8; ++idx) {
+                const int ix = (idx >> 2) * 2 - 1, iy = ((idx >> 1) & 1) * 2 - 1, iz = (idx & 1) * 2 - 1;
+                z[idx] = (mul(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca).z;
+            }
+            const uint32_t keep = ground_corner_mask(z, m.ground_margin);
 #pragma unroll 1
             for (int idx = 0; idx < 8; ++idx) {
                 const int ix = (idx >> 2) * 2 - 1, iy = ((idx >> 1) & 1) * 2 - 1, iz = (idx & 1) * 2 - 1;
                 const V3 pt = mul(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
-                if (pt.z < m.ground_margin) add_contact(m, L, xs, lane, nc, shape_ref(m, a), REF_STATIC, m.shape_slot[a], -1, pt, mk(0, 0, 1), -pt.z, mu);
+                if ((keep >> idx) & 1u) add_contact(m, L, xs, lane, nc, shape_ref(m, a), REF_STATIC, m.shape_slot[a], -1, pt, mk(0, 0, 1), -pt.z, mu);
             }
         }
         for (uint32_t mask = bmask[a]; mask; mask &= mask - 1) {          // partners in ascending order, as the oracle's loop visits them

@@ -599,12 +599,22 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
             if (m.ground_plane) {
                 const M3 Ra = ldM3(xs, sa + SH_R); const V3 ca = ld3(xs, sa + SH_C), ha = ld3(xs, sa + SH_HALF);
                 const float mu = 0.5f * (xs[sa + SH_MU] + m.ground_friction);
-                for (int i0 = 0; i0 < 8; i0 += GC) {
-                    const int idx = i0 + ic;
-                    const int ix = (idx >> 2) * 2 - 1, iy = ((idx >> 1) & 1) * 2 - 1, iz = (idx & 1) * 2 - 1;
-                    const V3 pt = mulM(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
-                    append(idx < 8 && pt.z < m.ground_margin, shape_ref(m, a), REF_STATIC, m.shape_slot[a], -1, pt, mk(0.f, 0.f, 1.f), -pt.z, mu);
+                // lane = corner; at most the 4 lowest corners (ties by corner index) are ground points (contact.cuh ground_corner_mask):
+                // with more than 4 below the margin (h above ~0.026 s) the lanes rank their heights by shuffles
+                static_assert(GC >= 8, "one corner per lane");
+                const int idx = ic;
+                const int ix = (idx >> 2) * 2 - 1, iy = ((idx >> 1) & 1) * 2 - 1, iz = (idx & 1) * 2 - 1;
+                const V3 pt = mulM(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
+                bool hit = idx < 8 && pt.z < m.ground_margin;
+                if (__any_sync(FULL, __popc(team_ballot<GC>(hit, tbc)) > 4)) {          // warp-uniform
+                    int rank = 0;
+                    for (int o = 0; o < 8; ++o) {
+                        const float zo = __shfl_sync(FULL, pt.z, o, GC);
+                        rank += zo < pt.z || (zo == pt.z && o < idx);
+                    }
+                    hit = hit && rank < 4;
                 }
+                append(hit, shape_ref(m, a), REF_STATIC, m.shape_slot[a], -1, pt, mk(0.f, 0.f, 1.f), -pt.z, mu);
             }
             pairs_of(a);
         }

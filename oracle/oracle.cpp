@@ -569,11 +569,20 @@ struct ContactWorld {
         for (int a = 0; a < ns; ++a) {
             if (sh[a].kind != MPPIB_OWNER_FREE) continue;
             if (m->ground_plane) {
+                // at most the 4 lowest corners (ties by corner index) are ground points: a box resting flat, on an edge or on a corner
+                // is carried by those, the higher ones only have a gap (a speculative row with no impulse) and would use up the cap
+                // when the margin 1.5 g h^2 exceeds the box's height (h = 0.1 s: 14.7 cm)
                 const S mu = (S)0.5 * (sh[a].mu + (S)m->ground_friction);
-                for (int ix = -1; ix <= 1; ix += 2) for (int iy = -1; iy <= 1; iy += 2) for (int iz = -1; iz <= 1; iz += 2) {
-                    S loc[3] = {ix * sh[a].half[0], iy * sh[a].half[1], iz * sh[a].half[2]}, pt[3];
-                    mat_vec(sh[a].R, loc, pt); for (int i = 0; i < 3; ++i) pt[i] += sh[a].c[i];
-                    if (pt[2] < (S)m->ground_margin) { S n[3] = {0, 0, 1}; add_contact(sh[a].ref, REF_STATIC, sh[a].slot, -1, pt, n, -pt[2], mu, 0); }
+                S pts[8][3];
+                for (int c = 0; c < 8; ++c) {
+                    const int ix = (c >> 2) * 2 - 1, iy = ((c >> 1) & 1) * 2 - 1, iz = (c & 1) * 2 - 1;
+                    S loc[3] = {ix * sh[a].half[0], iy * sh[a].half[1], iz * sh[a].half[2]};
+                    mat_vec(sh[a].R, loc, pts[c]); for (int i = 0; i < 3; ++i) pts[c][i] += sh[a].c[i];
+                }
+                for (int c = 0; c < 8; ++c) {
+                    int rank = 0;
+                    for (int o = 0; o < 8; ++o) rank += pts[o][2] < pts[c][2] || (pts[o][2] == pts[c][2] && o < c);
+                    if (rank < 4 && pts[c][2] < (S)m->ground_margin) { S n[3] = {0, 0, 1}; add_contact(sh[a].ref, REF_STATIC, sh[a].slot, -1, pts[c], n, -pts[c][2], mu, 0); }
                 }
             }
             for (int b = 0; b < ns; ++b) {

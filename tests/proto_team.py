@@ -263,10 +263,19 @@ def _one_substep(p):
 
 
 
+def ground_corners(R, c, half, margin):
+    """Ground points of a box (rotation R, centre c), in corner-index order: the corners among the 4 lowest of the 8 (ties by corner
+    index) that lie below `margin`."""
+    pts = [R @ (np.array([ix, iy, iz]) * half) + c for ix in (-1, 1) for iy in (-1, 1) for iz in (-1, 1)]
+    z = [p[2] for p in pts]
+    rank = [sum(z[o] < z[k] or (z[o] == z[k] and o < k) for o in range(8)) for k in range(8)]
+    return [pts[k] for k in range(8) if rank[k] < 4 and z[k] < margin]
+
+
 # ------------------------------------------------------------------------------------------------------------------------------
 # The contact solve of rollout_team.cu in GENERALISED COORDINATES, for the part that is new against the oracle: a free body's three
 # linear velocity components (world) and three angular velocity components IN BODY AXES, one scalar inverse inertia each, contact rows
-# cached once per substep.  Case: a free box on the ground plane (up to 8 corner contacts), one model step of the heijn_push scene with
+# cached once per substep.  Case: a free box on the ground plane (up to 4 corner contacts), one model step of the heijn_push scene with
 # the robot far away -- the oracle solves it with world-frame inverse inertia tensors and point velocities.
 def free_box_step(m, p, box_state, f=0):
     """One model step of free body f alone on the ground (no other contact partner in reach); box_state = its 13 root-state numbers.
@@ -287,13 +296,7 @@ def free_box_step(m, p, box_state, f=0):
         R = q2R(qt)
         sq, sp = np.array(m.shape_quat[shape][:], float), np.array(m.shape_pos[shape][:], float)
         Rs, cs = R @ q2R(sq), x + R @ sp
-        contacts = []
-        for ix in (-1, 1):
-            for iy in (-1, 1):
-                for iz in (-1, 1):
-                    pt = Rs @ (np.array([ix, iy, iz]) * half) + cs
-                    if pt[2] < float(m.ground_margin):
-                        contacts.append((pt, -pt[2]))
+        contacts = [(pt, -pt[2]) for pt in ground_corners(Rs, cs, half, float(m.ground_margin))]
         if m.free_gravity[f]:
             v = v + h * g
         u = np.concatenate([v, R.T @ w])                                       # generalised velocities: world linear, BODY-axis angular
@@ -445,12 +448,8 @@ def make_contact_phase(m, p, root0, free):
                 continue
             if m.ground_plane:
                 mu = 0.5 * (mu_s[a] + float(m.ground_friction))
-                for ix in (-1, 1):
-                    for iy in (-1, 1):
-                        for iz in (-1, 1):
-                            pt = Rs[a] @ (np.array([ix, iy, iz]) * half[a]) + cs[a]
-                            if pt[2] < float(m.ground_margin):
-                                add(ref(a), None, pt, [0, 0, 1.0], -pt[2], mu)
+                for pt in ground_corners(Rs[a], cs[a], half[a], float(m.ground_margin)):
+                    add(ref(a), None, pt, [0, 0, 1.0], -pt[2], mu)
             for b in range(ns):
                 if b == a or ref(b) == ref(a) or (kind[b] == 2 and b < a):
                     continue

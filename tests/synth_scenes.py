@@ -119,8 +119,9 @@ def _link_shapes_world(sc, q):
     return out
 
 
-def _free_rows(scenario, f, fb, rng, link_world, rot_quat, rot_half):
-    """(13,) root-state row of free box f (half extents fb[f]) in `scenario`."""
+def _free_rows(scenario, f, fb, rng, link_world, rot_quat, rot_half, lift=0.0):
+    """(13,) root-state row of free box f (half extents fb[f]) in `scenario`.  `lift`: how far the ground margin exceeds its 1 cm floor
+    (1.5 g h^2 - 0.01 above h = 0.026 s); a falling box starts that much higher, so that it keeps its clearance above the margin."""
     half = fb[f]
     spot = np.array([6.0, -6.0 + 1.5 * f])                           # a spot of its own on the ground for every box
     v, w = rng.uniform(-0.05, 0.05, 3), rng.uniform(-0.1, 0.1, 3)
@@ -151,7 +152,7 @@ def _free_rows(scenario, f, fb, rng, link_world, rot_quat, rot_half):
         x = c + d / np.linalg.norm(d) * (r + half.min() - 0.01)
         v = -0.2 * d / np.linalg.norm(d)
     elif scenario == "falling":
-        x = np.array([spot[0], spot[1], 0.2 + rng.uniform(0.0, 0.4)])
+        x = np.array([spot[0], spot[1], 0.2 + lift + rng.uniform(0.0, 0.4)])
         v, w = np.array([0.0, 0.0, -1.0]) + rng.uniform(-0.5, 0.5, 3), rng.uniform(-4, 4, 3)
         quat = _random_quat(rng)
     elif scenario == "far":
@@ -170,12 +171,12 @@ def _free_rows(scenario, f, fb, rng, link_world, rot_quat, rot_half):
 
 
 def make_contact_scene(tmp_path, seed, nb, topology, nfree, *, statics=2, static_spheres=1, link_shapes=3, link_spheres=1, noise=False,
-                       max_contacts=None, K=64, T=8, dt=0.02, substeps=2, gravity_off=True):
+                       max_contacts=None, K=64, T=8, dt=0.02, substeps=2, gravity_off=True, dof_mode="velocity"):
     """One generated contact scene: (scene, params, state (NS, K), root0 (A, 13)).  The robot gets `link_shapes` collision primitives
     (the root link's box, `link_spheres` spheres, the rest boxes and cylinders); free box f > 0 has gravity off if `gravity_off` and f is
     odd.  Static boxes: the ramp, a randomly rotated box, and the rest (like the static spheres) overlapping link shapes at the starting
-    joint positions.  `max_contacts` lowers the model's contact cap (on a copy of the model) so that it binds often.  Observed: the DOF
-    state, every free body, every contact slot."""
+    joint positions.  `max_contacts` lowers the model's contact cap (on a copy of the model) so that it binds often.  `dof_mode` is the
+    robot's drive (velocity, or effort: torque commands).  Observed: the DOF state, every free body, every contact slot."""
     assert 0 <= nfree <= 4 and statics >= 2 and 1 <= link_shapes <= nb + 1
     rng = np.random.default_rng([seed, nb, TOPOLOGIES.index(topology), nfree, 3])
     links = ["l0"] + [f"l{i}" for i in sorted(rng.choice(np.arange(1, nb + 1), link_shapes - 1, replace=False))]
@@ -214,7 +215,7 @@ def make_contact_scene(tmp_path, seed, nb, topology, nfree, *, statics=2, static
         return ([(OBS_DOF_STATE, 0)] + [(OBS_FREE_STATE, f) for f in range(sc.model.nfree)]
                 + [(OBS_CONTACT, s) for s in range(sc.model.ncontact_slots)])
     sc, p, s0 = make_robot(tmp_path, seed, nb, topology, K=K, T=T, dt=dt, substeps=substeps, base_pos=base_pos, collisions=collisions,
-                           actors=actors, obs=obs)
+                           actors=actors, obs=obs, dof_mode=dof_mode)
     m = sc.model
     assert m.nfree == nfree and m.nshapes == nfree + statics + static_spheres + link_shapes and m.nshapes <= 24 and m.max_contacts >= 12
     if max_contacts is not None:
@@ -226,10 +227,11 @@ def make_contact_scene(tmp_path, seed, nb, topology, nfree, *, statics=2, static
     st[:nb] = np.clip(s0[:nb, None] + rng.uniform(-0.03, 0.03, (nb, K)), lo[:, None], hi[:, None])
     st[nb:2 * nb] = rng.uniform(-0.3, 0.3, (nb, K))
     root0 = sc.root_state0.copy()
+    lift = max(0.0, float(m.ground_margin) - 0.01)
     for k in range(K):
         scen = SCENARIOS[k % len(SCENARIOS)]
         for f in range(nfree):
-            st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1), k] = _free_rows(scen, f, fb, rng, link_world, rot_quat, rot_half)
+            st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1), k] = _free_rows(scen, f, fb, rng, link_world, rot_quat, rot_half, lift)
     for f in range(nfree):                                  # the broadcast starting rows of the free bodies: resting on the ground
         root0[m.free_actor[f]] = _free_rows("ground", f, fb, rng, link_world, rot_quat, rot_half).astype(np.float32)
     return sc, p, st.astype(np.float32), root0
@@ -259,9 +261,9 @@ def _aside_robot(tmp_path, actors, K, T, dt, substeps):
     return sc, p, s0
 
 
-def cube_collision_scene(tmp_path, seed, ncubes, K=8, T=30, dt=0.02, substeps=2):
-    """2-4 free cubes, gravity off, no ground, no randomisation, sent into one another with random velocities and spins: the
-    contacts are the only forces.  Returns (scene, params, state (NS, K), masses, half sizes)."""
+def cube_collision_scene(tmp_path, seed, ncubes, K=8, T=30, dt=0.02, substeps=2, speed=1.0):
+    """2-4 free cubes, gravity off, no ground, no randomisation, sent into one another with random velocities and spins (scaled by
+    `speed`): the contacts are the only forces.  Returns (scene, params, state (NS, K), masses, half sizes)."""
     rng = np.random.default_rng([seed, ncubes, 11])
     h = rng.uniform(0.05, 0.12, ncubes)
     mass = rng.uniform(0.3, 2.0, ncubes)
@@ -280,7 +282,7 @@ def cube_collision_scene(tmp_path, seed, ncubes, K=8, T=30, dt=0.02, substeps=2)
             d /= np.linalg.norm(d)
             x = centre + d * rng.uniform(0.15, 0.35)
             v = (centre - x) / np.linalg.norm(centre - x) * rng.uniform(1.0, 3.0) + rng.uniform(-0.3, 0.3, 3)
-            st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1), k] = np.concatenate([x, _random_quat(rng), v, rng.uniform(-5, 5, 3)])
+            st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1), k] = np.concatenate([x, _random_quat(rng), speed * v, speed * rng.uniform(-5, 5, 3)])
     return sc, p, st.astype(np.float32), mass, h
 
 
@@ -301,6 +303,26 @@ def stack_scene(tmp_path, seed, nboxes, K=4, T=60, dt=0.02, substeps=4):
         row = np.concatenate([[5.0, 0.0, z + half[f][2]], [0, 0, 0, 1.0], np.zeros(6)])
         st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1)] = row[:, None]
         z += 2 * half[f][2]
+    return sc, p, st, mass
+
+
+def resting_boxes_scene(tmp_path, seed, nboxes, K=4, T=50, dt=0.1, substeps=1, max_contacts=None):
+    """`nboxes` boxes of 16 x 14 x 10 cm and 1.0 - 1.6 kg flat on the ground, 0.6 m apart, at rest, no randomisation; `max_contacts`
+    lowers the contact cap on a copy of the model.  Returns (scene, params, state, masses)."""
+    rng = np.random.default_rng([seed, nboxes, 13])
+    half = np.array([0.08, 0.07, 0.05])
+    mass = rng.uniform(1.0, 1.6, nboxes)
+    actors = [ActorWrapper(type="box", name=f"box{f}", size=(2 * half).tolist(), mass=float(mass[f]), friction=float(rng.uniform(0.5, 1.0)),
+                           fixed=False, init_pos=[5.0, 0.6 * f, half[2]]) for f in range(nboxes)]
+    sc, p, s0 = _aside_robot(tmp_path, actors, K, T, dt, substeps)
+    if max_contacts is not None:
+        sc.model = copy.deepcopy(sc.model)
+        sc.model.max_contacts = int(max_contacts)
+    nb = sc.ndof
+    st = np.zeros((2 * nb + 13 * nboxes, K), np.float32)
+    st[:nb] = s0[:nb, None]
+    for f in range(nboxes):
+        st[2 * nb + 13 * f: 2 * nb + 13 * (f + 1)] = np.concatenate([[5.0, 0.6 * f, half[2]], [0, 0, 0, 1.0], np.zeros(6)])[:, None]
     return sc, p, st, mass
 
 
@@ -332,13 +354,13 @@ SLIDER_URDF = """<robot name="slider">
 """
 
 
-def slider_scene(tmp_path, r=0.1, face=0.6, effort=1000.0, K=4, T=100, dt=0.02, substeps=2):
-    """A one-joint prismatic robot (velocity drive along world x) whose link is a sphere of radius r, and a static box whose -x face
-    is at x = face.  Returns (scene, params, state0)."""
+def slider_scene(tmp_path, r=0.1, face=0.6, effort=1000.0, K=4, T=100, dt=0.02, substeps=2, dof_mode="velocity"):
+    """A one-joint prismatic robot (a velocity or effort drive along world x) whose link is a sphere of radius r, and a static box
+    whose -x face is at x = face.  Returns (scene, params, state0)."""
     fn = "slider.urdf"
     with open(os.path.join(str(tmp_path), fn), "w") as f:
         f.write(SLIDER_URDF.format(r=r, effort=effort))
-    robot = ActorWrapper(type="robot", name="slider", urdf_file=fn, fixed=True, init_pos=[0.0, 0.0, 0.3], dof_mode="velocity", collision=True)
+    robot = ActorWrapper(type="robot", name="slider", urdf_file=fn, fixed=True, init_pos=[0.0, 0.0, 0.3], dof_mode=dof_mode, collision=True)
     wall = ActorWrapper(type="box", name="wall", size=[0.4, 0.6, 0.6], fixed=True, init_pos=[face + 0.2, 0.0, 0.3])
     sc = build_scene([robot, wall], assets_dirs=[str(tmp_path)], substep=dt / substeps)
     obs = [(OBS_DOF_STATE, 0)] + [(OBS_CONTACT, s) for s in range(sc.model.ncontact_slots)]

@@ -229,16 +229,30 @@ def test_full_plan_parity_through_planner_api(robot):
     assert float((rg.cpu() - rc).abs().max()) <= 1e-3
 
 
-def test_stepwise_protocol_on_gpu_matches_batched():
+def _stepwise_matches_batched(mk, obj, q):
     from mppi_isaac_b200 import MPPIisaacPlanner
-    from mppi_isaac_b200.objectives import PandaReachObjective
-    q = [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]
-    a = MPPIisaacPlanner(panda_cfg(K=256, T=12, device=DEV), PandaReachObjective(), rollout_mode="batched", use_cuda_graph=False)
-    b = MPPIisaacPlanner(panda_cfg(K=256, T=12, device=DEV), PandaReachObjective(), rollout_mode="stepwise")
+    a = MPPIisaacPlanner(mk(), obj(), rollout_mode="batched", use_cuda_graph=False)
+    b = MPPIisaacPlanner(mk(), obj(), rollout_mode="stepwise")
     for it in range(3):
-        ua, ub = a.compute_action(q, [0] * 7), b.compute_action(q, [0] * 7)
+        ua, ub = a.compute_action(q, [0] * len(q)), b.compute_action(q, [0] * len(q))
         assert float((ua - ub).abs().max()) <= 1e-6
     assert torch.equal(a.mppi.actions, b.mppi.actions)
+
+
+def test_stepwise_protocol_on_gpu_matches_batched():
+    from mppi_isaac_b200.objectives import PandaReachObjective
+    _stepwise_matches_batched(lambda: panda_cfg(K=256, T=12, device=DEV), PandaReachObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0])
+
+
+@pytest.mark.parametrize("config", ["push", "boxer"])
+def test_stepwise_protocol_on_gpu_matches_batched_with_contacts(config):
+    """The planner's stepwise path against its batched one on the contact scenes of configs C4 (push, h = 0.1 s) and C3 (the boxer's
+    planar base, h = 0.1 s)."""
+    from mppi_isaac_b200.objectives import PushObjective
+    if config == "push":
+        _stepwise_matches_batched(lambda: push_cfg(K=256, T=10, device=DEV), PushObjective, [0.0, 0.0, 0.0])
+    else:
+        _stepwise_matches_batched(lambda: boxer_cfg(K=256, T=12, device=DEV), lambda: PushObjective(robot="boxer", link="ee_link"), [0.0, 2.5, 0.0])
 
 
 # ---------------------------------------------------------------------------------------------------------------
