@@ -38,6 +38,10 @@
  *                               registered distribution
  *   dist     [1 + nu]           (lambda, cov[nu]) live sampling distribution of adaptive MPPI (mppib_set_distribution);
  *            [1 + 3*nu*nu]      (lambda, Sigma[nu][nu], L[nu][nu], Sigma^-1[nu][nu]) with cov_full, all row-major, L lower
+ *            [1 + 3*n*n]        (lambda, Sigma_H[n][n], L_H[n][n], Sigma_H^-1[n][n]) with cov_horizon, n = T*nu, the same layout
+ *                               over the whole control sequence, vectors ordered (t, j) like U
+ *   partial  [2 + n + n(n+1)/2] (beta_g, eta_g, W_g, C_g[lower triangle of n x n]) with update_cov, cov_horizon and a registered
+ *                               distribution
  */
 #ifndef MPPIB_H
 #define MPPIB_H
@@ -48,7 +52,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 15
+#define MPPIB_ABI_VERSION 16
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -206,6 +210,8 @@ typedef struct MppibParams {
     float   kappa;
     float   lambda_mult;
     int32_t cov_full;          /* with update_cov: adapt a full Sigma (K1 draws L z, K3 appends C, K4 updates Sigma, L, Sigma^-1) */
+    int32_t cov_horizon;       /* with update_cov: adapt one Sigma_H over the whole sequence, n = T*nu <= 256 (not with cov_full) */
+    float   sigma0[MPPIB_MAX_NU * MPPIB_MAX_NU];    /* cov_horizon: Sigma0 = noise_sigma, row major nu x nu, the block a shift appends */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -259,6 +265,10 @@ int32_t mppib_rollout(MppibHandle h, const float* state0, const float* root0, fl
  * M2_g[t][j] = sum_k w_k (x[t][j][k] - c[t][j])^2, c = U (MEAN) or 0 (SIMPLE).  With cov_full too, Sigma^-1 is the full one of
  * the buffer and the row carries C_g = sum_t sum_k w_k (x_tk - c_t)(x_tk - c_t)^T instead of M2_g, packed as its lower triangle
  * (i >= j, row-major, nu(nu+1)/2 floats); row length 2 + T*nu + nu(nu+1)/2.
+ * With cov_horizon instead, n = T*nu: the SIMPLE-mode term is g^T x_k with g = lambda Sigma_H^-1 U computed by the last
+ * mppib_shift, K3 stores every S_k in a handle-owned buffer, and a second kernel of this call (a weighted SYRK, tiled over the
+ * lower triangle and split over K, folded in a fixed order) appends C_g = sum_k w_k (x_k - c)(x_k - c)^T over the whole
+ * n-vector x_k, packed as its lower triangle; row length 2 + n + n(n+1)/2.
  * Single pass over HBM; the last CTA to finish folds the per-CTA partials.                  */
 int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const float* U,
                      float* partial, void* stream);
@@ -279,7 +289,8 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
  * Replaces the all-gather between K3 and K4 (the reference has no multi-GPU path; this is the
  * multi-GPU scale-out of its single-GPU mppi_torch reduction, SURVEY.md 8(e)).  Every rank owns a small
  * WINDOW in its HBM: [2 parities][world] rows of 2 + T*nu floats (2 + 2*T*nu with update_cov, 2 + T*nu + nu(nu+1)/2 with
- * update_cov and cov_full; rounded up to a multiple of 4) plus one arrival flag per row.
+ * update_cov and cov_full, 2 + n + n(n+1)/2 with update_cov and cov_horizon; rounded up to a multiple of 4) plus one arrival flag
+ * per row.  With cov_horizon the row is complete only after the SYRK, so its last CTA stores it into the windows.
  * With peers open, the last CTA of mppib_reduce stores this rank's (beta, eta, W) row straight
  * into the window of EVERY rank over NVLink (st.global + fence.sys + st.release.sys of the flag),
  * and mppib_finalize (called with partials == NULL) spins on its own window's flags
@@ -337,11 +348,17 @@ int32_t mppib_set_action_mirror(MppibHandle h, float* mirror);
  * L the lower Cholesky factor of Sigma (zero above the diagonal), all three consistent at registration.  K1 draws noise = L z
  * (the library sampler colours the white library by L), K3 uses the full Sigma^-1 in SIMPLE mode and appends C, and K4 updates
  * Sigma, then L and Sigma^-1 on the device; a non-positive-definite update leaves the three as they were.  The partial rows
- * are [2 + T*nu + nu(nu+1)/2].                                                                                              */
+ * are [2 + T*nu + nu(nu+1)/2].
+ * With update_cov and cov_horizon the buffer is dist[1 + 3*n*n] = (lambda, Sigma_H, L_H, Sigma_H^-1), n = T*nu, the same layout
+ * over the whole control sequence.  K1 draws noise = L_H z over the n-vector of a sample, K3 reads lambda Sigma_H^-1 U from
+ * mppib_shift in SIMPLE mode, the SYRK appends C, and K4 updates Sigma_H, shifts it by one step like U (the appended block is
+ * sigma0), then factors it in one CTA; a non-positive-definite result leaves the three as they were.  The partial rows are
+ * [2 + n + n(n+1)/2].                                                                                                       */
 int32_t mppib_set_distribution(MppibHandle h, float* dist);
 
 /* shift U by one step: U[t] <- U[t+1], U[T-1] <- u_init (mppi_torch command() prologue);
- * increments *plan_ctr (device, nullable) by one.                                            */
+ * increments *plan_ctr (device, nullable) by one.  With update_cov, cov_horizon and a registered distribution it also computes
+ * g = lambda Sigma_H^-1 U of the shifted U once per plan, which K3 reads in SIMPLE mode.                                     */
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
 
 #ifdef __cplusplus

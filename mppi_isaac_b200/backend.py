@@ -180,24 +180,37 @@ class CudaBackend:
     def _cov_full(self):
         return bool(self.params.update_cov) and bool(self.params.cov_full)
 
+    def _cov_horizon(self):
+        return bool(self.params.update_cov) and bool(self.params.cov_horizon)
+
     def partial_row_floats(self) -> int:
-        """Floats of one shard row K3 writes with a registered distribution: 2 + T*nu, + T*nu with update_cov, or + nu(nu+1)/2
-        with update_cov and cov_full."""
+        """Floats of one shard row K3 writes with a registered distribution: 2 + T*nu, + T*nu with update_cov, + nu(nu+1)/2
+        with update_cov and cov_full, or + n(n+1)/2 with update_cov and cov_horizon (n = T*nu)."""
         T, nu = int(self.params.T), int(self.model.nu)
+        if self._cov_horizon():
+            n = T * nu
+            return 2 + n + n * (n + 1) // 2
         if self._cov_full():
             return 2 + T * nu + nu * (nu + 1) // 2
         return 2 + T * nu * (2 if self.params.update_cov else 1)
 
     def _check_row(self, rows, what):
-        if self._cov_full() and self._dist_keepalive is not None and rows is not None and rows.shape[-1] != self.partial_row_floats():
-            raise RuntimeError(f"{what}: cov_full shard rows hold {self.partial_row_floats()} floats, got {rows.shape[-1]}")
+        if ((self._cov_full() or self._cov_horizon()) and self._dist_keepalive is not None and rows is not None
+                and rows.shape[-1] != self.partial_row_floats()):
+            kind = "cov_horizon" if self._cov_horizon() else "cov_full"
+            raise RuntimeError(f"{what}: {kind} shard rows hold {self.partial_row_floats()} floats, got {rows.shape[-1]}")
 
     def set_distribution(self, dist):
         """Adaptive MPPI: register the device tensor (lambda, cov[nu]) -- with cov_full (lambda, Sigma, L, Sigma^-1), 1 + 3 nu^2
-        floats -- that K1 / K3 read and K4 updates (None switches it off)."""
+        floats, with cov_horizon (lambda, Sigma_H, L_H, Sigma_H^-1), 1 + 3 n^2 floats, n = T*nu -- that K1 / K3 read and K4 updates
+        (None switches it off)."""
         if dist is not None and self._cov_full() and dist.numel() != 1 + 3 * self.model.nu ** 2:
             raise RuntimeError(f"mppib_set_distribution: cov_full needs (lambda, Sigma, L, Sigma^-1) = {1 + 3 * self.model.nu ** 2} floats, "
                                f"got {dist.numel()}")
+        n = int(self.params.T) * int(self.model.nu)
+        if dist is not None and self._cov_horizon() and dist.numel() != 1 + 3 * n * n:
+            raise RuntimeError(f"mppib_set_distribution: cov_horizon needs (lambda, Sigma_H, L_H, Sigma_H^-1) = {1 + 3 * n * n} floats "
+                               f"(n = T*nu = {n}), got {dist.numel()}")
         self._dist_keepalive = dist
         self._check(self.lib.mppib_set_distribution(self.handle, _ptr(dist)), "mppib_set_distribution")
 

@@ -44,6 +44,8 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->step_size_cov >= 0.f && p->step_size_cov <= 1.f && p->kappa >= 0.f && p->lambda_mult >= 0.f && p->lambda_mult < 1.f,
                       "adaptive MPPI: step_size_cov %g, kappa %g or lambda_mult %g out of range", p->step_size_cov, p->kappa, p->lambda_mult);
     MPPIB_REQUIRE(!p->cov_full || p->update_cov, "cov_full selects the update rule of update_cov and needs update_cov");
+    MPPIB_REQUIRE(!p->cov_horizon || (p->update_cov && !p->cov_full), "cov_horizon selects the update rule of update_cov: it needs update_cov and excludes cov_full");
+    MPPIB_REQUIRE(!p->cov_horizon || p->T * m->nu <= MPPIB_HZ_MAX_N, "cov_horizon: n = T*nu = %d exceeds %d", p->T * m->nu, MPPIB_HZ_MAX_N);
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -107,6 +109,7 @@ int32_t mppib_create(const MppibModel* model_h, const MppibParams* params_h, int
     read_mapping_knobs(c);                                                      // read once per handle, not per launch
     derive(c);
     if (int rc = alloc_scratch(c)) { delete c; return rc; }
+    if (int rc = alloc_horizon(c)) { cudaFree(c->reduce_scratch); cudaFree(c->reduce_ticket); delete c; return rc; }
     *out = c;
     return 0;
 }
@@ -171,6 +174,8 @@ int32_t mppib_destroy(MppibHandle h) {
     mppib_peer_close(h);
     if (h->reduce_scratch) cudaFree(h->reduce_scratch);
     if (h->reduce_ticket) cudaFree(h->reduce_ticket);
+    h->params.cov_horizon = 0;
+    alloc_horizon(h);                            // frees the cov_horizon buffers
     delete h;
     return 0;
 }
@@ -182,8 +187,9 @@ int32_t mppib_set_params(MppibHandle h, const MppibParams* params_h) {
     MPPIB_REQUIRE(h->peer_world <= 1 || partial_row_capacity(*params_h, h->model.nu) <= h->peer_pcap, "mppib_set_params: T*nu outgrows the open peer window; close and re-open the peers");
     h->params = *params_h;
     derive(h);
-    if (resize) { MPPIB_ON_DEVICE(h); return alloc_scratch(h); }
-    return 0;
+    MPPIB_ON_DEVICE(h);
+    if (resize) if (int rc = alloc_scratch(h)) return rc;
+    return alloc_horizon(h);
 }
 
 int32_t mppib_set_model(MppibHandle h, const MppibModel* model_h) {
@@ -193,8 +199,9 @@ int32_t mppib_set_model(MppibHandle h, const MppibModel* model_h) {
     MPPIB_REQUIRE(h->peer_world <= 1 || partial_row_capacity(h->params, model_h->nu) <= h->peer_pcap, "mppib_set_model: T*nu outgrows the open peer window; close and re-open the peers");
     h->model = *model_h;
     derive(h);
-    if (resize) { MPPIB_ON_DEVICE(h); return alloc_scratch(h); }
-    return 0;
+    MPPIB_ON_DEVICE(h);
+    if (resize) if (int rc = alloc_scratch(h)) return rc;
+    return alloc_horizon(h);
 }
 
 int32_t mppib_state_size(MppibHandle h) { return h ? h->state_rows : -1; }

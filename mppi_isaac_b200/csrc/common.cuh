@@ -47,6 +47,13 @@ struct MppibContext {
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
     float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) or, with cov_full, (lambda, Sigma, L, Sigma^-1)
                                                // read by K1 / K3, updated by K4 (nullable)
+    // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
+    float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
+    float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
+    float* hz_sig;                             // [n*n] the shifted Sigma_H of K4 while it is being factored
+    float* hz_scr;                             // SYRK split-K partial tiles
+    unsigned int* hz_ticket;                   // [HZ_MAX_TILES + 1] per-tile and final tickets of the SYRK (reset by their last CTA)
+    int hz_K, hz_n, hz_scr_floats;
     // K2 mappings the handle may use (rollout_mapping() picks by scene, never by K); both default to true
     bool k2_team;                              // a team of lanes per rollout for trees / contact scenes (rollout_team.cu); MPPIB_K2_TEAM=0 turns it off
     bool k2_lanes;                             // one body per lane for serial chains (rollout_lanes.cu); MPPIB_K2_LANES=0 turns it off
@@ -75,10 +82,15 @@ struct DeviceGuard {
 // distribution is registered too.
 static inline int partial_row_capacity(const MppibParams& p, int nu) {
     if (p.update_cov && p.cov_full) return 2 + p.T * nu + nu * (nu + 1) / 2;
+    if (p.update_cov && p.cov_horizon) return 2 + p.T * nu + p.T * nu * (p.T * nu + 1) / 2;
     return 2 + p.T * nu * (p.update_cov ? 2 : 1);
 }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
+static inline bool adaptive_horizon(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_horizon; }
+#define MPPIB_HZ_MAX_N 256                     // cov_horizon: largest n = T*nu (the packed n x n triangle K4 factors in shared memory)
+#define HZ_TILE 64                             // SYRK output tile
+#define HZ_MAX_TILES 10                        // lower-triangle tiles of a 256 x 256 C
 
 // device view of the peer windows, passed by value to K3 / K4
 struct PeerArgs {
@@ -109,6 +121,7 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
                   float* fin_stats, cudaStream_t s);
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s);
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s);
+int alloc_horizon(MppibContext* c);           // (re)sizes the hz_* buffers for the handle's K and T*nu (frees them without cov_horizon)
 long long rollout_smem_bytes(const MppibModel& m);
 // K2, lanes-per-rollout mapping for serial chains without contacts (rollout_lanes.cu)
 bool rollout_lanes_eligible(const MppibModel& m);

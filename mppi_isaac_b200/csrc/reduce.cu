@@ -30,6 +30,11 @@ __host__ __device__ __forceinline__ int row_floats(int T, int nu, int kind) {
 }
 // shared floats finalize_rows<true, true> needs after un[T*nu] and the G scales: m1[T*nu], d[T*nu], C[nu(nu+1)/2], Sigma, L, L^-1
 __host__ __device__ __forceinline__ int full_fin_floats(int T, int nu) { return 2 * T * nu + nu * (nu + 1) / 2 + 3 * nu * nu; }
+// cov_horizon, n = T*nu: the shard row (beta, eta, W[n], C[n(n+1)/2]) and the shared floats finalize_rows<true, false, true> needs
+// after un[n] and the G scales: m1[n], d[n], the packed lower triangle A[n(n+1)/2] it factors, pivots[n], a column buffer[n]
+__host__ __device__ __forceinline__ int hz_row_floats(int n) { return 2 + n + n * (n + 1) / 2; }
+__host__ __device__ __forceinline__ int hz_fin_floats(int n) { return 4 * n + n * (n + 1) / 2; }
+__device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }     // offset of row i in a packed lower triangle
 
 __device__ __forceinline__ float warp_min(float v) {
 #pragma unroll
@@ -73,6 +78,100 @@ __constant__ float c_sg_edge[4][9] = {{763.f, 441.f, 189.f, 7.f, -105.f, -147.f,
                                       {189.f, 220.5f, 232.f, 223.5f, 195.f, 146.5f, 78.f, -10.5f, -119.f},
                                       {7.f, 136.5f, 223.5f, 268.f, 270.f, 229.5f, 146.5f, 21.f, -147.f}};
 
+// K4 of cov_horizon (dist = (lambda, Sigma_H, L_H, Sigma_H^-1), n = T*nu, after the U update, e = eta > 0), one CTA:
+//   1. Sigma' = shift((1 - s) Sigma_H + s V + kappa I),  V = C/eta - (m1 d^T + d m1^T - d d^T),  C = sum_g scale_g C_g:
+//      Sigma'[a][b] = Sigma_new[a + nu][b + nu] for a, b < n - nu; the last block row and column are 0 but for the last diagonal
+//      block, sigma0.  Lower triangle, packed into A (shared) and written to both halves of hz_sig (global staging).
+//   2. L = chol(Sigma') in place in A, right-looking: pivot k, column k scaled (and kept in `col`), rank-1 update of the trailing
+//      triangle; every entry sees its updates in k order, so the result is fixed.  The pivots go to `piv`.
+//   3. If every pivot was finite and positive: Sigma' and L to dist, L^-1 in place in A (right-looking forward substitution for all
+//      columns at once), Sigma^-1 = L^-T L^-1 to both halves of dist.  Otherwise Sigma_H, L_H and Sigma_H^-1 stay as they were.
+// Every rank combines the same rows in the same order and runs the same fixed-order arithmetic, so all write the same bits.
+__device__ __noinline__ void horizon_update(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, const float* sg, float e,
+                                            const float* m1, const float* dd, float* A, float* __restrict__ dist, float* __restrict__ hz_sig) {
+    const int n = p.T * nu, m = n - nu, npairs = tri(n);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
+    float* piv = A + npairs;
+    float* col = piv + n;
+    const float s = p.step_size_cov;
+    float* dS = dist + 1;
+    float* dL = dS + (size_t)n * n;
+    float* dI = dL + (size_t)n * n;
+    for (int i = warp; i < n; i += nw) {
+        for (int j = lane; j <= i; j += 32) {
+            float v;
+            if (i < m) {
+                const int a = i + nu, b = j + nu;
+                float cq = 0.f;
+                for (int g = 0; g < G; ++g) cq += sg[g] * __ldcg(&partials[(size_t)g * P + 2 + n + tri(a) + b]);
+                const float vab = cq / e - (m1[a] * dd[b] + dd[a] * m1[b] - dd[a] * dd[b]);
+                v = (1.0f - s) * dS[(size_t)a * n + b] + s * vab + (a == b ? p.kappa : 0.f);
+            } else {
+                v = j >= m ? p.sigma0[(i - m) * nu + (j - m)] : 0.f;
+            }
+            A[tri(i) + j] = v;
+            hz_sig[(size_t)i * n + j] = v;
+            hz_sig[(size_t)j * n + i] = v;
+        }
+    }
+    __syncthreads();
+    bool ok = true;
+    for (int k = 0; k < n; ++k) {
+        const float dk = A[tri(k) + k];                                       // the same value in every thread: a uniform branch
+        ok = isfinite(dk) && dk > 0.f;
+        if (!ok) break;
+        const float lkk = sqrtf(dk);
+        if (tid == 0) piv[k] = lkk;
+        for (int i = k + 1 + tid; i < n; i += blockDim.x) {
+            const float l = A[tri(i) + k] / lkk;
+            A[tri(i) + k] = l;
+            col[i] = l;
+        }
+        __syncthreads();
+        for (int i = k + 1 + warp; i < n; i += nw) {
+            const float lik = col[i];
+            float* __restrict__ Ai = A + tri(i);
+#pragma unroll 4
+            for (int j = k + 1 + lane; j <= i; j += 32) Ai[j] -= lik * col[j];
+        }
+        __syncthreads();
+    }
+    if (!ok) return;
+    for (int i = warp; i < n; i += nw) {
+        for (int j = lane; j < n; j += 32) {
+            dS[(size_t)i * n + j] = hz_sig[(size_t)i * n + j];
+            dL[(size_t)i * n + j] = j < i ? A[tri(i) + j] : j == i ? piv[i] : 0.f;
+        }
+    }
+    __syncthreads();
+    // X = L^-1 in place: at step k row k of X is final (X[k][j] = B[k][j] / L[k][k], X[k][k] = 1 / L[k][k]) and the rows below get
+    // B[i][j] -= L[i][k] X[k][j] (j <= k; B[i][k] starts at 0, where L[i][k] stood, so column k of L is copied to `col` first)
+    for (int k = 0; k < n; ++k) {
+        float* Ak = A + tri(k);
+        const float pk = piv[k];
+        for (int j = tid; j <= k; j += blockDim.x) Ak[j] = j == k ? 1.0f / pk : Ak[j] / pk;
+        for (int i = k + 1 + tid; i < n; i += blockDim.x) col[i] = A[tri(i) + k];
+        __syncthreads();
+        for (int i = k + 1 + warp; i < n; i += nw) {
+            const float lik = col[i];
+            float* __restrict__ Ai = A + tri(i);
+            const float* __restrict__ Xk = Ak;
+#pragma unroll 4
+            for (int j = lane; j <= k; j += 32) Ai[j] = (j == k ? 0.f : Ai[j]) - lik * Xk[j];
+        }
+        __syncthreads();
+    }
+    for (int a = warp; a < n; a += nw) {                                      // Sigma^-1[a][b] = sum_{r >= a} X[r][a] X[r][b], b <= a
+        for (int b = lane; b <= a; b += 32) {
+            float acc = 0.f;
+#pragma unroll 4
+            for (int r = a; r < n; ++r) acc += A[tri(r) + a] * A[tri(r) + b];
+            dI[(size_t)a * n + b] = acc;
+            dI[(size_t)b * n + a] = acc;
+        }
+    }
+}
+
 // combine G rows (beta_g, eta_g, W_g) of stride P, update U (+ Savitzky-Golay, clamp), first action, statistics; one CTA of 256
 // threads, `un` = [T*nu + G] floats of shared memory (+ T*nu with update_cov).
 // ADAPT (a distribution is registered): lambda comes from dist[0]; after the U update the CTA updates dist in place --
@@ -87,15 +186,17 @@ __constant__ float c_sg_edge[4][9] = {{763.f, 441.f, 189.f, 7.f, -105.f, -147.f,
 // one thread per lower-triangle entry (t in order), written to both halves; then warp 0 computes L = chol(Sigma) (left-looking, lane =
 // row) and Sigma^-1 = L^-T L^-1 (lane = column of L^-1) in a fixed order.  A pivot that is not finite and positive leaves Sigma, L and
 // Sigma^-1 as they were.  The diagonal equals the diagonal rule above without its clamp at 0.
-template <bool ADAPT, bool FULL = false>
+// HZN (update_cov with cov_horizon): the rows carry C_g[n(n+1)/2] over the whole sequence; m1 and d are kept as n-vectors and
+// horizon_update does the rest.
+template <bool ADAPT, bool FULL = false, bool HZN = false>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
-                                              float* __restrict__ dist) {
+                                              float* __restrict__ dist, float* __restrict__ hz_sig = nullptr) {
     const int T = p.T, NR = T * nu;
     float* sg = un + NR;
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
-    const bool cov = ADAPT && !FULL && p.update_cov;
+    const bool cov = ADAPT && !FULL && !HZN && p.update_cov;
     float* var = sg + G;                                                      // [NR] per-element variance (update_cov)
     const int npairs = nu * (nu + 1) / 2;
     float* m1s = sg + G;                                                      // FULL: [NR] m1, [NR] d, [npairs] C, [nu*nu] Sigma, L, L^-1
@@ -125,7 +226,7 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
             const float m1 = w / e - c0, d = un[r] - U[r];
             var[r] = fmaxf(m2 / e - 2.0f * d * m1 + d * d, 0.f);
         }
-        if (FULL && e > 0.f) {
+        if ((FULL || HZN) && e > 0.f) {
             m1s[r] = w / e - (p.mode == MPPIB_MODE_SIMPLE ? 0.f : U[r]);
             dds[r] = un[r] - U[r];
         }
@@ -163,6 +264,7 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
         if (r < nu) { action_out[r] = out; if (action_mirror) action_mirror[r] = out; }
     }
     if (threadIdx.x == 0 && stats) { stats[0] = b; stats[1] = e; }
+    if (HZN && e > 0.f) horizon_update(p, nu, partials, G, P, sg, e, m1s, dds, dds + NR, dist, hz_sig);
     if (FULL && e > 0.f) {
         const float* Sig = dist + 1;
         for (int q = threadIdx.x; q < npairs; q += blockDim.x) {
@@ -374,19 +476,23 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // lower triangle of sum_t w_k (x_tk - c_t)(x_tk - c_t)^T of its own sample k across tiles (lane = sample: column reads of the tile,
 // conflict-free like phase A; c = U staged in g in MEAN mode), rescaled online like W and summed over the warp once after the loop;
 // the shard row becomes (beta, eta, W[T*nu], C[nu(nu+1)/2]).
-template <int RPL, bool ADAPT, bool FULL = false>   // rows of W per lane: T*nu <= 32 * RPL
+// HZN (update_cov with cov_horizon): the SIMPLE-mode g = lambda Sigma_H^-1 U is read from hz_g (mppib_shift computed it), phase B
+// stores every S_k (INFINITY for an invalid sample) to hz_S for the SYRK that follows, and the row this kernel writes is
+// (beta, eta, W[n]) only; the SYRK appends C.
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
-                       float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist) {
+                       float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
+                       const float* __restrict__ hz_g) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
     const bool simple = p.mode == MPPIB_MODE_SIMPLE;
-    const bool m2 = ADAPT && !FULL && p.update_cov;
+    const bool m2 = ADAPT && !FULL && !HZN && p.update_cov;
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
     const int P = 2 + (m2 ? 2 : 1) * NR + npairs;
 
@@ -422,7 +528,9 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     }
     for (int r = tid; r < NR4; r += NT) {
         float acc = 0.f;
-        if (simple && r < NR) {
+        if (HZN && simple && r < NR) {
+            acc = hz_g[r];
+        } else if (simple && r < NR) {
             const int t = r / nu, i = r % nu;
             if (FULL) {
                 const float* sinv = dist + 1 + 2 * nu * nu;
@@ -501,6 +609,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             // ---- B: tile minimum, weights, their sum
             const bool valid = (k0 + lane < K) && isfinite(sum);
             const float S = valid ? sum : INFINITY;
+            if (HZN && k0 + lane < K) hz_S[k0 + lane] = S;
             const float b_c = warp_min(S);
             const float w = (S == INFINITY) ? 0.f : expf(-(S - b_c) * inv_lambda);
             const float e_c = warp_sum(w);
@@ -616,15 +725,15 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
-// distribution update of finalize_rows (FULL: of the full covariance).
-template <bool ADAPT, bool FULL = false>
+// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon).
+template <bool ADAPT, bool FULL = false, bool HZN = false>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
-                float* __restrict__ action_mirror, float* __restrict__ dist) {
+                float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const int T = p.T, NR = T * nu;
-    int P = FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
+    int P = HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
     const float* partials = partials_in;
     uint32_t seq = 0;
     if (partials_in == nullptr) {
@@ -650,17 +759,160 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
         partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
         P = peers.pcap;
     }
-    finalize_rows<ADAPT, FULL>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
+    finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
 }
 
-__global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu, float* __restrict__ U, uint32_t* __restrict__ plan_ctr) {
+// ------------------------------------------------------------------------------------------------------------------
+// cov_horizon: the weighted SYRK after K3.  C = sum_k w_k (x_k - c)(x_k - c)^T over the n-vectors x_k = x[:, k] (n = T*nu),
+// w_k = exp(-(S_k - beta)/lambda) with S_k from K3 (hz_S) and beta = partial[0] from K3's row, c = U (MEAN) or 0 (SIMPLE).
+//   grid = lower-triangle 64 x 64 output tiles x ksplit K-chunks; 256 threads, a 4 x 4 register block each; 32 samples at a time
+//   are staged to shared memory (weighted, centred rows of the tile's row block, centred rows of its column block; the next 32
+//   are loaded into registers meanwhile), FP32 FFMA in sample order.
+//   The last CTA of a tile (ticket) folds the ksplit partial tiles in split order and writes its entries of the packed lower
+//   triangle into the shard row; the last tile to finish pushes the whole row into the peer windows (multi-GPU) and, for
+//   single-GPU plans (fin_U != NULL), does K4's work in place, as K3's last CTA does for the other rules.
+constexpr int HZ_KB = 32;   // samples per staged chunk
+
+__global__ void __launch_bounds__(256, 1)
+mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int kchunk, const float* __restrict__ x, const float* __restrict__ U,
+                  const float* __restrict__ S, float* __restrict__ partial, float* __restrict__ scr, unsigned int* __restrict__ ticket,
+                  const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action, float* __restrict__ fin_stats,
+                  float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_sig) {
+    extern __shared__ __align__(16) float hsm[];
+    const int n = p.T * nu, K = p.K, P = hz_row_floats(n);
+    const int tid = threadIdx.x;
+    const int nb = (n + HZ_TILE - 1) / HZ_TILE, ntiles = nb * (nb + 1) / 2;
+    const int tile = (int)blockIdx.x / ksplit, split = (int)blockIdx.x % ksplit;
+    int bi = 0;
+    while (tri(bi + 1) <= tile) ++bi;
+    const int bj = tile - tri(bi);
+    const int i0 = bi * HZ_TILE, j0 = bj * HZ_TILE;
+    float* As = hsm;                        // [HZ_KB][64] w_k (x[i0 + r][k] - c), sample-major
+    float* Bs = hsm + HZ_KB * HZ_TILE;      // [HZ_KB][64] x[j0 + r][k] - c
+    const float inv_lambda = 1.0f / dist[0];
+    const float beta = __ldcg(&partial[0]);
+    const bool simple = p.mode == MPPIB_MODE_SIMPLE;
+    // loader: row lr of both blocks, samples lk .. lk + 7 of the chunk
+    const int lr = tid & (HZ_TILE - 1), lk = (tid >> 6) * 8;
+    const int ra = i0 + lr, rb = j0 + lr;
+    const float ca = (!simple && ra < n) ? U[ra] : 0.f, cb = (!simple && rb < n) ? U[rb] : 0.f;
+    const int ty = tid >> 4, tx = tid & 15;
+    const int kbeg = split * kchunk, kend = min(K, kbeg + kchunk);
+    float va[8], vb[8], wv[8];
+    auto load = [&](int k0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int k = k0 + lk + 4 * h;                                    // kend is a multiple of 4: a float4 is all in or all out
+            float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a, sv = make_float4(INFINITY, INFINITY, INFINITY, INFINITY);
+            if (k < kend) {
+                if (ra < n) a = __ldcs(reinterpret_cast<const float4*>(x + (size_t)ra * K + k));
+                if (rb < n) b = __ldcs(reinterpret_cast<const float4*>(x + (size_t)rb * K + k));
+                sv = __ldg(reinterpret_cast<const float4*>(S + k));
+            }
+            va[4 * h] = a.x; va[4 * h + 1] = a.y; va[4 * h + 2] = a.z; va[4 * h + 3] = a.w;
+            vb[4 * h] = b.x; vb[4 * h + 1] = b.y; vb[4 * h + 2] = b.z; vb[4 * h + 3] = b.w;
+            wv[4 * h] = sv.x; wv[4 * h + 1] = sv.y; wv[4 * h + 2] = sv.z; wv[4 * h + 3] = sv.w;
+        }
+    };
+    float acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[a][b] = 0.f;
+    if (kbeg < kend) load(kbeg);
+    for (int k0 = kbeg; k0 < kend; k0 += HZ_KB) {
+        __syncthreads();                                                      // the previous chunk is consumed
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            const float w = isfinite(wv[e]) ? expf(-(wv[e] - beta) * inv_lambda) : 0.f;
+            As[(lk + e) * HZ_TILE + lr] = ra < n ? w * (va[e] - ca) : 0.f;
+            Bs[(lk + e) * HZ_TILE + lr] = rb < n ? vb[e] - cb : 0.f;
+        }
+        __syncthreads();
+        if (k0 + HZ_KB < kend) load(k0 + HZ_KB);                              // in flight while this chunk is multiplied
+#pragma unroll 8
+        for (int kk = 0; kk < HZ_KB; ++kk) {
+            const float4 a4 = *reinterpret_cast<const float4*>(As + kk * HZ_TILE + ty * 4);
+            const float4 b4 = *reinterpret_cast<const float4*>(Bs + kk * HZ_TILE + tx * 4);
+            const float av[4] = {a4.x, a4.y, a4.z, a4.w}, bv[4] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = 0; b < 4; ++b) acc[a][b] = fmaf(av[a], bv[b], acc[a][b]);
+        }
+    }
+    float* mine = scr + ((size_t)tile * ksplit + split) * (HZ_TILE * HZ_TILE);
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+        reinterpret_cast<float4*>(mine + (ty * 4 + a) * HZ_TILE)[tx] = make_float4(acc[a][0], acc[a][1], acc[a][2], acc[a][3]);
+    __threadfence();
+    __syncthreads();
+    __shared__ unsigned int s_last;
+    if (tid == 0) s_last = atomicAdd(&ticket[tile], 1u) == (unsigned)ksplit - 1u ? 1u : 0u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    // the tile's last CTA: fold the splits in order, write the packed lower-triangle entries of the tile
+    const float* base = scr + (size_t)tile * ksplit * (HZ_TILE * HZ_TILE);
+    for (int q = tid; q < HZ_TILE * HZ_TILE; q += blockDim.x) {
+        const int li = q / HZ_TILE, lj = q % HZ_TILE, gi = i0 + li, gj = j0 + lj;
+        if (gi >= n || gj > gi) continue;
+        float c = 0.f;
+        for (int sp = 0; sp < ksplit; ++sp) c += __ldcg(base + (size_t)sp * (HZ_TILE * HZ_TILE) + q);
+        partial[2 + n + tri(gi) + gj] = c;
+    }
+    if (tid == 0) ticket[tile] = 0u;
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(&ticket[HZ_MAX_TILES], 1u) == (unsigned)ntiles - 1u ? 1u : 0u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (tid == 0) ticket[HZ_MAX_TILES] = 0u;
+    if (peers.world > 1) {
+        // the complete row goes into the window of every rank, then one release-store of the arrival flag per peer (as in
+        // fold_and_finish)
+        const uint32_t seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
+        const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
+        for (int e = tid; e < P; e += blockDim.x) {
+            const float v = __ldcg(&partial[e]);
+            for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + e] = v;
+        }
+        __threadfence_system();
+        __syncthreads();
+        if (tid < peers.world) {
+            uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
+            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
+        }
+    }
+    if (fin_U != nullptr) {
+        // single-GPU plans: every CTA read U and lambda before it took its ticket, so this CTA is the only reader left
+        __syncthreads();
+        finalize_rows<true, false, true>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, hsm, dist, hz_sig);
+    }
+}
+
+// hz_g (cov_horizon with a registered distribution, SIMPLE mode): g = lambda Sigma_H^-1 U of the shifted U, once per plan, for K3's
+// control cost (a row of Sigma_H^-1 per thread, summed in column order).
+__global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu, float* __restrict__ U, uint32_t* __restrict__ plan_ctr,
+                                   const float* __restrict__ dist, float* __restrict__ hz_g) {
     extern __shared__ float tmp[];
     const int NR = p.T * nu;
     for (int r = threadIdx.x; r < NR; r += blockDim.x) tmp[r] = r + nu < NR ? U[r + nu] : p.u_init[r % nu];
     __syncthreads();
     for (int r = threadIdx.x; r < NR; r += blockDim.x) U[r] = tmp[r];
     if (threadIdx.x == 0 && plan_ctr) *plan_ctr += 1u;
+    if (hz_g != nullptr) {
+        const float lam = dist[0];
+        const float* sinv = dist + 1 + 2 * (size_t)NR * NR;
+        for (int r = threadIdx.x; r < NR; r += blockDim.x) {
+            float acc = 0.f;
+#pragma unroll 4
+            for (int c = 0; c < NR; ++c) acc += sinv[(size_t)r * NR + c] * tmp[c];
+            hz_g[r] = lam * acc;
+        }
+    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -707,7 +959,7 @@ static int reduce_ws_stages(int T, int nu, int kind) {
     return ns;
 }
 
-template <int RPL, bool ADAPT, bool FULL = false>
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
@@ -721,7 +973,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -738,13 +990,77 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
     if (grid > MAX_GRID) grid = MAX_GRID;
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
-    mppib_reduce_ws_kernel<RPL, ADAPT, FULL><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch, c->reduce_ticket,
-                                                             partial, reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist);
+    PeerArgs peers = reduce_peers(c);
+    if (HZN) peers.world = 0;                                                 // the row is complete only after the SYRK, which stores it
+    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch,
+                                                                    c->reduce_ticket, partial, peers, fin_U, fin_action, fin_stats,
+                                                                    fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ksplit x chunk length of the SYRK: about one CTA per SM over the lower-triangle tiles, chunks a multiple of HZ_KB samples
+static void syrk_split(const MppibContext* c, int n, int* ntiles, int* ksplit, int* kchunk) {
+    const int nb = (n + HZ_TILE - 1) / HZ_TILE, K = c->params.K;
+    *ntiles = nb * (nb + 1) / 2;
+    int ks = c->num_sms / *ntiles;
+    if (ks < 1) ks = 1;
+    int kc = (K + ks - 1) / ks;
+    kc = (kc + HZ_KB - 1) / HZ_KB * HZ_KB;
+    *kchunk = kc;
+    *ksplit = (K + kc - 1) / kc;
+}
+
+static int hz_fin_smem(int n, int G) { return (int)sizeof(float) * (n + G + hz_fin_floats(n)); }
+
+int launch_syrk(MppibContext* c, const float* x, const float* U, float* partial, float* fin_U, float* fin_action, float* fin_stats, cudaStream_t s) {
+    const int n = c->params.T * c->model.nu;
+    int ntiles, ksplit, kchunk;
+    syrk_split(c, n, &ntiles, &ksplit, &kchunk);
+    MPPIB_REQUIRE((size_t)ntiles * ksplit * HZ_TILE * HZ_TILE <= (size_t)c->hz_scr_floats, "mppib_reduce: SYRK scratch too small");
+    int smem = (int)sizeof(float) * 2 * HZ_KB * HZ_TILE;
+    if (fin_U != nullptr && hz_fin_smem(n, 1) > smem) smem = hz_fin_smem(n, 1);
+    static int smem_attr[64] = {0};
+    int& attr = smem_attr[c->device & 63];
+    if (smem > attr) {
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr = smem;
+    }
+    mppib_syrk_kernel<<<ntiles * ksplit, 256, smem, s>>>(c->params, c->model.nu, ksplit, kchunk, x, U, c->hz_S, partial, c->hz_scr, c->hz_ticket,
+                                                         reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist,
+                                                         c->hz_sig);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
 }  // namespace
+
+int alloc_horizon(MppibContext* c) {
+    const bool on = c->params.update_cov && c->params.cov_horizon;
+    const int K = c->params.K, n = c->params.T * c->model.nu;
+    if (on && c->hz_S && c->hz_K == K && c->hz_n == n) return 0;
+    if (c->hz_S) cudaFree(c->hz_S);
+    if (c->hz_g) cudaFree(c->hz_g);
+    if (c->hz_sig) cudaFree(c->hz_sig);
+    if (c->hz_scr) cudaFree(c->hz_scr);
+    if (c->hz_ticket) cudaFree(c->hz_ticket);
+    c->hz_S = c->hz_g = c->hz_sig = c->hz_scr = nullptr;
+    c->hz_ticket = nullptr;
+    c->hz_K = c->hz_n = c->hz_scr_floats = 0;
+    if (!on) return 0;
+    const int tiles = c->num_sms > HZ_MAX_TILES ? c->num_sms : HZ_MAX_TILES;  // ntiles * ksplit of syrk_split never exceeds this
+    c->hz_scr_floats = tiles * HZ_TILE * HZ_TILE;
+    MPPIB_CHECK_CUDA(cudaMalloc(&c->hz_S, sizeof(float) * (size_t)((K + 3) & ~3)));
+    MPPIB_CHECK_CUDA(cudaMalloc(&c->hz_g, sizeof(float) * (size_t)n));
+    MPPIB_CHECK_CUDA(cudaMemset(c->hz_g, 0, sizeof(float) * (size_t)n));
+    MPPIB_CHECK_CUDA(cudaMalloc(&c->hz_sig, sizeof(float) * (size_t)n * n));
+    MPPIB_CHECK_CUDA(cudaMalloc(&c->hz_scr, sizeof(float) * (size_t)c->hz_scr_floats));
+    MPPIB_CHECK_CUDA(cudaMalloc(&c->hz_ticket, sizeof(unsigned int) * (HZ_MAX_TILES + 1)));
+    MPPIB_CHECK_CUDA(cudaMemset(c->hz_ticket, 0, sizeof(unsigned int) * (HZ_MAX_TILES + 1)));
+    c->hz_K = K;
+    c->hz_n = n;
+    return 0;
+}
 
 int launch_reduce(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                   float* fin_stats, cudaStream_t s) {
@@ -758,6 +1074,15 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(T, nu, ROW_C) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the covariance row of cov_full", T, nu);
     const int NR = T * nu;
+    if (adaptive_horizon(c)) {
+        MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N, "mppib_reduce: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, NR);
+        MPPIB_REQUIRE(c->hz_S != nullptr && c->hz_K == c->params.K && c->hz_n == NR, "mppib_reduce: cov_horizon buffers are not sized for K = %d, n = %d",
+                      c->params.K, NR);
+        const int rc = NR <= 32 * 4 ? launch_reduce_ws_t<4, true, false, true>(c, cost, x, U, partial, nullptr, nullptr, nullptr, s)
+                                    : launch_reduce_ws_t<8, true, false, true>(c, cost, x, U, partial, nullptr, nullptr, nullptr, s);
+        if (rc) return rc;
+        return launch_syrk(c, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
     if (adaptive_full(c)) {
         if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
         if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
@@ -775,15 +1100,29 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    if (adaptive_full(c)) {
+    if (adaptive_horizon(c)) {
+        MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N && c->hz_sig != nullptr && c->hz_n == NR, "mppib_finalize: cov_horizon buffers are not sized for n = %d", NR);
+        const int smem = hz_fin_smem(NR, G);
+        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: cov_horizon with n = %d and G = %d needs %d bytes of shared memory", NR, G, smem);
+        static int smem_attr[64] = {0};
+        int& attr = smem_attr[c->device & 63];
+        if (smem > attr) {
+            MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_finalize_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            attr = smem;
+        }
+        mppib_finalize_kernel<true, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror,
+                                                                      c->dist, c->hz_sig);
+    } else if (adaptive_full(c)) {
         const size_t smem = (NR + G + full_fin_floats(c->params.T, c->model.nu)) * sizeof(float);
-        mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist);
+        mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
+                                                               nullptr);
     } else if (c->dist) {
         const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
-        mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist);
+        mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
+                                                         nullptr);
     } else {
         mppib_finalize_kernel<false><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                              c->action_mirror, nullptr);
+                                                                              c->action_mirror, nullptr, nullptr);
     }
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -791,7 +1130,8 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
 
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr);
+    float* hz_g = adaptive_horizon(c) && c->params.mode == MPPIB_MODE_SIMPLE ? c->hz_g : nullptr;
+    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -182,6 +182,115 @@ mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     }
 }
 
+// HORIZON (update_cov with cov_horizon, n = T*nu <= 256): noise = L_H z over the whole n-vector of a sample, with L_H =
+// dist[1 + n*n ..] the live lower Cholesky factor of Sigma_H, rows and columns ordered (t, j) like U.  A CTA of 128 threads owns a
+// tile of HZ_S = 64 samples: the white draws of the tile go to shared memory first -- the Philox draws of the fixed-Sigma kernel
+// (counter (global sample, t, block)) or, LIB, the white library Z -- then L_H is staged 32 rows at a time, transposed, and every
+// warp multiplies 8 of those rows with the tile: lane = samples lane and lane + 32, an 8 x 2 register block, two broadcast LDS.128
+// of L_H and two LDS of z per 16 FFMA.  The sum over columns runs from 0 upwards (the zeros above the diagonal add nothing), so a
+// sample's noise depends only on its global index.  Clamping and the null / prior rows are those of the other K1 variants.
+constexpr int HZ_S = 64;        // samples per CTA
+constexpr int HZ_LP = 36;       // padded row of the transposed L_H panel (16-byte aligned, 4-way store conflicts at most)
+
+__host__ __device__ __forceinline__ int horizon_smem_bytes(int n) { return (int)sizeof(float) * n * (HZ_S + HZ_LP); }
+
+template <bool LIB>
+__global__ void __launch_bounds__(128)
+mppib_sample_horizon_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+                            const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
+                            const float* __restrict__ prior_row, const float* __restrict__ Z, float* __restrict__ actions, float* __restrict__ noise,
+                            const float* __restrict__ dist) {
+    extern __shared__ __align__(16) float hs[];
+    const int K = p.K, T = p.T, n = T * nu;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int k0 = blockIdx.x * HZ_S;
+    float* zs = hs;                       // [n][HZ_S] white draws of the tile
+    float* Lt = hs + n * HZ_S;            // [n][HZ_LP] Lt[c][i] = L_H[r0 + i][c] of the current 32-row panel
+    if (LIB) {
+        for (int idx = tid; idx < n * HZ_S; idx += blockDim.x) {
+            const int r = idx / HZ_S, sl = idx % HZ_S, k = k0 + sl;
+            zs[idx] = k < K ? Z[(size_t)r * K + k] : 0.f;
+        }
+    } else {
+        const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
+        const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
+        const int nblk = (nu + 3) / 4;
+        for (int idx = tid; idx < HZ_S * T * nblk; idx += blockDim.x) {
+            const int sl = idx % HZ_S, rest = idx / HZ_S, blk = rest % nblk, t = rest / nblk;
+            const uint32_t kg = k_offset + (uint32_t)(k0 + sl);
+            const uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
+            float z[4];
+            box_muller(r.x, r.y, z[0], z[1]);
+            box_muller(r.z, r.w, z[2], z[3]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e)
+                if (4 * blk + e < nu) zs[(t * nu + 4 * blk + e) * HZ_S + sl] = z[e];
+        }
+    }
+    const float* Ld = dist + 1 + (size_t)n * n;
+    for (int r0 = 0; r0 < n; r0 += 32) {
+        const int cmax = min(n, r0 + 32);                                     // columns of the panel that can be non-zero
+        __syncthreads();                                                      // z staged / the previous panel consumed
+        for (int idx = tid; idx < 32 * cmax; idx += blockDim.x) {
+            const int i = idx / cmax, c = idx % cmax;
+            Lt[c * HZ_LP + i] = r0 + i < n ? Ld[(size_t)(r0 + i) * n + c] : 0.f;
+        }
+        __syncthreads();
+        const int rb = r0 + warp * 8;
+        if (rb >= n) continue;
+        float acc0[8], acc1[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+        const int cend = min(n, rb + 8);
+        for (int c = 0; c < cend; ++c) {
+            const float za = zs[c * HZ_S + lane], zb = zs[c * HZ_S + 32 + lane];
+            const float4 la = *reinterpret_cast<const float4*>(Lt + c * HZ_LP + warp * 8);
+            const float4 lb = *reinterpret_cast<const float4*>(Lt + c * HZ_LP + warp * 8 + 4);
+            const float lv[8] = {la.x, la.y, la.z, la.w, lb.x, lb.y, lb.z, lb.w};
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { acc0[i] = fmaf(lv[i], za, acc0[i]); acc1[i] = fmaf(lv[i], zb, acc1[i]); }
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int r = rb + i;
+            if (r >= n) break;
+            const int t = r / nu, j = r % nu;
+            const float u = U[r];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int k = k0 + lane + 32 * h;
+                if (k >= K) continue;
+                const uint32_t kg = k_offset + (uint32_t)k;
+                float a = u + (h ? acc1[i] : acc0[i]);
+                if (p.sample_null_action && kg == k_total - 1) a = 0.f;
+                a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+                if (prior_row != nullptr && kg == k_total - 2) a = prior_row[t * nu + j];
+                const size_t idx = (size_t)r * K + k;
+                actions[idx] = a;
+                if (noise) noise[idx] = a - u;
+            }
+        }
+    }
+}
+
+template <bool LIB>
+int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                            const float* U, const float* prior_row, const float* Z, float* actions, float* noise, cudaStream_t s) {
+    const int K = c->params.K, n = c->params.T * c->model.nu;
+    MPPIB_REQUIRE(n <= MPPIB_HZ_MAX_N, "K1: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, n);
+    const int smem = horizon_smem_bytes(n);
+    static int smem_attr[64] = {0};
+    int& attr = smem_attr[c->device & 63];
+    if (smem > attr) {
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_horizon_kernel<LIB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr = smem;
+    }
+    mppib_sample_horizon_kernel<LIB><<<(K + HZ_S - 1) / HZ_S, 128, smem, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
+                                                                              plan_ctr, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
@@ -200,6 +309,8 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
                           float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
+    if (adaptive_horizon(c))
+        return launch_sample_horizon_t<true>(c, 0, 0, nullptr, k_offset, k_total, U, prior_row, Z, actions, noise, s);
     if (adaptive_full(c))
         mppib_sample_library_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
     else if (adaptive_cov(c))
@@ -214,6 +325,8 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
+    if (adaptive_horizon(c))
+        return launch_sample_horizon_t<false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, nullptr, actions, noise, s);
     if (adaptive_full(c))
         mppib_sample_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset,
                                                                 k_total, U, prior_row, actions, noise, c->dist);

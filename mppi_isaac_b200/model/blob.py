@@ -18,9 +18,10 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
+HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
 
 JOINT_REVOLUTE, JOINT_PRISMATIC = 0, 1
 DRIVE_VELOCITY, DRIVE_EFFORT = 0, 1
@@ -73,6 +74,7 @@ class MppibParams(C.Structure):
         ("nobs", i32), ("obs", MppibObsItem * MAX_OBS),
         ("update_cov", i32), ("update_lambda", i32), ("eta_u_bound", f32), ("eta_l_bound", f32),
         ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32), ("cov_full", i32),
+        ("cov_horizon", i32), ("sigma0", f32 * (MAX_NU * MAX_NU)),
     ]
 
 
@@ -390,11 +392,14 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     p.eta_l_bound = float(getattr(mppi_cfg, "eta_l_bound", 5.0))
     p.step_size_cov, p.kappa, p.lambda_mult = 0.7, 0.005, 0.1
     cov_type = str(getattr(mppi_cfg, "cov_type", "diag"))
-    if cov_type not in ("diag", "full"):
-        raise ValueError(f"unknown cov_type {cov_type!r} (diag | full)")
-    if cov_type == "full" and not p.update_cov:
-        raise ValueError("cov_type: full selects the update rule of update_cov and needs update_cov: true")
+    if cov_type not in ("diag", "full", "horizon"):
+        raise ValueError(f"unknown cov_type {cov_type!r} (diag | full | horizon)")
+    if cov_type in ("full", "horizon") and not p.update_cov:
+        raise ValueError(f"cov_type: {cov_type} selects the update rule of update_cov and needs update_cov: true")
     p.cov_full = int(cov_type == "full")
+    p.cov_horizon = int(cov_type == "horizon")
+    if p.cov_horizon and p.T * nu > HZ_MAX_N:
+        raise ValueError(f"cov_type: horizon adapts a (T*nu) x (T*nu) covariance with T*nu <= {HZ_MAX_N}; T*nu = {p.T * nu}")
     p.u_scale = float(mppi_cfg.u_scale)
     p.sample_null_action = int(bool(mppi_cfg.sample_null_action))
     p.filter_u = int(bool(mppi_cfg.filter_u))
@@ -411,8 +416,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     umin, umax = bc(mppi_cfg.u_min, -1e30), bc(mppi_cfg.u_max, 1e30)
     uinit = bc(mppi_cfg.u_init, 0.0)
     sigma = np.asarray(mppi_cfg.noise_sigma, np.float64).reshape(nu, nu)
-    if p.cov_full and (np.any(sigma != sigma.T) or np.any(np.linalg.eigvalsh(sigma) <= 0)):
-        raise ValueError("cov_type: full needs a symmetric positive-definite noise_sigma")
+    if (p.cov_full or p.cov_horizon) and (np.any(sigma != sigma.T) or np.any(np.linalg.eigvalsh(sigma) <= 0)):
+        raise ValueError(f"cov_type: {cov_type} needs a symmetric positive-definite noise_sigma")
     chol = np.linalg.cholesky(sigma)
     sinv = np.linalg.inv(sigma)
     for j in range(nu):
@@ -420,6 +425,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         for i in range(nu):
             p.sigma_chol[j * nu + i] = chol[j, i]
             p.sigma_inv[j * nu + i] = sinv[j, i]
+            p.sigma0[j * nu + i] = sigma[j, i]
     if len(obs_items) > MAX_OBS:
         raise ValueError("too many observation items")
     p.k_offset = int(getattr(mppi_cfg, "_k_offset", 0))

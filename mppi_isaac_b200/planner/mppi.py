@@ -129,7 +129,9 @@ class MPPIPlanner:
         # cov_type chooses the update rule of update_cov: "diag" adapts diag(Sigma), "full" the whole Sigma with its Cholesky factor
         # and inverse (DESIGN.md section 2); make_params rejects other values, full without update_cov and a Sigma that is not SPD
         self.cov_full = self.update_cov and str(getattr(cfg, "cov_type", "diag")) == "full"
-        if self.update_cov and not self.cov_full:
+        # "horizon" adapts one Sigma_H over the whole control sequence (n = T*nu), started at I_T (x) Sigma
+        self.cov_horizon = self.update_cov and str(getattr(cfg, "cov_type", "diag")) == "horizon"
+        if self.update_cov and not self.cov_full and not self.cov_horizon:
             import numpy as np
             sigma = np.asarray(cfg.noise_sigma, np.float64).reshape(self.nu, self.nu)
             if np.any(sigma != np.diag(np.diag(sigma))):
@@ -213,6 +215,8 @@ class MPPIPlanner:
         P = 2 + T * nu * (2 if self.update_cov else 1)      # (beta, eta, W[T*nu]) + M2[T*nu] with update_cov
         if self.cov_full:
             P = 2 + T * nu + nu * (nu + 1) // 2               # (beta, eta, W[T*nu]) + C[lower triangle] with cov_type full
+        if self.cov_horizon:
+            P = 2 + T * nu + T * nu * (T * nu + 1) // 2       # (beta, eta, W[n]) + C[lower triangle of n x n] with cov_type horizon
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
@@ -226,13 +230,15 @@ class MPPIPlanner:
         self.plan_ctr = torch.zeros((1,), dtype=torch.int32, device=dev)
         self._prior_rows = torch.zeros((T, nu), **f32) if self.use_priors else None
         # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma), or with cov_type full (lambda, Sigma, L, Sigma^-1)
-        # computed in float64 and rounded; registered before the noise library is built (update_cov makes it white)
+        # (horizon: the same of Sigma_H = I_T (x) Sigma, n = T*nu) computed in float64 and rounded; registered before the noise library is built (update_cov makes it white)
         self.dist = None
         if not self.adaptive and hasattr(self.backend, "set_distribution"):
             self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
         if self.adaptive:
             sigma = torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)
-            if self.cov_full:
+            if self.cov_horizon:
+                sigma = torch.kron(torch.eye(T, dtype=torch.float64), sigma)       # Sigma_H = I_T (x) Sigma
+            if self.cov_full or self.cov_horizon:
                 chol = torch.linalg.cholesky(sigma)
                 parts = [sigma.reshape(-1), chol.reshape(-1), torch.cholesky_inverse(chol).reshape(-1)]
             else:
@@ -273,10 +279,14 @@ class MPPIPlanner:
     @property
     def cov_action(self):
         """(nu,) device view of the diagonal sampling covariance of adaptive MPPI: adapted with update_cov, the constant diag(Sigma)
-        with update_lambda alone, None with both flags off; with cov_type full the (nu, nu) view of the adapted Sigma.  ``lambda_``
-        stays the configured float; the live temperature is ``current_lambda``."""
+        with update_lambda alone, None with both flags off; with cov_type full the (nu, nu) view of the adapted Sigma, with
+        cov_type horizon the (T*nu, T*nu) view of Sigma_H.  ``lambda_`` stays the configured float; the live temperature is
+        ``current_lambda``."""
         if self.dist is None:
             return None
+        if self.cov_horizon:
+            n = self.T * self.nu
+            return self.dist[1:1 + n * n].view(n, n)
         if self.cov_full:
             return self.dist[1:1 + self.nu * self.nu].view(self.nu, self.nu)
         return self.dist[1:]

@@ -3,9 +3,11 @@
 1. K3 alone without and with the second-moment row (a registered distribution with update_cov), and with the covariance row of
    cov_type full, cold L2: inputs rotated over more than twice the L2 size as bench.py's roofline sweep does, the variants alternated
    round by round in one process.  Panda (T = 30, nu = 7) and omnipanda (T = 30, nu = 12).
-2. The panda reach plan (config_panda_b200: K = 10 000, T = 30) with both flags off, with both flags on (diagonal rule) and with both
-   flags on and cov_type full, plans of the planners alternated in blocks, L2 flushed before every plan, CUDA-graph replay as in
-   production.
+2. The panda reach plan (config_panda_b200: K = 10 000, T = 30) with both flags off, with both flags on (diagonal rule), with both
+   flags on and cov_type full, and with both flags on and cov_type horizon (n = T*nu = 210), plans of the planners alternated in
+   blocks, L2 flushed before every plan, CUDA-graph replay as in production.
+3. Per-kernel device times of the cov_type full and horizon plans (torch.profiler with CUDA activities, in a run of its own after
+   the timed plans): K1, K3, the SYRK and K4 of the horizon rule next to the kernels of the full rule.
 
 Prints the card name and its power limit (read through NVML, nothing is changed) next to the numbers.
     python tools/adaptive_bench.py [--ks 10000,65536,262144] [--rounds 5] [--plans 200] [--scenes panda,omnipanda]
@@ -13,6 +15,7 @@ Prints the card name and its power limit (read through NVML, nothing is changed)
 import argparse
 import json
 import os
+import re
 import statistics
 import sys
 
@@ -113,10 +116,10 @@ def plan_ab(plans, block=20):
     import copy
     q0 = [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]
     pls = {}
-    for name, on in (("flags_off", False), ("flags_on", True), ("flags_on_full", True)):
+    for name, on in (("flags_off", False), ("flags_on", True), ("flags_on_full", True), ("flags_on_horizon", True)):
         cfg = copy.deepcopy(load_isaacgym_config("config_panda_b200"))
         cfg.mppi.device, cfg.mppi.update_cov, cfg.mppi.update_lambda = "cuda:0", on, on
-        cfg.mppi.cov_type = "full" if name == "flags_on_full" else "diag"
+        cfg.mppi.cov_type = {"flags_on_full": "full", "flags_on_horizon": "horizon"}.get(name, "diag")
         pl = MPPIisaacPlanner(cfg, PandaReachObjective(), use_cuda_graph=True)
         for _ in range(5):
             pl.compute_action(q0, [0.0] * 7)
@@ -137,6 +140,33 @@ def plan_ab(plans, block=20):
     out["lambda_after"] = float(pls["flags_on"].mppi.current_lambda)
     out["cov_after"] = pls["flags_on"].mppi.cov_action.cpu().tolist()
     out["sigma_after_full"] = pls["flags_on_full"].mppi.cov_action.cpu().tolist()
+    S_h = pls["flags_on_horizon"].mppi.cov_action.double().cpu()
+    out["sigma_h_after"] = {"n": S_h.shape[0], "max_abs": float(S_h.abs().max()),
+                            "max_abs_off_block_diagonal": float((S_h - torch.block_diag(*[S_h[i:i + 7, i:i + 7] for i in range(0, S_h.shape[0], 7)])).abs().max()),
+                            "cond": float(torch.linalg.cond(S_h))}
+    out["kernels_us"] = kernel_times({n: pls[n] for n in ("flags_on_full", "flags_on_horizon")}, flush)
+    return out
+
+
+def kernel_times(pls, flush, plans=50):
+    """Mean device time per launch of every kernel of a plan (torch.profiler, CUDA activities), per planner."""
+    from torch.profiler import ProfilerActivity, profile
+    out = {}
+    for n, pl in pls.items():
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(plans):
+                flush.zero_()
+                pl.mppi.command()
+            torch.cuda.synchronize()
+        rows = {}
+        for ev in prof.key_averages():
+            if ev.device_type == torch.autograd.DeviceType.CUDA and "mppib" in ev.key:
+                key = ev.key.replace("(anonymous namespace)", "")
+                name = re.search(r"mppib_\w+", key).group(0) + ("<" + key.split("<", 1)[1].split(">")[0] + ">" if "<" in key.split("(")[0] else "")
+                r = rows.setdefault(name, {"us": 0.0, "count": 0})
+                r["us"] += ev.device_time_total
+                r["count"] += ev.count
+        out[n] = {k: round(v["us"] / max(1, v["count"]), 2) for k, v in rows.items()}
     return out
 
 

@@ -2,7 +2,7 @@
 """Small, complete pass over every kernel of libmppib.so for compute-sanitizer (tools/sanitize.sh): K1 (Gaussian and Halton-spline
 library), K2 (lanes-per-rollout chain kernel, team kernel on contact scenes of small and large robots, thread-per-rollout chain / tree /
 contact kernels), fused cost, K3 (warp-specialised
-ring, ragged last tile), K4, shift, and whole plans (eager and CUDA-graph replay).  Sizes are
+ring, ragged last tile), K4, shift, the cov_type horizon kernels (horizon-colour K1, SYRK, its fused K4), and whole plans (eager and CUDA-graph replay).  Sizes are
 small: the sanitizer serialises the GPU.  With WORLD_SIZE > 1 (torchrun) the plans also run the peer-memory exchange."""
 import os
 import sys
@@ -31,6 +31,11 @@ CASES = [
     ("point robot (lanes K2 G=4, Halton-spline K1, savgol K4)", lambda: point_cfg(K=256 * world, T=12, device=dev), PointReachObjective, [0.1, 0.0, 0.0]),
     ("heijn push (team K2: contacts, 8 lanes per rollout, 2 coordinate slots)", lambda: push_cfg(K=128 * world, T=10, device=dev), PushObjective, [0.0, 0.0, 0.0]),
     ("boxer push (team K2: contacts, planar base tree)", lambda: boxer_cfg(K=128 * world, T=10, device=dev), lambda: PushObjective(robot="boxer", link="ee_link"), [0.0, 2.5, 0.0]),
+    ("panda reach, cov_type horizon (horizon-colour K1, K3 with S_k, SYRK with the fused K4 factorisation; n = 210)",
+     lambda: panda_cfg(K=1000 * world, T=30, device=dev, update_cov=True, update_lambda=True, cov_type="horizon"), PandaReachObjective,
+     [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]),
+    ("point robot, cov_type horizon (horizon-colour library K1, savgol K4; n = 36)",
+     lambda: point_cfg(K=256 * world, T=12, device=dev, update_cov=True, cov_type="horizon"), PointReachObjective, [0.1, 0.0, 0.0]),
     ("panda pick (team K2: contacts, 16-lane articulation in 2 passes, compact layout)", lambda: pick_cfg(K=64 * world, T=9, device=dev), PandaPickObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0, 0.02, 0.02]),
 ]
 for name, mk, obj, q in CASES:
