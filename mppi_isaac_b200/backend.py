@@ -56,6 +56,18 @@ def _ptr(t):
     return C.c_void_p(0 if t is None else t.data_ptr())
 
 
+def dist_floats(params, nu):
+    """(floats, layout) of the distribution buffer that K1 / K3 / K4 read under `params` with `nu` inputs: 1 + 3 n^2 with cov_horizon
+    (n = T*nu), 1 + 3 nu^2 with cov_full, 1 + nu otherwise (update_cov with a diagonal Sigma, or update_lambda alone)."""
+    nu = int(nu)
+    if params.update_cov and params.cov_horizon:
+        n = int(params.T) * nu
+        return 1 + 3 * n * n, f"cov_horizon (lambda, Sigma_H, L_H, Sigma_H^-1, n = T*nu = {n})"
+    if params.update_cov and params.cov_full:
+        return 1 + 3 * nu * nu, "cov_full (lambda, Sigma, L, Sigma^-1)"
+    return 1 + nu, "(lambda, cov[nu])"
+
+
 def _destroy_handle(lib, handle_value):
     """Finalizer of a live MppibHandle (garbage collection or interpreter exit): frees the handle's device scratch."""
     try:
@@ -111,10 +123,12 @@ class CudaBackend:
             self.handle = C.c_void_p(0)
 
     def set_params(self, params: MppibParams):
+        self._check_dist_fits(params, self.model, "mppib_set_params")
         self.params = params
         self._check(self.lib.mppib_set_params(self.handle, C.byref(params)), "mppib_set_params")
 
     def set_model(self, model: MppibModel):
+        self._check_dist_fits(self.params, model, "mppib_set_model")
         self.model = model
         self._check(self.lib.mppib_set_model(self.handle, C.byref(model)), "mppib_set_model")
 
@@ -200,17 +214,23 @@ class CudaBackend:
             kind = "cov_horizon" if self._cov_horizon() else "cov_full"
             raise RuntimeError(f"{what}: {kind} shard rows hold {self.partial_row_floats()} floats, got {rows.shape[-1]}")
 
+    def _check_dist_fits(self, params, model, what):
+        """The library keeps only a pointer to the registered distribution, so every change of (T, nu) or of the update rule is checked
+        against its length before the library sees it: a shorter buffer would be read past its end by the next K1, shift or K4."""
+        if self._dist_keepalive is not None:
+            need, layout = dist_floats(params, model.nu)
+            if self._dist_keepalive.numel() != need:
+                raise RuntimeError(f"{what}: the registered distribution holds {self._dist_keepalive.numel()} floats, but T = {int(params.T)}, "
+                                   f"nu = {int(model.nu)} needs {layout} = {need}; register a new one (set_distribution) first")
+
     def set_distribution(self, dist):
         """Adaptive MPPI: register the device tensor (lambda, cov[nu]) -- with cov_full (lambda, Sigma, L, Sigma^-1), 1 + 3 nu^2
         floats, with cov_horizon (lambda, Sigma_H, L_H, Sigma_H^-1), 1 + 3 n^2 floats, n = T*nu -- that K1 / K3 read and K4 updates
         (None switches it off)."""
-        if dist is not None and self._cov_full() and dist.numel() != 1 + 3 * self.model.nu ** 2:
-            raise RuntimeError(f"mppib_set_distribution: cov_full needs (lambda, Sigma, L, Sigma^-1) = {1 + 3 * self.model.nu ** 2} floats, "
-                               f"got {dist.numel()}")
-        n = int(self.params.T) * int(self.model.nu)
-        if dist is not None and self._cov_horizon() and dist.numel() != 1 + 3 * n * n:
-            raise RuntimeError(f"mppib_set_distribution: cov_horizon needs (lambda, Sigma_H, L_H, Sigma_H^-1) = {1 + 3 * n * n} floats "
-                               f"(n = T*nu = {n}), got {dist.numel()}")
+        if dist is not None:
+            need, layout = dist_floats(self.params, self.model.nu)
+            if dist.numel() != need:
+                raise RuntimeError(f"mppib_set_distribution: {layout} = {need} floats, got {dist.numel()}")
         self._dist_keepalive = dist
         self._check(self.lib.mppib_set_distribution(self.handle, _ptr(dist)), "mppib_set_distribution")
 

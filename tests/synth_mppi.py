@@ -6,10 +6,14 @@ and, for the adaptive row kinds, the live distribution:
 
 * ``W``  -- fixed Sigma (``sigma_chol`` / ``sigma_inv``), shard row ``[beta, eta, W[T*nu]]``;
 * ``M2`` -- ``update_cov`` with a diagonal Sigma, ``dist = [lambda, cov[nu]]``, row ``+ M2[T*nu]``;
-* ``C``  -- ``update_cov`` with ``cov_type: full``, ``dist = [lambda, Sigma, L, Sigma^-1]``, row ``+ C[nu(nu+1)/2]``.
+* ``C``  -- ``update_cov`` with ``cov_type: full``, ``dist = [lambda, Sigma, L, Sigma^-1]``, row ``+ C[nu(nu+1)/2]``;
+* ``H``  -- ``update_cov`` with ``cov_type: horizon``, ``dist = [lambda, Sigma_H, L_H, Sigma_H^-1]`` (n = T*nu), row ``+ C[n(n+1)/2]``
+  over the whole horizon (the SYRK after K3 appends it).
 
 ``ws_layout`` restates the shared-memory plan of the warp-specialised K3 (``WsLayout`` and the ring-depth rule of
-``launch_reduce_ws_t`` in ``csrc/reduce.cu``), so a case id can name the instantiation and the consumer-warp count that run.
+``launch_reduce_ws_t`` in ``csrc/reduce.cu``), so a case id can name the instantiation and the consumer-warp count that run.  For
+``H`` the host sizes the ring with the M2 layout while the kernel addresses the (smaller) W layout, and the restatement follows the
+host.  ``syrk_split`` restates the split of the SYRK over lower-triangle 64 x 64 tiles and K-chunks.
 
 The K3 gate (``k3_gate``) bounds the float32 error of the kernel per case instead of using a constant tolerance:
   dS_k <= eps * [(n/4 + 6 + 2 ln2 |log2 gamma| T) * sum_t |gamma^t c_tk| + (n/4 + nu + 6) * sum_r |x_rk| |lambda Sigma^-1|_r |U|]
@@ -37,7 +41,7 @@ WS_W, WS_NCONS, MAX_GRID, SMEM_CAP = 32, 7, 512, 224 * 1024
 
 def row_floats(T, nu, kind):
     NR = T * nu
-    return 2 + NR + (NR if kind == "M2" else nu * (nu + 1) // 2 if kind == "C" else 0)
+    return 2 + NR + (NR if kind == "M2" else nu * (nu + 1) // 2 if kind == "C" else NR * (NR + 1) // 2 if kind == "H" else 0)
 
 
 def _ws_bytes(T, nu, nstage, kind):
@@ -64,6 +68,10 @@ def ws_stages(T, nu, kind):
 def ws_layout(T, nu, kind):
     """(rows of W per lane, consumer warps, ring stages, rows per x TMA box) of the K3 launch, or None if the shape is refused."""
     NR = T * nu
+    if kind == "H":
+        if NR > HZ_MAX_N:
+            return None
+        kind = "M2"                    # the host sizes the horizon K3 (row W only) with the update_cov rule's M2 layout
     if NR > 512 or T > 256 or ws_stages(T, nu, "W") < 2 or ws_stages(T, nu, kind) < 2:
         return None
     ns = ws_stages(T, nu, kind)
@@ -78,6 +86,38 @@ def wrap_K(T, nu, kind, sms=NUM_SMS):
     """A ragged K (multiple of 4) whose every CTA streams more than three full rings of tiles."""
     _, _, nstage, _ = ws_layout(T, nu, kind)
     return WS_W * sms * (3 * nstage + 1) - 12
+
+
+# ---------------------------------------------------------------------------------------------------------------- SYRK split
+HZ_MAX_N, HZ_TILE, HZ_KB = 256, 64, 32
+
+
+def syrk_split(n, K, sms=NUM_SMS):
+    """(ntiles, ksplit, kchunk) of the SYRK (``syrk_split`` in csrc/reduce.cu): about one CTA per SM over the lower-triangle 64 x 64
+    tiles of C, chunks rounded up to a multiple of 32 samples; the last chunk holds what is left (4 samples at least)."""
+    nb = (n + HZ_TILE - 1) // HZ_TILE
+    ntiles = nb * (nb + 1) // 2
+    ks = max(sms // ntiles, 1)
+    kc = -(-K // ks)
+    kc = -(-kc // HZ_KB) * HZ_KB
+    return ntiles, -(-K // kc), kc
+
+
+def last4_K(n, sms=NUM_SMS):
+    """A K that splits into as many chunks as large K does, the last of them holding only 4 samples."""
+    _, ks0, _ = syrk_split(n, 1 << 20, sms)                                     # the split count at large K
+    for kc in range(HZ_KB, 1 << 16, HZ_KB):
+        for ks in range(ks0, 1, -1):
+            K = kc * (ks - 1) + 4
+            if syrk_split(n, K, sms)[1:] == (ks, kc):
+                return K
+    raise ValueError(n)
+
+
+def hz_id(T, nu, K, tag, sms=NUM_SMS):
+    rpl, ncons, _, _ = ws_layout(T, nu, "H")
+    ntiles, ksplit, _ = syrk_split(T * nu, K, sms)
+    return f"hz-RPL{rpl}-T{T}nu{nu}-ncons{ncons}-t{ntiles}x{ksplit}-K{K}-{tag}"
 
 
 # ---------------------------------------------------------------------------------------------------------------- cases
@@ -124,9 +164,15 @@ class Case:
     def lam(self):
         return float(self.dist[0]) if self.dist is not None else float(self.params.lambda_)
 
+    @property
+    def n(self):
+        return self.T * self.nu
+
     def chol(self):
-        """The float32 lower factor K1 colours with."""
-        nu = self.nu
+        """The float32 lower factor K1 colours with (n x n for H)."""
+        nu, n = self.nu, self.n
+        if self.kind == "H":
+            return self.dist[1 + n * n:1 + 2 * n * n].reshape(n, n)
         if self.kind == "M2":
             return np.diag(np.sqrt(self.dist[1:1 + nu].astype(np.float32)))
         if self.kind == "C":
@@ -134,8 +180,10 @@ class Case:
         return np.array(self.params.sigma_chol[:nu * nu], np.float32).reshape(nu, nu)
 
     def sinv(self):
-        """The float32 Sigma^-1 K3 weights the SIMPLE-mode perturbation cost with."""
-        nu = self.nu
+        """The float32 Sigma^-1 K3 weights the SIMPLE-mode perturbation cost with (n x n Sigma_H^-1 for H)."""
+        nu, n = self.nu, self.n
+        if self.kind == "H":
+            return self.dist[1 + 2 * n * n:].reshape(n, n)
         if self.kind == "M2":
             return np.diag(np.float32(1) / self.dist[1:1 + nu].astype(np.float32))
         if self.kind == "C":
@@ -146,14 +194,34 @@ class Case:
         return row_floats(self.T, self.nu, self.kind)
 
 
+def horizon_sigma(T, sig0, sigma_h="iid", tau=3.0):
+    """Sigma_H of an H case: "iid" I_T (x) Sigma0; "corr" exp(-|t - t'| / tau) (x) Sigma0; a number c: the correlated one with its
+    eigenvalues spread geometrically (order and eigenvectors kept) to condition number c."""
+    sig0 = np.asarray(sig0, np.float64)
+    if sigma_h == "iid":
+        return np.kron(np.eye(T), sig0)
+    t = np.arange(T)
+    S = np.kron(np.exp(-np.abs(t[:, None] - t[None, :]) / tau), sig0)
+    if sigma_h == "corr":
+        return S
+    w, V = np.linalg.eigh(S)
+    if len(w) > 1:
+        pw = math.log(float(sigma_h)) / math.log(w[-1] / w[0])
+        w = w[-1] * (w / w[-1]) ** pw
+    S = (V * w) @ V.T
+    return 0.5 * (S + S.T)
+
+
 def make_case(T, nu, K, mode="simple", gamma=0.95, lam=0.5, kind="W", sigma=None, filter_u=False, update_lambda=False, u_min=None, u_max=None,
-              u_init=None, seed=3, **kw):
-    """(model, params[, dist]) of one generated case through make_params.  `gamma` is used in MEAN mode ("halton-spline")."""
+              u_init=None, seed=3, sigma_h="corr", **kw):
+    """(model, params[, dist]) of one generated case through make_params.  `gamma` is used in MEAN mode ("halton-spline"); `sigma_h`
+    chooses Sigma_H of an H case (``horizon_sigma``)."""
     sig = corr_sigma(nu, seed=seed) if sigma is None else np.asarray(sigma, np.float64)
     if kind == "M2":
         sig = np.diag(np.diag(sig))
+    cov_type = {"C": "full", "H": "horizon"}.get(kind, "diag")
     mc = MPPIConfig(num_samples=K, horizon=T, mppi_mode=mode, sampling_method="random", noise_sigma=sig.tolist(), lambda_=lam, sample_null_action=True,
-                    rollout_var_discount=gamma, filter_u=filter_u, update_cov=kind != "W", cov_type="full" if kind == "C" else "diag",
+                    rollout_var_discount=gamma, filter_u=filter_u, update_cov=kind != "W", cov_type=cov_type,
                     update_lambda=update_lambda, u_min=u_min if u_min is not None else [-1e3], u_max=u_max if u_max is not None else [1e3],
                     u_init=u_init if u_init is not None else 0.0, **kw)
     m = nu_model(nu)
@@ -164,6 +232,9 @@ def make_case(T, nu, K, mode="simple", gamma=0.95, lam=0.5, kind="W", sigma=None
     elif kind == "C":
         import adaptive_full_oracle as afo
         dist = afo.make_dist(lam, sig)
+    elif kind == "H":
+        import adaptive_horizon_oracle as aho
+        dist = aho.make_dist(lam, horizon_sigma(T, sig, sigma_h))
     return Case(m, p, T, nu, K, kind, sig, dist)
 
 
@@ -181,17 +252,28 @@ def k3_inputs(case, seed=0, spread=4.0, favour_tail=True):
 
     S_k spans about `spread` * lambda over the samples and sum_t |gamma^t c_tk| stays a few lambda, so the float32 error of S
     stays far below lambda (the gate then tests the weights, not only the argmin).  With `favour_tail` the samples of the last
-    (ragged) tile get S lower by 2 lambda: they carry a share of the weight that a kernel dropping them cannot hide."""
+    (ragged) tile get S lower by 2 lambda: they carry a share of the weight that a kernel dropping them cannot hide.
+    For H the noise is coloured by L_H over the whole horizon, and the last step of U is u_init = 0: U is what mppib_shift leaves
+    (``shifted_from``), which is where the device computes the SIMPLE-mode g = lambda Sigma_H^-1 U."""
     T, nu, K, lam = case.T, case.nu, case.K, case.lam
     rng = np.random.default_rng(seed)
     L = case.chol().astype(np.float64)
     NR = T * nu
-    if case.simple:
+    if case.kind == "H":
+        if case.simple:
+            U = (L @ rng.normal(0, 0.5 / math.sqrt(NR), NR)).reshape(T, nu)
+        else:
+            U = rng.normal(0, 0.1, (T, nu))
+        U[-1] = 0.0
+    elif case.simple:
         U = np.einsum("ij,tj->ti", L, rng.normal(0, 0.5 / math.sqrt(NR), (T, nu)))      # |L^-1 U| ~ 0.5: g.x ~ lambda / 2
     else:
         U = rng.normal(0, 0.1, (T, nu))
     U = U.astype(np.float32)
-    noise = np.einsum("ij,tjk->tik", L, rng.standard_normal((T, nu, K))).astype(np.float32)
+    if case.kind == "H":
+        noise = (L @ rng.standard_normal((NR, K))).reshape(T, nu, K).astype(np.float32)
+    else:
+        noise = np.einsum("ij,tjk->tik", L, rng.standard_normal((T, nu, K))).astype(np.float32)
     x = noise if case.simple else (U[:, :, None] + noise).astype(np.float32)
     g = 1.0 if case.simple else float(case.params.gamma)
     Gam = sum(abs(g) ** t for t in range(T)) if g != 0 else 1.0
@@ -200,6 +282,14 @@ def k3_inputs(case, seed=0, spread=4.0, favour_tail=True):
     if favour_tail:
         cost[0, WS_W * ((K - 1) // WS_W):] -= 2.0 * lam
     return np.ascontiguousarray(cost, np.float32), np.ascontiguousarray(x), U
+
+
+def shifted_from(U, seed=0):
+    """A U_prev whose mppib_shift is U (the last step of U must be u_init): U_prev[t + 1] = U[t], U_prev[0] arbitrary."""
+    Up = np.empty_like(U)
+    Up[1:] = U[:-1]
+    Up[0] = np.random.default_rng(seed).uniform(-1, 1, U.shape[1])
+    return Up
 
 
 # ---------------------------------------------------------------------------------------------------------------- K3 restatements
@@ -217,7 +307,10 @@ def k3_restate(case, cost, x, U, keep=None):
     with np.errstate(invalid="ignore"):
         S = (_gammas(case)[:, None] * c64).sum(0)
     if case.simple:
-        g = lam * (U64 @ case.sinv().astype(np.float64).T).reshape(-1)       # g_r = lambda sum_j Sinv_ij U_tj
+        if case.kind == "H":
+            g = lam * (case.sinv().astype(np.float64) @ U64.reshape(-1))      # g = lambda Sigma_H^-1 U over the horizon
+        else:
+            g = lam * (U64 @ case.sinv().astype(np.float64).T).reshape(-1)   # g_r = lambda sum_j Sinv_ij U_tj
         S = S + g @ x64
     ok = np.isfinite(S) if keep is None else np.isfinite(S) & keep
     b = S[ok].min() if ok.any() else np.inf
@@ -231,7 +324,20 @@ def k3_restate(case, cost, x, U, keep=None):
         C = (d * np.tile(w, T)[None]) @ d.T
         i, j = np.tril_indices(nu)
         row.append(C[i, j])
+    elif case.kind == "H":
+        row.append(hz_C(case, x, U, w))
     return S, w, np.concatenate(row)
+
+
+def hz_C(case, x, U, w, k0=0, k1=None):
+    """Packed lower triangle of C = sum_k w_k (x_k - c)(x_k - c)^T over the samples [k0, k1) (float64; c = U in MEAN mode, else 0)."""
+    n, K = case.n, case.K
+    k1 = K if k1 is None else k1
+    d = np.asarray(x, np.float64).reshape(n, K)[:, k0:k1]
+    if not case.simple:
+        d = d - np.asarray(U, np.float64).reshape(n, 1)
+    C = (d * w[None, k0:k1]) @ d.T
+    return C[np.tril_indices(n)]
 
 
 def k3_S32(case, cost, x, U):
@@ -247,7 +353,16 @@ def k3_S32(case, cost, x, U):
     terms = [(gp[t], cost[t]) for t in range(T)]
     T4 = (T + 3) & ~3
     terms += [(f(0), cost[T - 1])] * (T4 - T)
-    if case.simple:
+    if case.simple and case.kind == "H":
+        si, Uf = case.sinv().astype(f), np.asarray(U, f).reshape(NR)
+        acc = np.zeros(NR, f)
+        for c in range(NR):                                                     # mppib_shift: a row per thread, columns in order
+            acc = (acc + si[:, c] * Uf[c]).astype(f)
+        g = (acc * f(case.lam)).astype(f)
+        xr = np.asarray(x, f).reshape(NR, K)
+        terms += [(g[r], xr[r]) for r in range(NR)]
+        terms += [(f(0), xr[NR - 1])] * (((NR + 3) & ~3) - NR)
+    elif case.simple:
         si, Uf = case.sinv().astype(f), np.asarray(U, f).reshape(T, nu)
         g = np.zeros(NR, f)
         for t in range(T):
@@ -278,18 +393,25 @@ def k3_dS(case, cost, x, U):
     n = (T + 3) // 4 * 4 + ((NR + 3) // 4 * 4 if case.simple else 0)          # terms of the four chains
     dS = (n / 4 + 6 + 2 * math.log(2) * lg * T) * A
     if case.simple:
-        gabs = lam * (np.abs(np.asarray(U, np.float64)) @ np.abs(case.sinv().astype(np.float64)).T).reshape(-1)
-        dS = dS + (n / 4 + nu + 6) * (gabs @ np.abs(np.asarray(x, np.float64).reshape(NR, K)))
+        if case.kind == "H":                                                    # g sums n terms (mppib_shift), not nu
+            gabs, inner = lam * (np.abs(case.sinv().astype(np.float64)) @ np.abs(np.asarray(U, np.float64)).reshape(-1)), NR
+        else:
+            gabs, inner = lam * (np.abs(np.asarray(U, np.float64)) @ np.abs(case.sinv().astype(np.float64)).T).reshape(-1), nu
+        dS = dS + (n / 4 + inner + 6) * (gabs @ np.abs(np.asarray(x, np.float64).reshape(NR, K)))
     return EPS * dS
 
 
-def k3_gate(case, cost, x, U, S, w):
-    """Element-wise bound on |row_kernel - row_reference| for the case's row kind (S, w: of ``k3_restate``)."""
+def k3_gate(case, cost, x, U, S, w, sms=NUM_SMS):
+    """Element-wise bound on |row_kernel - row_reference| for the case's row kind (S, w: of ``k3_restate``; sms: of the device).
+
+    The C of H (the SYRK) recomputes every weight from K3's float32 S_k and beta = row[0] with one expf, so a weight carries the
+    spread of S and beta (w_hi - w) plus a few roundings; each entry is then a sample-ordered FFMA sum over a chunk of kchunk
+    samples and a fold of ksplit chunk sums:  |dC_ij| <= sum_k |dx_ik| |dx_jk| (dw_k + (kchunk + ksplit + 4) eps w_k)."""
     T, nu, K, lam = case.T, case.nu, case.K, case.lam
     NR = T * nu
     _, ncons, _, _ = ws_layout(T, nu, case.kind)
     ntiles = (K + WS_W - 1) // WS_W
-    grid = min(ntiles, NUM_SMS)
+    grid = min(ntiles, sms)
     per_cta = -(-ntiles // grid)
     per_warp = -(-per_cta // ncons)
     rho = EPS * (64 + 3 * per_warp + grid / 4)
@@ -311,7 +433,32 @@ def k3_gate(case, cost, x, U, S, w):
         M = (d * np.tile(dw + (T + 8) * EPS * w, T)[None]) @ d.T + EPS * ((d * np.tile(w, T)[None]) @ d.T)
         i, j = np.tril_indices(nu)
         gate.append(M[i, j])
+    elif case.kind == "H":
+        _, ksplit, kchunk = syrk_split(NR, K, sms)
+        d = np.abs(x64 - c)
+        gate.append((((d * ((w_hi - w) + (kchunk + ksplit + 4) * EPS * w)[None]) @ d.T))[np.tril_indices(NR)])
     return np.concatenate(gate)
+
+
+def hz_k1_gate(L, z, U, a_ref):
+    """Per-element bound on |a_kernel - a_ref| of the horizon K1 against the float32-rounded float64 colouring of the device's own white
+    draws z [n][K]: row r sums r + 1 products in column order, so |da_r| <= eps ((r + 2) sum_{c<=r} |L_rc z_c| + |U_r|) + eps |a_ref|.
+    Clamping is monotone and adds nothing."""
+    n = L.shape[0]
+    Lz = np.abs(np.asarray(L, np.float64)) @ np.abs(np.asarray(z, np.float64).reshape(n, -1))
+    r = np.arange(n, dtype=np.float64)[:, None]
+    return EPS * ((r + 2) * Lz + np.abs(np.asarray(U, np.float64)).reshape(n, 1) + np.abs(np.asarray(a_ref, np.float64)).reshape(n, -1))
+
+
+def hz_k1_f32(L, z, U):
+    """float32 restatement of the horizon K1 before clamping: U_r + sum_c L_rc z_c accumulated in column order from c = 0."""
+    f = np.float32
+    n = L.shape[0]
+    Lf, zf = np.asarray(L, f), np.asarray(z, f).reshape(n, -1)
+    acc = np.zeros_like(zf)
+    for c in range(n):
+        acc = (acc + Lf[:, c:c + 1] * zf[c:c + 1]).astype(f)
+    return (np.asarray(U, f).reshape(n, 1) + acc).astype(f)
 
 
 def drop_tail_mask(K):

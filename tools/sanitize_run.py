@@ -36,6 +36,9 @@ CASES = [
      [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]),
     ("point robot, cov_type horizon (horizon-colour library K1, savgol K4; n = 36)",
      lambda: point_cfg(K=256 * world, T=12, device=dev, update_cov=True, cov_type="horizon"), PointReachObjective, [0.1, 0.0, 0.0]),
+    ("point robot, cov_type horizon at n = 255 (ragged K against the 64-sample K1 tile and the SYRK chunks, SYRK-fused K4 with 127 KB of "
+     "shared memory)", lambda: point_cfg(K=4100 * world, T=85, device=dev, update_cov=True, update_lambda=True, cov_type="horizon", filter_u=True),
+     PointReachObjective, [0.1, 0.0, 0.0]),
     ("panda pick (team K2: contacts, 16-lane articulation in 2 passes, compact layout)", lambda: pick_cfg(K=64 * world, T=9, device=dev), PandaPickObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0, 0.02, 0.02]),
 ]
 for name, mk, obj, q in CASES:
