@@ -100,6 +100,7 @@ class Scene:
     root_state0: np.ndarray               # (A,13) float32 initial root states
     dof_state0: np.ndarray                # (2*ndof,) interleaved
     contact_slot: Dict[int, int] = field(default_factory=dict)  # env rigid-body index -> slot
+    shape_bodies: frozenset = frozenset()  # env rigid-body indices that own a collision shape (slotted or not)
     ndof: int = 0
     nu: int = 0
     virtual_dofs: int = 0                 # leading virtual joints of a planar (differential-drive) base: x, y, yaw
@@ -366,7 +367,7 @@ def build_scene(actor_cfgs: list, gravity=(0.0, 0.0, -9.8), assets_dirs=None, su
         dof0[4] = math.atan2(2 * (qw * qz + qx * qy), 1 - 2 * (qy * qy + qz * qz))
     return Scene(model=m, robot=robot, actor_cfgs=actor_cfgs, actor_names=[a.name for a in actor_cfgs],
                  robot_actor=ra, body_names=body_names, body_offset=body_offset, free_actor=free_actor,
-                 root_state0=root0, dof_state0=dof0, contact_slot=contact_slot, ndof=ndof, nu=int(m.nu), virtual_dofs=nvirt)
+                 root_state0=root0, dof_state0=dof0, contact_slot=contact_slot, shape_bodies=frozenset(sh["body"] for sh in shapes), ndof=ndof, nu=int(m.nu), virtual_dofs=nvirt)
 
 
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:

@@ -30,7 +30,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ..model.blob import (OBS_CONTACT, OBS_DOF_STATE, OBS_FREE_STATE, OBS_LINK_STATE, MppibParams, Scene, build_scene,
+from ..model.blob import (MAX_SLOTS, OBS_CONTACT, OBS_DOF_STATE, OBS_FREE_STATE, OBS_LINK_STATE, MppibParams, Scene, build_scene,
                           make_params, obs_width)
 from ..utils.config_store import ActorWrapper, IsaacGymConfig, MPPIConfig, load_actor_cfgs
 
@@ -296,7 +296,12 @@ class RolloutSim:
         rb = self.find_actor_rigid_body_index(actor_idx, link_name)
         if rb in self.scene.contact_slot:
             return self._rows(OBS_CONTACT, self.scene.contact_slot[rb], 3)
-        return torch.zeros((1, 3), dtype=torch.float32, device=self.device).expand(self._n(), 3)
+        if rb in self.scene.shape_bodies:
+            # the body collides, but the rollout kernel reports no force for it: zeros would silently drop a collision term
+            raise ObservationError(
+                f"net contact force of '{actor_name}' / '{link_name}': the body has a collision shape but no contact-force slot; "
+                f"forces are reported for at most {MAX_SLOTS} bodies (non-robot bodies first, then robot links while slots remain)")
+        return torch.zeros((1, 3), dtype=torch.float32, device=self.device).expand(self._n(), 3)     # no collision shape: no force
 
     def get_dof_state(self):
         return self._dof_state

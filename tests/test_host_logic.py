@@ -506,3 +506,68 @@ def test_jackal_four_wheel_differential_drive():
     assert abs(adv - 0.5) < 0.03 and abs(st[2, 0] - s0[2]) < 1e-3            # straight: 0.5 m in 1 s, no yaw
     assert abs((st[2, 1] - s0[2]) - 1.0) < 0.06                              # omega = 1 rad/s for 1 s
     assert abs(st[7 + wheels["front_left_wheel"], 0] - 0.5 / r) < 0.05      # wheel speed v / r
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# net contact forces: at most MAX_SLOTS bodies get a force slot; a read of any other colliding body is refused
+# ---------------------------------------------------------------------------------------------------------------------
+def _boxes(n):
+    from mppi_isaac_b200.utils.config_store import ActorWrapper
+    return [ActorWrapper(type="box", name=f"box{i}", size=[0.1, 0.1, 0.1], init_pos=[3.0 + 0.5 * i, -3.0, 0.05], fixed=True) for i in range(n)]
+
+
+class _ContactReadObjective:
+    """Distance to the goal plus the net contact force of each named (actor, link) -- the shape of the push and pick costs."""
+
+    def __init__(self, reads):
+        self.reads = reads
+
+    def reset(self):
+        pass
+
+    def compute_cost(self, sim):
+        r = sim.get_actor_link_by_name("point_robot", "base_link")
+        cost = torch.linalg.norm(r[:, 0:2] - sim.get_actor_position_by_name("goal")[:, 0:2], axis=1)
+        for actor, link in self.reads(sim):
+            cost = cost + torch.sum(torch.abs(sim.get_actor_contact_forces_by_name(actor, link)), axis=1)
+        return cost
+
+
+def test_contact_force_read_without_a_slot_is_refused():
+    """Nine static boxes: the first eight get the eight force slots, the ninth collides without one.  An Objective that reads
+    its force is refused while the planner traces it, instead of seeing zeros."""
+    cfg = point_cfg(K=16, T=9)
+    cfg.actors = list(cfg.actors) + _boxes(9)
+    with pytest.raises(ObservationError, match=r"'box8'.*no contact-force slot.*at most 8 bodies"):
+        make(cfg, _ContactReadObjective(lambda s: [("box8", "box")]))
+    # robot links that collide lost their slots to the boxes: refused as well
+    with pytest.raises(ObservationError, match="no contact-force slot"):
+        make(cfg, _ContactReadObjective(lambda s: [("point_robot", "base_link")]))
+
+
+def test_contact_force_read_of_a_slotted_or_shapeless_body_builds():
+    cfg = point_cfg(K=16, T=9)
+    cfg.actors = list(cfg.actors) + _boxes(9)
+    reads = [("box0", "box"), ("box7", "box"), ("point_robot", "base_link_x"), ("goal", "sphere")]
+    p = make(cfg, _ContactReadObjective(lambda s: reads))
+    sc = p.sim.scene
+    assert len(sc.contact_slot) == 8 and sc.body_offset[2 + 8] in sc.shape_bodies and sc.body_offset[2 + 8] not in sc.contact_slot
+    a = p.compute_action([0.1, 0.0, 0.0], [0.0, 0.0, 0.0])
+    assert torch.isfinite(a).all()
+    s = p.sim
+    assert s.get_actor_contact_forces_by_name("box0", "box").shape == (144, 3)
+    for actor, link in reads[2:]:                                   # no collision shape: the force really is zero
+        f = s.get_actor_contact_forces_by_name(actor, link)
+        assert f.shape == (144, 3) and f.stride(0) == 0 and float(f.abs().max()) == 0.0
+
+
+def test_obstacle_rebuild_retraces_and_refuses_the_ninth_obstacle():
+    """compute_action(obst=...) adds sphere actors and rebuilds the simulator; the re-trace refuses an Objective that reads
+    the force on an obstacle that got no slot (the ninth)."""
+    def spheres(n):
+        return {f"o{i}": {"position": [2.0 + 0.6 * i, -2.0, 0.1], "velocity": [0.0, 0.0, 0.0], "size": [0.1]} for i in range(n)}
+    p = make(point_cfg(K=16, T=9), _ContactReadObjective(lambda s: [(a.name, "sphere") for a in s.env_cfg if a.name.startswith("sphere")]))
+    a = p.compute_action([0.1, 0.0, 0.0], [0.0, 0.0, 0.0], obst=spheres(8))
+    assert torch.isfinite(a).all() and len(p.sim.scene.contact_slot) == 8
+    with pytest.raises(ObservationError, match=r"'sphere8'.*no contact-force slot"):
+        p.compute_action([0.1, 0.0, 0.0], [0.0, 0.0, 0.0], obst=spheres(9))
