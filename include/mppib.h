@@ -239,6 +239,16 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
                      uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row,
                      float* actions, float* noise, void* stream);
 
+/* K1 (colored variant, `sampling_method: colored`): the white draws z[t][i] of mppib_sample (same counters and transform) are
+ * first correlated over the horizon, w[t][i] = sum_{t' <= t} Lt[t][t'] z[t'][i], with Lt[T][T] (caller-owned device memory,
+ * row-major, lower) the Cholesky factor of the power-law temporal covariance, then coloured over the controls, clamped and
+ * stored as in mppib_sample (the fixed Sigma, or the live diagonal / full one of a registered distribution with update_cov).
+ * Both sums run in a fixed order: with Lt = I the result equals mppib_sample's bit for bit.  Needs T <= 256, T*nu <= 512 and
+ * no cov_horizon.                                                                                                          */
+int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr,
+                             uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row,
+                             const float* Lt, float* actions, float* noise, void* stream);
+
 /* Halton-spline noise library (mppi_torch `sampling_method: halton` / `mppi_mode: halton-spline`, conf/mppi/panda.yaml:4-5;
  * SURVEY.md 8(a) M4, 8(f) N3): Gaussian knots from a scrambled Halton sequence (dimension n*nu + i, bases / digit multipliers
  * in halton_tab[2][n_knots*nu], index = global sample + 1), z = sqrt(2) erfinv(2u - 1), interpolated to T points by the fixed

@@ -24,7 +24,7 @@ SYMBOLS = [
     "mppib_set_model", "mppib_state_size", "mppib_obs_size", "mppib_sample", "mppib_rollout",
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
-    "mppib_set_distribution",
+    "mppib_set_distribution", "mppib_sample_colored",
 ]
 
 
@@ -146,6 +146,20 @@ class CudaBackend:
         self.launches += 1
         self._check(self.lib.mppib_sample(self.handle, C.c_uint64(seed), C.c_uint64(plan_idx), _ptr(plan_ctr), C.c_uint32(k_offset), C.c_uint32(k_total),
                                           _ptr(U), _ptr(prior_row), _ptr(actions), _ptr(noise), self._stream()), "mppib_sample")
+
+    def sample_colored(self, seed, plan_idx, k_offset, k_total, U, prior_row, Lt, actions, noise, plan_ctr=None):
+        """K1 with time-correlated noise: the draws of ``sample`` correlated over the horizon by the lower (T, T) float32 device
+        tensor ``Lt`` (``planner.mppi.colored_noise_chol``) before the control-space colour."""
+        T, n = int(self.params.T), int(self.params.T) * int(self.model.nu) * int(self.params.K)
+        if tuple(Lt.shape) != (T, T) or Lt.dtype != torch.float32 or not Lt.is_contiguous():
+            raise RuntimeError(f"mppib_sample_colored: Lt must be a contiguous float32 ({T}, {T}) tensor, got {Lt.dtype} {tuple(Lt.shape)}")
+        for name, t in (("actions", actions), ("noise", noise)):
+            if t is not None and t.numel() != n:
+                raise RuntimeError(f"mppib_sample_colored: {name} must hold T*nu*K = {n} floats, got {t.numel()}")
+        self.launches += 1
+        self._check(self.lib.mppib_sample_colored(self.handle, C.c_uint64(seed), C.c_uint64(plan_idx), _ptr(plan_ctr), C.c_uint32(k_offset),
+                                                  C.c_uint32(k_total), _ptr(U), _ptr(prior_row), _ptr(Lt), _ptr(actions), _ptr(noise),
+                                                  self._stream()), "mppib_sample_colored")
 
     def noise_library(self, k_offset, k_total, halton_tab, B, n_knots, Z):
         self.launches += 1

@@ -215,6 +215,14 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
     return launch_sample(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, actions, noise, (cudaStream_t)stream);
 }
 
+int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                             const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, void* stream) {
+    MPPIB_REQUIRE(h && U && Lt && actions, "mppib_sample_colored: null argument");
+    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_colored: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
+    MPPIB_ON_DEVICE(h);
+    return launch_sample_colored(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, (cudaStream_t)stream);
+}
+
 int32_t mppib_noise_library(MppibHandle h, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int32_t n_knots,
                             float* Z, void* stream) {
     MPPIB_REQUIRE(h && halton_tab && B && Z, "mppib_noise_library: null argument");

@@ -111,6 +111,8 @@ static inline PeerArgs peer_args(const MppibContext* c) {
 // kernel launchers (defined in the .cu files)
 int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s);
+int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                          const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s);
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s);
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,

@@ -32,33 +32,15 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
     z0 = r * c; z1 = r * s;
 }
 
-// DIAG (adaptive MPPI with update_cov): noise_j = sqrt(cov_j) z_j with cov = dist[1..nu], the live diagonal covariance; the Philox
-// counters, clamping and the null / prior rows are those of the fixed-Sigma kernel.
-// FULL (update_cov with cov_full): noise = L z with L = dist[1 + nu*nu ..], the live lower Cholesky factor, summed in the order of the
-// fixed-Sigma kernel.
-template <bool DIAG, bool FULL = false>
-__global__ void __launch_bounds__(128)
-mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
-              const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
-              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
+// The control-space colour, clamp and store of one (t, k) of every Philox K1: noise_j = sum_{i <= j} L0[j][i] z_i with the fixed
+// Sigma's Cholesky factor, summed from i = 0 upwards; DIAG (adaptive MPPI with update_cov): sqrt(cov_j) z_j with cov = dist[1..nu],
+// the live diagonal covariance; FULL (update_cov with cov_full): the live lower Cholesky factor L = dist[1 + nu*nu ..] in the same
+// order.  a = clamp(U + noise) with the null / prior rows, noise := a - U.
+template <bool DIAG, bool FULL>
+__device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int t, int k, bool is_null,
+                                                   bool is_prior, const float* __restrict__ U, const float* __restrict__ prior_row,
+                                                   float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
     const int K = p.K;
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    const int t = blockIdx.y;
-    if (k >= K) return;
-    const uint32_t kg = k_offset + (uint32_t)k;
-    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
-    const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
-    float z[MPPIB_MAX_NU];
-#pragma unroll
-    for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk) {
-        if (blk * 4 < nu) {
-            uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
-            box_muller(r.x, r.y, z[4 * blk], z[4 * blk + 1]);
-            box_muller(r.z, r.w, z[4 * blk + 2], z[4 * blk + 3]);
-        }
-    }
-    const bool is_null = p.sample_null_action && kg == k_total - 1;
-    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
 #pragma unroll
     for (int j = 0; j < MPPIB_MAX_NU; ++j) {
         if (j >= nu) break;
@@ -84,6 +66,134 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
         actions[idx] = a;
         if (noise) noise[idx] = a - u;
     }
+}
+
+// DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block).
+template <bool DIAG, bool FULL = false>
+__global__ void __launch_bounds__(128)
+mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+              const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
+              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
+    const int K = p.K;
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    const int t = blockIdx.y;
+    if (k >= K) return;
+    const uint32_t kg = k_offset + (uint32_t)k;
+    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
+    const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
+    float z[MPPIB_MAX_NU];
+#pragma unroll
+    for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk) {
+        if (blk * 4 < nu) {
+            uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
+            box_muller(r.x, r.y, z[4 * blk], z[4 * blk + 1]);
+            box_muller(r.z, r.w, z[4 * blk + 2], z[4 * blk + 3]);
+        }
+    }
+    const bool is_null = p.sample_null_action && kg == k_total - 1;
+    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
+    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+}
+
+// The white Philox draws of a tile of S samples [k0, k0 + S) to shared memory, zs[(t*nu + i) * S + sample]: the draws of the
+// fixed-Sigma kernel (counter (global sample, t, block)), spread over the CTA.
+template <int S>
+__device__ __forceinline__ void stage_white_tile(float* zs, int T, int nu, int k0, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+                                                 const uint32_t* __restrict__ plan_ctr, uint32_t k_offset) {
+    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
+    const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
+    const int nblk = (nu + 3) / 4;
+    for (int idx = threadIdx.x; idx < S * T * nblk; idx += blockDim.x) {
+        const int sl = idx % S, rest = idx / S, blk = rest % nblk, t = rest / nblk;
+        const uint32_t kg = k_offset + (uint32_t)(k0 + sl);
+        const uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
+        float z[4];
+        box_muller(r.x, r.y, z[0], z[1]);
+        box_muller(r.z, r.w, z[2], z[3]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+            if (4 * blk + e < nu) zs[(t * nu + 4 * blk + e) * S + sl] = z[e];
+    }
+}
+
+// COLORED (sampling_method: colored): time-correlated noise w[t][i] = sum_{t' <= t} L_b[t][t'] z[t'][i] over the white draws of
+// the fixed-Sigma kernel, with L_b = Lt[T][T] the lower Cholesky factor of the power-law temporal covariance, then the control-space
+// colour, clamp and store of colour_clamp_store (fixed L0, or DIAG / FULL the live adaptive ones).  A CTA of 128 threads owns a tile
+// of CL_S = 32 samples, lane = sample: the tile's white draws go to shared memory, then warp w takes the row pairs (t, T-1-t),
+// t = w, w + 4, ..., so that every warp sums about the same number of terms and every shared-memory load of z feeds two rows.  The
+// rows of L_b are read with warp-uniform loads (one L1 line per row segment, shared by all CTAs).  Both sums run in a fixed order
+// (t' and i from 0 upwards), so a sample's noise depends only on its global index; with L_b = I the temporal sum adds only exact
+// zeros before z[t][i] itself, and the result is that of mppib_sample_kernel bit for bit.
+constexpr int CL_S = 32;            // samples per CTA
+constexpr int CL_MAX_T = 256;
+constexpr int CL_MAX_N = 512;       // T*nu: the tile's draws take CL_MAX_N * CL_S * 4 = 64 KB of shared memory
+
+template <bool DIAG, bool FULL>
+__global__ void __launch_bounds__(128)
+mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+                            const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
+                            const float* __restrict__ prior_row, const float* __restrict__ Lt, float* __restrict__ actions,
+                            float* __restrict__ noise, const float* __restrict__ dist) {
+    extern __shared__ __align__(16) float cs[];
+    const int K = p.K, T = p.T;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int k0 = blockIdx.x * CL_S, k = k0 + lane;
+    stage_white_tile<CL_S>(cs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
+    __syncthreads();
+    const uint32_t kg = k_offset + (uint32_t)k;
+    const bool is_null = p.sample_null_action && kg == k_total - 1;
+    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
+    const float* zl = cs + lane;
+    for (int tl = warp; tl < (T + 1) / 2; tl += 4) {
+        const int th = T - 1 - tl;                                            // th >= tl; th == tl for the middle row of an odd T
+        const float* Llo = Lt + (size_t)tl * T;
+        const float* Lhi = Lt + (size_t)th * T;
+        float wl[MPPIB_MAX_NU], wh[MPPIB_MAX_NU];
+#pragma unroll
+        for (int i = 0; i < MPPIB_MAX_NU; ++i) { wl[i] = 0.f; wh[i] = 0.f; }
+        int tp = 0;
+        for (; tp <= tl; ++tp) {
+            const float a = __ldg(Llo + tp), b = __ldg(Lhi + tp);
+            const float* zr = zl + tp * nu * CL_S;
+#pragma unroll
+            for (int i = 0; i < MPPIB_MAX_NU; ++i) {
+                if (i >= nu) break;
+                const float zv = zr[i * CL_S];
+                wl[i] = fmaf(a, zv, wl[i]);
+                wh[i] = fmaf(b, zv, wh[i]);
+            }
+        }
+        for (; tp <= th; ++tp) {
+            const float b = __ldg(Lhi + tp);
+            const float* zr = zl + tp * nu * CL_S;
+#pragma unroll
+            for (int i = 0; i < MPPIB_MAX_NU; ++i) {
+                if (i >= nu) break;
+                wh[i] = fmaf(b, zr[i * CL_S], wh[i]);
+            }
+        }
+        if (k >= K) continue;
+        colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+        if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+    }
+}
+
+template <bool DIAG, bool FULL>
+int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                            const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
+    const int K = c->params.K, T = c->params.T, nu = c->model.nu;
+    const int smem = (int)sizeof(float) * T * nu * CL_S;
+    static int smem_attr[64] = {0};
+    int& attr = smem_attr[c->device & 63];
+    if (smem > attr) {
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_colored_kernel<DIAG, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr = smem;
+    }
+    mppib_sample_colored_kernel<DIAG, FULL><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
+                                                                                     plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
+                                                                                     DIAG || FULL ? c->dist : nullptr);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 // generalised Halton: radical inverse of `index` in base b with multiplicative digit scrambling (digit -> mult * digit mod b)
@@ -212,20 +322,7 @@ mppib_sample_horizon_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             zs[idx] = k < K ? Z[(size_t)r * K + k] : 0.f;
         }
     } else {
-        const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
-        const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
-        const int nblk = (nu + 3) / 4;
-        for (int idx = tid; idx < HZ_S * T * nblk; idx += blockDim.x) {
-            const int sl = idx % HZ_S, rest = idx / HZ_S, blk = rest % nblk, t = rest / nblk;
-            const uint32_t kg = k_offset + (uint32_t)(k0 + sl);
-            const uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
-            float z[4];
-            box_muller(r.x, r.y, z[0], z[1]);
-            box_muller(r.z, r.w, z[2], z[3]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-                if (4 * blk + e < nu) zs[(t * nu + 4 * blk + e) * HZ_S + sl] = z[e];
-        }
+        stage_white_tile<HZ_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
     }
     const float* Ld = dist + 1 + (size_t)n * n;
     for (int r0 = 0; r0 < n; r0 += 32) {
@@ -338,4 +435,15 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                                                           prior_row, actions, noise, nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                          const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
+    const int T = c->params.T, nu = c->model.nu;
+    MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
+    MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
+                  CL_MAX_N, T, T * nu);
+    if (adaptive_full(c)) return launch_sample_colored_t<false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    if (adaptive_cov(c)) return launch_sample_colored_t<true, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    return launch_sample_colored_t<false, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
 }

@@ -401,6 +401,14 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     p.cov_horizon = int(cov_type == "horizon")
     if p.cov_horizon and p.T * nu > HZ_MAX_N:
         raise ValueError(f"cov_type: horizon adapts a (T*nu) x (T*nu) covariance with T*nu <= {HZ_MAX_N}; T*nu = {p.T * nu}")
+    beta = float(getattr(mppi_cfg, "noise_beta", 2.0))
+    if not (math.isfinite(beta) and beta >= 0.0):
+        raise ValueError(f"noise_beta = {beta} must be finite and >= 0")
+    if str(getattr(mppi_cfg, "sampling_method", "halton")) == "colored":
+        if p.cov_horizon:
+            raise ValueError("sampling_method: colored excludes cov_type: horizon, whose Sigma_H already models the time correlation")
+        if p.T > 256 or p.T * nu > 512:
+            raise ValueError(f"sampling_method: colored needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
     p.u_scale = float(mppi_cfg.u_scale)
     p.sample_null_action = int(bool(mppi_cfg.sample_null_action))
     p.filter_u = int(bool(mppi_cfg.filter_u))

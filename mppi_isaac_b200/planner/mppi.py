@@ -80,6 +80,34 @@ def halton_spline_operator(T: int, n_knots: int):
     return B.astype(np.float32)
 
 
+def colored_noise_cov(T: int, beta: float):
+    """(T, T) float64 temporal covariance of power-law (1/f^beta) noise, normalised to unit diagonal: the covariance of the
+    `powerlaw_psd_gaussian` FFT recipe (iCEM), Sigma[t][t'] = c(|t - t'|) / c(0) with c(tau) = sum_{m=0}^{T//2} a_m s_m^2
+    cos(2 pi m tau / T), s_m = max(m, 1)^(-beta/2) (the recipe's fmin = 1/T), a_0 = a_{T/2} (T even) = 1, a_m = 2 otherwise.
+    Circulant with eigenvalues proportional to s_m^2 > 0, so positive definite; exactly I at beta = 0."""
+    import numpy as np
+    if beta == 0.0:
+        return np.eye(T)
+    m = np.arange(T // 2 + 1)
+    a = np.full(m.shape, 2.0)
+    a[0] = 1.0
+    if T % 2 == 0:
+        a[-1] = 1.0
+    w = a * np.maximum(m, 1).astype(np.float64) ** (-float(beta))
+    ch = w @ np.cos(2.0 * np.pi * np.outer(m, m) / T)               # c(tau), tau = 0 .. T // 2
+    lag = np.arange(T)
+    c = ch[np.minimum(lag, T - lag)]                                # c(T - tau) = c(tau) exactly: circulant to the bit
+    tau = np.abs(lag[:, None] - lag[None, :])
+    return c[tau] / c[0]
+
+
+def colored_noise_chol(T: int, beta: float):
+    """(T, T) float32 lower Cholesky factor of ``colored_noise_cov``, computed in float64: the temporal colour of K1's
+    ``sampling_method: colored`` (include/mppib.h mppib_sample_colored)."""
+    import numpy as np
+    return np.linalg.cholesky(colored_noise_cov(T, beta)).astype(np.float32)
+
+
 def shard_samples(k_total: int, rank: int, world: int):
     """Split k_total samples over `world` ranks in units of 4 (128-bit loads need K_local % 4 == 0)."""
     if k_total % 4 != 0:
@@ -118,9 +146,12 @@ class MPPIPlanner:
         self.world = 1
         if torch.distributed.is_available() and torch.distributed.is_initialized():
             self.world = torch.distributed.get_world_size(self.pg)
-        if str(cfg.sampling_method) not in ("random", "halton"):
+        if str(cfg.sampling_method) not in ("random", "halton", "colored"):
             raise ValueError(f"unknown sampling_method {cfg.sampling_method}")
         self.use_library = str(cfg.sampling_method) == "halton"     # Halton-spline noise library, drawn once (SURVEY 8(a) M4)
+        # power-law noise correlated over the horizon, drawn fresh on every plan (DESIGN.md section 2); make_params checks noise_beta
+        self.use_colored = str(cfg.sampling_method) == "colored"
+        self.noise_beta = float(getattr(cfg, "noise_beta", 2.0))
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))
@@ -251,6 +282,9 @@ class MPPIPlanner:
         self._plans = 0
         if self.use_library:
             self._build_library()
+        self._noise_Lt = None
+        if self.use_colored:                             # the temporal Cholesky factor of the horizon, once per planner
+            self._noise_Lt = torch.from_numpy(colored_noise_chol(T, self.noise_beta)).to(dev)
 
     def _build_library(self):
         """Halton-spline perturbations Z[T][nu][K]: scrambled-Halton Gaussian knots (T//4 per control, at least degree+1) interpolated
@@ -269,6 +303,8 @@ class MPPIPlanner:
         be = self.backend
         if self.use_library:
             be.sample_library(self.k_offset, self.K_total, self.U, None, self.Z, self.actions, self.noise)
+        elif self.use_colored:
+            be.sample_colored(self.seed, 0, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise, self.plan_ctr)
         else:
             be.sample(self.seed, 0, self.k_offset, self.K_total, self.U, None, self.actions, self.noise, self.plan_ctr)
 

@@ -29,7 +29,7 @@ class MPPIConfig:
     num_samples: int = 100
     horizon: int = 30
     mppi_mode: str = "halton-spline"     # halton-spline | simple
-    sampling_method: str = "halton"      # halton | random
+    sampling_method: str = "halton"      # halton | random | colored
     noise_sigma: Optional[List[List[float]]] = None
     noise_mu: Optional[List[float]] = None
     device: str = "cuda:0"
@@ -37,6 +37,7 @@ class MPPIConfig:
     update_lambda: bool = False
     update_cov: bool = False
     cov_type: str = "diag"               # update rule of update_cov: diag | full | horizon (T*nu <= 256) (DESIGN.md section 2)
+    noise_beta: float = 2.0              # sampling_method colored: power-law exponent of the temporal spectrum, 0 = white (DESIGN.md section 2)
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0
