@@ -52,7 +52,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 16
+#define MPPIB_ABI_VERSION 17
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -89,6 +89,8 @@ extern "C" {
 /* MPPI update modes (mppi_torch `mppi_mode`, conf/mppi/panda.yaml:4 / omnipanda_effort.yaml:4) */
 #define MPPIB_MODE_SIMPLE 0   /* U += sum_k w_k noise_k, cost += lambda U^T Sigma^-1 noise, gamma = 1 */
 #define MPPIB_MODE_MEAN   1   /* "halton-spline" rule: mean <- (1-a) mean + a sum_k w_k action_k, discounted cost */
+#define MPPIB_MODE_CEM    2   /* iCEM rule: the E best samples (elites) by discounted cost; U, sigma <- momentum step towards their mean / std */
+#define MPPIB_CEM_MAX_ELITES 128
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -212,6 +214,10 @@ typedef struct MppibParams {
     int32_t cov_full;          /* with update_cov: adapt a full Sigma (K1 draws L z, K3 appends C, K4 updates Sigma, L, Sigma^-1) */
     int32_t cov_horizon;       /* with update_cov: adapt one Sigma_H over the whole sequence, n = T*nu <= 256 (not with cov_full) */
     float   sigma0[MPPIB_MAX_NU * MPPIB_MAX_NU];    /* cov_horizon: Sigma0 = noise_sigma, row major nu x nu, the block a shift appends */
+    /* MODE_CEM (see "Cross-entropy planning" below); sigma_chol must be diagonal, its diagonal is sigma0_j = sqrt(Sigma_jj)      */
+    int32_t n_elites;          /* E, 1 .. MPPIB_CEM_MAX_ELITES                                                                   */
+    int32_t n_keep;            /* E_keep <= E elites of the last update carried into the next samples (rows K_total - 3 - e)     */
+    float   elite_alpha;       /* momentum alpha in [0, 1]: U <- (1 - alpha) mean + alpha U, sigma <- (1 - alpha) std + alpha sigma */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -370,6 +376,25 @@ int32_t mppib_set_distribution(MppibHandle h, float* dist);
  * increments *plan_ctr (device, nullable) by one.  With update_cov, cov_horizon and a registered distribution it also computes
  * g = lambda Sigma_H^-1 U of the shifted U once per plan, which K3 reads in SIMPLE mode.                                     */
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
+
+/* Cross-entropy planning (mode MPPIB_MODE_CEM, `mppi_mode: cem`, iCEM).  The distribution is diagonal and per step: the mean U[T][nu]
+ * and sigma[T][nu], both in the CEM state, a device buffer registered with mppib_set_distribution (NR = T*nu, E = n_elites):
+ *   state    [2 + E + NR + E*NR]  (carry offset, elites valid, S_elite[E], sigma[T][nu], elites[E][T][nu]); offset and flag are 0.0 / 1.0
+ * One plan is mppib_shift, then I iterations of K1 -> K2 -> cost -> mppib_reduce (+ mppib_finalize); nothing on the host changes
+ * between iterations but plan_idx, so the whole plan is one CUDA graph.
+ *   K1     mppib_sample_colored only (white noise: Lt = I): a = clamp(U + sigma (.) w); global rows K_total - 3 - e, e < n_keep, copy
+ *          clamp(elites[e][t + off]) with off = the carry offset (the row's own draw where t + off = T) once the elites are valid.
+ *   K3     mppib_reduce / mppib_reduce_finalize with x = actions: S_k = sum_t gamma^t cost[t][k] in t order (+0 for -0), key =
+ *          (S_k, global index) lexicographically, non-finite S never an elite.  The shard row holds the shard's E smallest keys in
+ *          order and their actions:
+ *   partial  [4-aligned 2E + E*NR]  (S_e, index bits as float)[E], actions[E][T][nu]; a missing entry is (+inf, 0xFFFFFFFF, zeros)
+ *   K4     mppib_finalize (or the last CTA of mppib_reduce_finalize) merges the G*E candidates into the global E smallest keys --
+ *          the elite set does not depend on G -- and, with E finite elites, sets m = mean_e a_e, s = sqrt(mean_e (a_e - m)^2) in
+ *          elite-rank order, U <- (1 - alpha) m + alpha U, sigma <- (1 - alpha) s + alpha sigma, stores the elites and their S and sets
+ *          the carry offset to 0; with fewer it leaves U, sigma, the elites and the offset as they are.  Then Savitzky-Golay, clamp,
+ *          first action and mirror as in the other modes; stats = (S of the best elite, S of the E-th).
+ *   shift  U as in the other modes, sigma <- sigma0 for every t, carry offset <- 1, *plan_ctr += 1.
+ * mppib_sample and mppib_sample_library refuse this mode.                                                                   */
 
 #ifdef __cplusplus
 }

@@ -46,6 +46,16 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     MPPIB_REQUIRE(!p->cov_full || p->update_cov, "cov_full selects the update rule of update_cov and needs update_cov");
     MPPIB_REQUIRE(!p->cov_horizon || (p->update_cov && !p->cov_full), "cov_horizon selects the update rule of update_cov: it needs update_cov and excludes cov_full");
     MPPIB_REQUIRE(!p->cov_horizon || p->T * m->nu <= MPPIB_HZ_MAX_N, "cov_horizon: n = T*nu = %d exceeds %d", p->T * m->nu, MPPIB_HZ_MAX_N);
+    MPPIB_REQUIRE(p->mode >= MPPIB_MODE_SIMPLE && p->mode <= MPPIB_MODE_CEM, "mode %d unknown", p->mode);
+    if (p->mode == MPPIB_MODE_CEM) {
+        MPPIB_REQUIRE(p->n_elites >= 1 && p->n_elites <= MPPIB_CEM_MAX_ELITES, "mode cem: n_elites = %d out of range [1, %d]", p->n_elites, MPPIB_CEM_MAX_ELITES);
+        MPPIB_REQUIRE(p->n_keep >= 0 && p->n_keep <= p->n_elites, "mode cem: n_keep = %d out of range [0, n_elites = %d]", p->n_keep, p->n_elites);
+        MPPIB_REQUIRE(p->elite_alpha >= 0.f && p->elite_alpha <= 1.f, "mode cem: elite_alpha = %g outside [0, 1]", p->elite_alpha);
+        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "mode cem excludes update_cov and update_lambda");
+        MPPIB_REQUIRE(p->T <= 256 && p->T * m->nu <= 512, "mode cem needs T <= 256 and T*nu <= 512, got T = %d, T*nu = %d", p->T, p->T * m->nu);
+        for (int j = 0; j < m->nu; ++j)
+            for (int i = 0; i < m->nu; ++i) MPPIB_REQUIRE(i == j || p->sigma_chol[j * m->nu + i] == 0.f, "mode cem needs a diagonal noise_sigma");
+    }
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -252,6 +262,7 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
     MPPIB_REQUIRE(h && cost && x && U && partial, "mppib_reduce: null argument");
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
+    if (cem_mode(h)) return launch_elite(h, cost, x, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     return launch_reduce(h, cost, x, U, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
@@ -259,6 +270,7 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
     MPPIB_REQUIRE(h && cost && x && U && partial && action_out, "mppib_reduce_finalize: null argument");
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
+    if (cem_mode(h)) return launch_elite(h, cost, x, partial, U, action_out, stats, (cudaStream_t)stream);
     return launch_reduce(h, cost, x, U, partial, U, action_out, stats, (cudaStream_t)stream);
 }
 
@@ -269,6 +281,7 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
     }
     MPPIB_ON_DEVICE(h);
+    if (cem_mode(h)) return launch_cem_finalize(h, partials, G, U, action_out, stats, (cudaStream_t)stream);
     return launch_finalize(h, partials, G, U, action_out, stats, (cudaStream_t)stream);
 }
 
@@ -308,6 +321,7 @@ int32_t mppib_set_distribution(MppibHandle h, float* dist) {
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream) {
     MPPIB_REQUIRE(h && U, "mppib_shift: null argument");
     MPPIB_ON_DEVICE(h);
+    if (cem_mode(h)) return launch_cem_shift(h, U, plan_ctr, (cudaStream_t)stream);
     return launch_shift(h, U, plan_ctr, (cudaStream_t)stream);
 }
 

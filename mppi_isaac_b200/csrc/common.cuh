@@ -80,11 +80,16 @@ struct DeviceGuard {
 // Floats of one shard row (beta, eta, W[T*nu] and, with update_cov, M2[T*nu], or with cov_full too C[nu(nu+1)/2]).  Buffers are
 // sized by the flags alone, so that registering a distribution never needs a reallocation; the kernels append M2 / C only when a
 // distribution is registered too.
+// MODE_CEM: the shard row (S, index bits)[E] + actions[E][T*nu], padded to 4 floats; the CEM state (include/mppib.h)
+__host__ __device__ static inline int cem_row_floats(int T, int nu, int E) { return (2 * E + E * T * nu + 3) & ~3; }
+static inline int cem_state_floats(int T, int nu, int E) { return 2 + E + T * nu + E * T * nu; }
 static inline int partial_row_capacity(const MppibParams& p, int nu) {
+    if (p.mode == MPPIB_MODE_CEM) return cem_row_floats(p.T, nu, p.n_elites);
     if (p.update_cov && p.cov_full) return 2 + p.T * nu + nu * (nu + 1) / 2;
     if (p.update_cov && p.cov_horizon) return 2 + p.T * nu + p.T * nu * (p.T * nu + 1) / 2;
     return 2 + p.T * nu * (p.update_cov ? 2 : 1);
 }
+static inline bool cem_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_CEM; }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
 static inline bool adaptive_horizon(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_horizon; }
@@ -123,6 +128,11 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
                   float* fin_stats, cudaStream_t s);
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s);
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s);
+// MODE_CEM (elite.cu): the elite kernel (+ the fused K4 when fin_U != NULL), K4 and the shift
+int launch_elite(MppibContext* c, const float* cost, const float* x, float* partial, float* fin_U, float* fin_action, float* fin_stats,
+                 cudaStream_t s);
+int launch_cem_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s);
+int launch_cem_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s);
 int alloc_horizon(MppibContext* c);           // (re)sizes the hz_* buffers for the handle's K and T*nu (frees them without cov_horizon)
 long long rollout_smem_bytes(const MppibModel& m);
 // K2, lanes-per-rollout mapping for serial chains without contacts (rollout_lanes.cu)

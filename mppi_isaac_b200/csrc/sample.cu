@@ -116,6 +116,34 @@ __device__ __forceinline__ void stage_white_tile(float* zs, int T, int nu, int k
     }
 }
 
+// CEM (mppi_mode: cem): the colour, clamp and store of one (t, k) with the per-step diagonal sigma[t][j] of the CEM state
+// (include/mppib.h): a = clamp(U + sigma (.) w), the product rounded on its own as colour_clamp_store rounds L0[j][j] z_j, so a diagonal
+// Sigma with sigma = sigma0 draws what colour_clamp_store draws, bit for bit.  Once the state holds elites, global rows
+// k_total - 3 - e (e < n_keep) copy clamp(elites[e][t + off]), off = the state's carry offset; a row whose t + off = T keeps its draw.
+__device__ __forceinline__ void cem_clamp_store(const MppibParams& p, int nu, const float (&w)[MPPIB_MAX_NU], int t, int k, uint32_t kg,
+                                                uint32_t k_total, bool is_null, bool is_prior, const float* __restrict__ U,
+                                                const float* __restrict__ prior_row, float* __restrict__ actions, float* __restrict__ noise,
+                                                const float* __restrict__ state) {
+    const int K = p.K, NR = p.T * nu;
+    const float* sig = state + 2 + p.n_elites;
+    const float* el = sig + NR;
+    const uint32_t e = k_total - 3u - kg;                                     // carried row e when kg = k_total - 3 - e
+    const int ts = t + (int)state[0];
+    const bool carried = state[1] != 0.f && kg + 3u <= k_total && e < (uint32_t)p.n_keep && ts < p.T;
+#pragma unroll
+    for (int j = 0; j < MPPIB_MAX_NU; ++j) {
+        if (j >= nu) break;
+        const float u = U[t * nu + j];
+        float a = carried ? el[(size_t)e * NR + ts * nu + j] : u + __fmul_rn(sig[t * nu + j], w[j]);
+        if (is_null) a = 0.f;
+        a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+        if (is_prior) a = prior_row[t * nu + j];
+        const size_t idx = ((size_t)t * nu + j) * K + k;
+        actions[idx] = a;
+        if (noise) noise[idx] = a - u;
+    }
+}
+
 // COLORED (sampling_method: colored): time-correlated noise w[t][i] = sum_{t' <= t} L_b[t][t'] z[t'][i] over the white draws of
 // the fixed-Sigma kernel, with L_b = Lt[T][T] the lower Cholesky factor of the power-law temporal covariance, then the control-space
 // colour, clamp and store of colour_clamp_store (fixed L0, or DIAG / FULL the live adaptive ones).  A CTA of 128 threads owns a tile
@@ -128,7 +156,7 @@ constexpr int CL_S = 32;            // samples per CTA
 constexpr int CL_MAX_T = 256;
 constexpr int CL_MAX_N = 512;       // T*nu: the tile's draws take CL_MAX_N * CL_S * 4 = 64 KB of shared memory
 
-template <bool DIAG, bool FULL>
+template <bool DIAG, bool FULL, bool CEM = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
                             const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
@@ -173,12 +201,17 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             }
         }
         if (k >= K) continue;
-        colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, U, prior_row, actions, noise, dist);
-        if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+        if constexpr (CEM) {
+            cem_clamp_store(p, nu, wl, tl, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
+            if (th != tl) cem_clamp_store(p, nu, wh, th, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
+        } else {
+            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+        }
     }
 }
 
-template <bool DIAG, bool FULL>
+template <bool DIAG, bool FULL, bool CEM = false>
 int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                             const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T, nu = c->model.nu;
@@ -186,12 +219,12 @@ int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
     static int smem_attr[64] = {0};
     int& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_colored_kernel<DIAG, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_colored_kernel<DIAG, FULL, CEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr = smem;
     }
-    mppib_sample_colored_kernel<DIAG, FULL><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
-                                                                                     plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
-                                                                                     DIAG || FULL ? c->dist : nullptr);
+    mppib_sample_colored_kernel<DIAG, FULL, CEM><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
+                                                                                          plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
+                                                                                          DIAG || FULL || CEM ? c->dist : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -392,6 +425,7 @@ int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
 
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s) {
+    MPPIB_REQUIRE(!cem_mode(c), "mppib_noise_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
     if (adaptive_cov(c))
@@ -404,6 +438,7 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
 
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,
                           float* actions, float* noise, cudaStream_t s) {
+    MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -420,6 +455,7 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
 
 int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
+    MPPIB_REQUIRE(!cem_mode(c), "mppib_sample: mode cem samples through mppib_sample_colored (white noise: Lt = I)");
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -443,6 +479,10 @@ int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, con
     MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
     MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
                   CL_MAX_N, T, T * nu);
+    if (cem_mode(c)) {
+        MPPIB_REQUIRE(c->dist != nullptr, "mppib_sample_colored: mppi_mode cem needs its state registered with mppib_set_distribution");
+        return launch_sample_colored_t<false, false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    }
     if (adaptive_full(c)) return launch_sample_colored_t<false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
     if (adaptive_cov(c)) return launch_sample_colored_t<true, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
     return launch_sample_colored_t<false, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -28,7 +28,8 @@ DRIVE_VELOCITY, DRIVE_EFFORT = 0, 1
 OBS_LINK_STATE, OBS_DOF_STATE, OBS_FREE_STATE, OBS_CONTACT = 0, 1, 2, 3
 SHAPE_BOX, SHAPE_SPHERE = 0, 1
 OWNER_STATIC, OWNER_LINK, OWNER_FREE = 0, 1, 2
-MODE_SIMPLE, MODE_MEAN = 0, 1
+MODE_SIMPLE, MODE_MEAN, MODE_CEM = 0, 1, 2
+CEM_MAX_ELITES = 128
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -75,6 +76,7 @@ class MppibParams(C.Structure):
         ("update_cov", i32), ("update_lambda", i32), ("eta_u_bound", f32), ("eta_l_bound", f32),
         ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32), ("cov_full", i32),
         ("cov_horizon", i32), ("sigma0", f32 * (MAX_NU * MAX_NU)),
+        ("n_elites", i32), ("n_keep", i32), ("elite_alpha", f32),
     ]
 
 
@@ -370,6 +372,37 @@ def build_scene(actor_cfgs: list, gravity=(0.0, 0.0, -9.8), assets_dirs=None, su
                  root_state0=root0, dof_state0=dof0, contact_slot=contact_slot, shape_bodies=frozenset(sh["body"] for sh in shapes), ndof=ndof, nu=int(m.nu), virtual_dofs=nvirt)
 
 
+def _cem_params(p: MppibParams, mppi_cfg, nu: int) -> None:
+    """The `mppi_mode: cem` keys (DESIGN.md section 2, "Cross-entropy planning"): E elites, momentum alpha, E_keep = floor(xi E)
+    carried elites, I iterations per plan; the refusals of the mode."""
+    E = int(getattr(mppi_cfg, "n_elites", 10))
+    alpha = float(getattr(mppi_cfg, "elite_momentum", 0.1))
+    xi = float(getattr(mppi_cfg, "keep_elites", 0.3))
+    iters = int(getattr(mppi_cfg, "cem_iterations", 3))
+    k_total = int(mppi_cfg.num_samples)
+    if not 1 <= E <= CEM_MAX_ELITES:
+        raise ValueError(f"n_elites = {E} must lie in 1 .. {CEM_MAX_ELITES}")
+    if not 0.0 <= alpha <= 1.0:
+        raise ValueError(f"elite_momentum = {alpha} must lie in [0, 1]")
+    if not 0.0 <= xi <= 1.0:
+        raise ValueError(f"keep_elites = {xi} must lie in [0, 1]")
+    if iters < 1:
+        raise ValueError(f"cem_iterations = {iters} must be at least 1")
+    keep = int(math.floor(xi * E))
+    if E + keep + 2 > k_total:
+        raise ValueError(f"mppi_mode: cem needs n_elites + floor(keep_elites * n_elites) + 2 <= num_samples; {E} + {keep} + 2 > {k_total}")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("mppi_mode: cem has its own update rule and excludes update_cov and update_lambda")
+    if str(getattr(mppi_cfg, "sampling_method", "halton")) not in ("random", "colored"):
+        raise ValueError("mppi_mode: cem samples with sampling_method random or colored, not halton")
+    sigma = np.asarray(mppi_cfg.noise_sigma, np.float64).reshape(nu, nu)
+    if np.any(sigma != np.diag(np.diag(sigma))):
+        raise ValueError("mppi_mode: cem adapts a diagonal per-step sigma: noise_sigma must be diagonal")
+    if p.T > 256 or p.T * nu > 512:
+        raise ValueError(f"mppi_mode: cem needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
+    p.n_elites, p.n_keep, p.elite_alpha = E, keep, alpha
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -380,6 +413,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         p.mode, p.gamma = MODE_SIMPLE, 1.0
     elif mode == "halton-spline":
         p.mode, p.gamma = MODE_MEAN, float(mppi_cfg.rollout_var_discount)
+    elif mode == "cem":
+        p.mode, p.gamma = MODE_CEM, float(mppi_cfg.rollout_var_discount)
     else:
         raise ValueError(f"unknown mppi_mode {mode}")
     if not (math.isfinite(p.gamma) and p.gamma >= 0.0):     # gamma = 0 is legal: score only the first step
@@ -409,6 +444,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
             raise ValueError("sampling_method: colored excludes cov_type: horizon, whose Sigma_H already models the time correlation")
         if p.T > 256 or p.T * nu > 512:
             raise ValueError(f"sampling_method: colored needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
+    if p.mode == MODE_CEM:
+        _cem_params(p, mppi_cfg, nu)
     p.u_scale = float(mppi_cfg.u_scale)
     p.sample_null_action = int(bool(mppi_cfg.sample_null_action))
     p.filter_u = int(bool(mppi_cfg.filter_u))

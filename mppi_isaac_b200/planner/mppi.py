@@ -152,6 +152,10 @@ class MPPIPlanner:
         # power-law noise correlated over the horizon, drawn fresh on every plan (DESIGN.md section 2); make_params checks noise_beta
         self.use_colored = str(cfg.sampling_method) == "colored"
         self.noise_beta = float(getattr(cfg, "noise_beta", 2.0))
+        # iCEM (DESIGN.md section 2, "Cross-entropy planning"): the elites of each iteration move the mean U and a per-step sigma,
+        # both on the device; make_params checks the keys and refuses the combinations the mode excludes
+        self.cem = str(getattr(cfg, "mppi_mode", "")) == "cem"
+        self.cem_iterations = int(getattr(cfg, "cem_iterations", 3)) if self.cem else 1
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))
@@ -170,6 +174,8 @@ class MPPIPlanner:
         self.backend = sim.backend
         if self.adaptive and not hasattr(self.backend, "set_distribution"):
             raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
+        if self.cem and not hasattr(self.backend, "set_distribution"):
+            raise ValueError(f"mppi_mode: cem needs a backend with set_distribution ({type(self.backend).__name__} has none)")
         self._peer_exchange = False
         self._peer_capable = (self.world > 1 and getattr(self.backend, "name", "") == "cuda"
                               and os.environ.get("MPPIB_EXCHANGE", "peer") == "peer")
@@ -248,6 +254,9 @@ class MPPIPlanner:
             P = 2 + T * nu + nu * (nu + 1) // 2               # (beta, eta, W[T*nu]) + C[lower triangle] with cov_type full
         if self.cov_horizon:
             P = 2 + T * nu + T * nu * (T * nu + 1) // 2       # (beta, eta, W[n]) + C[lower triangle of n x n] with cov_type horizon
+        if self.cem:
+            E = int(self.backend.params.n_elites)
+            P = (2 * E + E * T * nu + 3) & ~3                 # (S, index)[E] + actions[E][T*nu] of mppi_mode cem, padded to 4
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
@@ -263,7 +272,15 @@ class MPPIPlanner:
         # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma), or with cov_type full (lambda, Sigma, L, Sigma^-1)
         # (horizon: the same of Sigma_H = I_T (x) Sigma, n = T*nu) computed in float64 and rounded; registered before the noise library is built (update_cov makes it white)
         self.dist = None
-        if not self.adaptive and hasattr(self.backend, "set_distribution"):
+        if self.cem:
+            # the CEM state (carry offset, elites valid, S_elite[E], sigma[T][nu], elites[E][T][nu]): sigma starts at sqrt(diag(Sigma))
+            E = int(self.backend.params.n_elites)
+            sigma0 = torch.sqrt(torch.diagonal(torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)))
+            state = torch.zeros((2 + E + T * nu + E * T * nu,), dtype=torch.float64)
+            state[2 + E:2 + E + T * nu] = sigma0.repeat(T)
+            self.dist = state.to(**f32)
+            self.backend.set_distribution(self.dist)
+        elif not self.adaptive and hasattr(self.backend, "set_distribution"):
             self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
         if self.adaptive:
             sigma = torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)
@@ -285,6 +302,8 @@ class MPPIPlanner:
         self._noise_Lt = None
         if self.use_colored:                             # the temporal Cholesky factor of the horizon, once per planner
             self._noise_Lt = torch.from_numpy(colored_noise_chol(T, self.noise_beta)).to(dev)
+        elif self.cem:                                   # cem with white noise runs the colored K1 with L_b = I
+            self._noise_Lt = torch.eye(T, dtype=torch.float32, device=dev)
 
     def _build_library(self):
         """Halton-spline perturbations Z[T][nu][K]: scrambled-Halton Gaussian knots (T//4 per control, at least degree+1) interpolated
@@ -299,9 +318,12 @@ class MPPIPlanner:
         self.Z = torch.zeros((T, nu, K), dtype=torch.float32, device=dev)
         self.backend.noise_library(self.k_offset, self.K_total, self._halton_tab, self._spline_B, n_knots, self.Z)
 
-    def _sample(self):
+    def _sample(self, iteration=0):
         be = self.backend
-        if self.use_library:
+        if self.cem:                                     # iteration i keys Philox with plan_idx = i << 32: iteration 0 draws what colored MPPI draws
+            be.sample_colored(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise,
+                              self.plan_ctr)
+        elif self.use_library:
             be.sample_library(self.k_offset, self.K_total, self.U, None, self.Z, self.actions, self.noise)
         elif self.use_colored:
             be.sample_colored(self.seed, 0, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise, self.plan_ctr)
@@ -316,10 +338,13 @@ class MPPIPlanner:
     def cov_action(self):
         """(nu,) device view of the diagonal sampling covariance of adaptive MPPI: adapted with update_cov, the constant diag(Sigma)
         with update_lambda alone, None with both flags off; with cov_type full the (nu, nu) view of the adapted Sigma, with
-        cov_type horizon the (T*nu, T*nu) view of Sigma_H.  ``lambda_`` stays the configured float; the live temperature is
-        ``current_lambda``."""
+        cov_type horizon the (T*nu, T*nu) view of Sigma_H; with mppi_mode cem the (T, nu) view of the per-step sigma (a standard
+        deviation).  ``lambda_`` stays the configured float; the live temperature is ``current_lambda``."""
         if self.dist is None:
             return None
+        if self.cem:
+            E = int(self.backend.params.n_elites)
+            return self.dist[2 + E:2 + E + self.T * self.nu].view(self.T, self.nu)
         if self.cov_horizon:
             n = self.T * self.nu
             return self.dist[1:1 + n * n].view(n, n)
@@ -329,8 +354,25 @@ class MPPIPlanner:
 
     @property
     def current_lambda(self):
-        """0-d device view of the live temperature of adaptive MPPI (None without update_cov / update_lambda)."""
-        return None if self.dist is None else self.dist[0]
+        """0-d device view of the live temperature of adaptive MPPI (None without update_cov / update_lambda, and with mppi_mode cem)."""
+        return None if self.dist is None or self.cem else self.dist[0]
+
+    @property
+    def elites(self):
+        """(E, T, nu) device view of the elites of the last CEM update, best first (None unless mppi_mode cem); ``elite_costs`` holds
+        their discounted costs.  Before the first update with E finite samples they are zeros."""
+        if not self.cem:
+            return None
+        E, n = int(self.backend.params.n_elites), self.T * self.nu
+        return self.dist[2 + E + n:2 + E + n + E * n].view(E, self.T, self.nu)
+
+    @property
+    def elite_costs(self):
+        """(E,) device view of the discounted costs S of ``elites`` (None unless mppi_mode cem)."""
+        if not self.cem:
+            return None
+        E = int(self.backend.params.n_elites)
+        return self.dist[2:2 + E]
 
     @property
     def perturbed_action(self):
@@ -371,9 +413,15 @@ class MPPIPlanner:
 
     def _plan_batched(self):
         be = self.backend
-        with _nvtx("mppi/shift+K1 sample"):
+        with _nvtx("mppi/shift"):
             be.shift(self.U, self.plan_ctr)
-            self._sample()
+        for i in range(self.cem_iterations):             # cem_iterations with mppi_mode cem, one otherwise
+            self._iterate_batched(i)
+
+    def _iterate_batched(self, iteration):
+        be = self.backend
+        with _nvtx("mppi/K1 sample"):
+            self._sample(iteration)
         with _nvtx("mppi/K2 rollout"):
             self.sim.rollout_all(self.actions)
         with _nvtx("mppi/objective cost"):
@@ -388,9 +436,13 @@ class MPPIPlanner:
             be.finalize(partials, G, self.U, self._action, self.stats)
 
     def _plan_stepwise(self, state):
+        self.backend.shift(self.U, self.plan_ctr)
+        for i in range(self.cem_iterations):             # cem_iterations with mppi_mode cem, one otherwise
+            state = self._iterate_stepwise(state, i)
+
+    def _iterate_stepwise(self, state, iteration):
         be, sim, T = self.backend, self.sim, self.T
-        be.shift(self.U, self.plan_ctr)
-        self._sample()
+        self._sample(iteration)
         sim.begin_step_mode()
         prior_local = self.use_priors and (self.k_offset <= self.K_total - 2 < self.k_offset + self.K)
         for t in range(T):
@@ -412,6 +464,7 @@ class MPPIPlanner:
         be.reduce(self.cost, x, self.U, self.partial)
         partials, G = self._exchange()
         be.finalize(partials, G, self.U, self._action, self.stats)
+        return state
 
     def _try_capture(self):
         dev = torch.device(self.device)

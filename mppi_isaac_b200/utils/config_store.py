@@ -28,7 +28,7 @@ BUILTIN_CONF = os.path.join(PKG_DIR, "conf")
 class MPPIConfig:
     num_samples: int = 100
     horizon: int = 30
-    mppi_mode: str = "halton-spline"     # halton-spline | simple
+    mppi_mode: str = "halton-spline"     # halton-spline | simple | cem
     sampling_method: str = "halton"      # halton | random | colored
     noise_sigma: Optional[List[List[float]]] = None
     noise_mu: Optional[List[float]] = None
@@ -38,6 +38,10 @@ class MPPIConfig:
     update_cov: bool = False
     cov_type: str = "diag"               # update rule of update_cov: diag | full | horizon (T*nu <= 256) (DESIGN.md section 2)
     noise_beta: float = 2.0              # sampling_method colored: power-law exponent of the temporal spectrum, 0 = white (DESIGN.md section 2)
+    n_elites: int = 10                   # mppi_mode cem (iCEM, DESIGN.md section 2): elites E in 1 .. 128
+    elite_momentum: float = 0.1          # mppi_mode cem: momentum alpha of the mean and sigma updates, in [0, 1]
+    keep_elites: float = 0.3             # mppi_mode cem: fraction xi of the elites carried into the next samples, floor(xi E) rows
+    cem_iterations: int = 3              # mppi_mode cem: sample / roll out / update iterations per plan, at least 1
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0

@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer over every kernel of libmppib.so (tools/sanitize_run.py): memcheck (out-of-bounds / misaligned global and shared
 # accesses, leaks of device memory), racecheck (shared-memory hazards: the mbarrier ring of K3, the per-rollout slots of K2, the
-# staged tiles of the horizon and colored K1 and the SYRK, the in-place Cholesky and inverse of the horizon K4),
+# staged tiles of the horizon and colored K1 and the SYRK, the elite kernel's sorts and last-CTA merge, the in-place Cholesky and inverse of the horizon K4),
 # synccheck (barrier / mbarrier misuse), and memcheck of the 2-GPU peer-memory exchange when two GPUs are visible.
 #   bash tools/sanitize.sh [outdir] [all|1gpu|2gpu]     (on the GPU box; writes <outdir>/sanitize_<tool>.log and a summary line per tool)
 set -u
