@@ -52,7 +52,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 17
+#define MPPIB_ABI_VERSION 18
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -90,6 +90,7 @@ extern "C" {
 #define MPPIB_MODE_SIMPLE 0   /* U += sum_k w_k noise_k, cost += lambda U^T Sigma^-1 noise, gamma = 1 */
 #define MPPIB_MODE_MEAN   1   /* "halton-spline" rule: mean <- (1-a) mean + a sum_k w_k action_k, discounted cost */
 #define MPPIB_MODE_CEM    2   /* iCEM rule: the E best samples (elites) by discounted cost; U, sigma <- momentum step towards their mean / std */
+#define MPPIB_MODE_SMOOTH 3   /* Smooth MPPI: U is the control DERIVATIVE; actions are integrated from the last executed action (see below) */
 #define MPPIB_CEM_MAX_ELITES 128
 
 typedef struct MppibModel {
@@ -218,6 +219,10 @@ typedef struct MppibParams {
     int32_t n_elites;          /* E, 1 .. MPPIB_CEM_MAX_ELITES                                                                   */
     int32_t n_keep;            /* E_keep <= E elites of the last update carried into the next samples (rows K_total - 3 - e)     */
     float   elite_alpha;       /* momentum alpha in [0, 1]: U <- (1 - alpha) mean + alpha U, sigma <- (1 - alpha) std + alpha sigma */
+    /* MODE_SMOOTH (see "Smooth MPPI" below); u_min / u_max bound the ACTION, these the derivative                                  */
+    float   du_min[MPPIB_MAX_NU];
+    float   du_max[MPPIB_MAX_NU];
+    float   smooth_weight;     /* omega >= 0: S_k += omega sum_t |a_t - a_{t-1}|^2 (t = 0 against the last executed action)        */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -395,6 +400,28 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
  *          first action and mirror as in the other modes; stats = (S of the best elite, S of the E-th).
  *   shift  U as in the other modes, sigma <- sigma0 for every t, carry offset <- 1, *plan_ctr += 1.
  * mppib_sample and mppib_sample_library refuse this mode.                                                                   */
+
+/* Smooth MPPI (mode MPPIB_MODE_SMOOTH, `mppi_mode: smooth`, after Kim, Kwon, Yoon, RA-L 2022).  U[T][nu] is the mean of the control
+ * DERIVATIVE v; the rolled-out and executed actions are its integral from the last executed action, so with derivative bounds the
+ * executed command changes by at most du_max * dt per plan.  noise_sigma is the covariance of the derivative noise, u_min / u_max
+ * bound the action, du_min / du_max the derivative, dt = MppibParams.dt is the integration step, gamma = 1.  The smooth state is a
+ * device buffer registered with mppib_set_smooth_state (caller-owned, initialised by the caller):
+ *   state    [nu + T*nu]  (a_prev[nu], A[T][nu]): the last executed action and the planned action sequence; only K4 writes it
+ *   K1     mppib_sample_smooth: per sample, t = 0 .. T-1 in order from a = a_prev: the white draws z of mppib_sample (same counters),
+ *          n = L0 z (colour_clamp_store's order), v = clamp(U[t] + n, du_min, du_max) (v = 0 on the null row), a_t = clamp(fmaf(v, dt,
+ *          a_{t-1}), u_min, u_max); actions = a_t, noise = v - U[t] where the action clamp did not bind, (a_t - a_{t-1})/dt - U[t]
+ *          where it did (the derivative actually applied)
+ *   K3     mppib_reduce / mppib_reduce_finalize with x = noise, as SIMPLE (gamma = 1, g = lambda Sigma^-1 U) plus the smoothness cost:
+ *          S_k = sum_t c[t][k] + sum_r g_r x_rk + omega dt^2 sum_r (U_r + x_rk)^2; the shard row is SIMPLE's [2 + T*nu]
+ *   K4     mppib_finalize (or the fused tail): U' = clamp(U + W/eta, du_min, du_max) (U' = U when eta = 0), then per j in t order from
+ *          a = a_prev: A_t = clamp(fmaf(U'_t, dt, a), u_min, u_max), U'_t := (A_t - a)/dt where that clamp bound, a = A_t; U <- U',
+ *          A stored, action_out and the mirror <- A_0, a_prev <- A_0; stats = (beta, eta).  filter_u is refused in this mode.
+ *   shift  U as in the other modes (the appended u_init is a derivative: 0 holds the last action), *plan_ctr += 1; A is not shifted.
+ * mppib_sample, mppib_sample_colored and the noise-library entry points refuse this mode; reduce and finalize refuse it while no
+ * state is registered.  A distribution registered with mppib_set_distribution is ignored in this mode.                      */
+int32_t mppib_set_smooth_state(MppibHandle h, float* state);
+int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset,
+                            uint32_t k_total, const float* U, float* actions, float* noise, void* stream);
 
 #ifdef __cplusplus
 }

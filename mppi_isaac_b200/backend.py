@@ -14,7 +14,7 @@ import weakref
 
 import torch
 
-from .model.blob import ABI_VERSION, MODE_CEM, MppibModel, MppibParams
+from .model.blob import ABI_VERSION, MODE_CEM, MODE_SMOOTH, MppibModel, MppibParams
 
 _LIB_PATH = os.environ.get("MPPIB_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libmppib.so")   # MPPIB_LIB: tuning builds
 _lib = None
@@ -24,7 +24,7 @@ SYMBOLS = [
     "mppib_set_model", "mppib_state_size", "mppib_obs_size", "mppib_sample", "mppib_rollout",
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
-    "mppib_set_distribution", "mppib_sample_colored",
+    "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth",
 ]
 
 
@@ -71,6 +71,11 @@ def dist_floats(params, nu):
     return 1 + nu, "(lambda, cov[nu])"
 
 
+def smooth_state_floats(T, nu):
+    """Floats of the smooth state of mppi_mode smooth: (a_prev[nu], A[T][nu])."""
+    return int(nu) + int(T) * int(nu)
+
+
 def cem_row_floats(T, nu, E):
     """Floats of one shard row of mppi_mode cem: (S, index bits)[E], actions[E][T*nu], padded to a multiple of 4."""
     return (2 * int(E) + int(E) * int(T) * int(nu) + 3) & ~3
@@ -104,6 +109,7 @@ class CudaBackend:
         self.params = None
         self._mirror_keepalive = None
         self._dist_keepalive = None
+        self._smooth_keepalive = None
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -121,6 +127,8 @@ class CudaBackend:
             self.set_action_mirror(self._mirror_keepalive)
         if self._dist_keepalive is not None:             # ... and keeps following the planner's adaptive distribution
             self.set_distribution(self._dist_keepalive)
+        if self._smooth_keepalive is not None:           # ... and the planner's smooth state
+            self.set_smooth_state(self._smooth_keepalive)
 
     def destroy(self):
         if self.handle:
@@ -168,6 +176,17 @@ class CudaBackend:
         self._check(self.lib.mppib_sample_colored(self.handle, C.c_uint64(seed), C.c_uint64(plan_idx), _ptr(plan_ctr), C.c_uint32(k_offset),
                                                   C.c_uint32(k_total), _ptr(U), _ptr(prior_row), _ptr(Lt), _ptr(actions), _ptr(noise),
                                                   self._stream()), "mppib_sample_colored")
+
+    def sample_smooth(self, seed, plan_idx, k_offset, k_total, U, actions, noise, plan_ctr=None):
+        """K1 of mppi_mode smooth: the draws of ``sample`` are derivatives, integrated from the registered state's last action
+        (``set_smooth_state``) into ``actions``; ``noise`` receives the applied derivative minus U."""
+        n = int(self.params.T) * int(self.model.nu) * int(self.params.K)
+        for name, t in (("actions", actions), ("noise", noise)):
+            if t is not None and t.numel() != n:
+                raise RuntimeError(f"mppib_sample_smooth: {name} must hold T*nu*K = {n} floats, got {t.numel()}")
+        self.launches += 1
+        self._check(self.lib.mppib_sample_smooth(self.handle, C.c_uint64(seed), C.c_uint64(plan_idx), _ptr(plan_ctr), C.c_uint32(k_offset),
+                                                 C.c_uint32(k_total), _ptr(U), _ptr(actions), _ptr(noise), self._stream()), "mppib_sample_smooth")
 
     def noise_library(self, k_offset, k_total, halton_tab, B, n_knots, Z):
         self.launches += 1
@@ -240,7 +259,14 @@ class CudaBackend:
 
     def _check_dist_fits(self, params, model, what):
         """The library keeps only a pointer to the registered distribution, so every change of (T, nu) or of the update rule is checked
-        against its length before the library sees it: a shorter buffer would be read past its end by the next K1, shift or K4."""
+        against its length before the library sees it: a shorter buffer would be read past its end by the next K1, shift or K4.  The
+        same holds for the smooth state of mppi_mode smooth."""
+        state = getattr(self, "_smooth_keepalive", None)
+        if state is not None and params.mode == MODE_SMOOTH:
+            need = smooth_state_floats(params.T, model.nu)
+            if state.numel() != need:
+                raise RuntimeError(f"{what}: the registered smooth state holds {state.numel()} floats, but T = {int(params.T)}, "
+                                   f"nu = {int(model.nu)} needs nu + T*nu = {need}; register a new one (set_smooth_state) first")
         if self._dist_keepalive is not None:
             need, layout = dist_floats(params, model.nu)
             if self._dist_keepalive.numel() != need:
@@ -257,6 +283,15 @@ class CudaBackend:
                 raise RuntimeError(f"mppib_set_distribution: {layout} = {need} floats, got {dist.numel()}")
         self._dist_keepalive = dist
         self._check(self.lib.mppib_set_distribution(self.handle, _ptr(dist)), "mppib_set_distribution")
+
+    def set_smooth_state(self, state):
+        """mppi_mode smooth: register the device tensor (a_prev[nu], A[T][nu]) that K1 reads and K4 updates (None switches it off)."""
+        if state is not None:
+            need = smooth_state_floats(self.params.T, self.model.nu)
+            if state.numel() != need:
+                raise RuntimeError(f"mppib_set_smooth_state: (a_prev[nu], A[T][nu]) = nu + T*nu = {need} floats, got {state.numel()}")
+        self._smooth_keepalive = state
+        self._check(self.lib.mppib_set_smooth_state(self.handle, _ptr(state)), "mppib_set_smooth_state")
 
     def reduce(self, cost, x, U, partial):
         self._check_row(partial, "mppib_reduce")

@@ -46,7 +46,16 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     MPPIB_REQUIRE(!p->cov_full || p->update_cov, "cov_full selects the update rule of update_cov and needs update_cov");
     MPPIB_REQUIRE(!p->cov_horizon || (p->update_cov && !p->cov_full), "cov_horizon selects the update rule of update_cov: it needs update_cov and excludes cov_full");
     MPPIB_REQUIRE(!p->cov_horizon || p->T * m->nu <= MPPIB_HZ_MAX_N, "cov_horizon: n = T*nu = %d exceeds %d", p->T * m->nu, MPPIB_HZ_MAX_N);
-    MPPIB_REQUIRE(p->mode >= MPPIB_MODE_SIMPLE && p->mode <= MPPIB_MODE_CEM, "mode %d unknown", p->mode);
+    MPPIB_REQUIRE(p->mode >= MPPIB_MODE_SIMPLE && p->mode <= MPPIB_MODE_SMOOTH, "mode %d unknown", p->mode);
+    if (p->mode == MPPIB_MODE_SMOOTH) {
+        MPPIB_REQUIRE(isfinite(p->smooth_weight) && p->smooth_weight >= 0.f, "mode smooth: smooth_weight = %g must be finite and >= 0", p->smooth_weight);
+        MPPIB_REQUIRE(p->dt > 0.f, "mode smooth: the integration step dt = %g must be positive", p->dt);
+        for (int j = 0; j < m->nu; ++j)
+            MPPIB_REQUIRE(p->du_min[j] <= p->du_max[j], "mode smooth: du_min[%d] = %g > du_max[%d] = %g", j, p->du_min[j], j, p->du_max[j]);
+        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "mode smooth excludes update_cov and update_lambda");
+        MPPIB_REQUIRE(!p->filter_u, "mode smooth excludes filter_u (the derivative is integrated, not smoothed)");
+        MPPIB_REQUIRE(p->T <= 256 && p->T * m->nu <= 512, "mode smooth needs T <= 256 and T*nu <= 512, got T = %d, T*nu = %d", p->T, p->T * m->nu);
+    }
     if (p->mode == MPPIB_MODE_CEM) {
         MPPIB_REQUIRE(p->n_elites >= 1 && p->n_elites <= MPPIB_CEM_MAX_ELITES, "mode cem: n_elites = %d out of range [1, %d]", p->n_elites, MPPIB_CEM_MAX_ELITES);
         MPPIB_REQUIRE(p->n_keep >= 0 && p->n_keep <= p->n_elites, "mode cem: n_keep = %d out of range [0, n_elites = %d]", p->n_keep, p->n_elites);
@@ -233,6 +242,14 @@ int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, co
     return launch_sample_colored(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, (cudaStream_t)stream);
 }
 
+int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                            const float* U, float* actions, float* noise, void* stream) {
+    MPPIB_REQUIRE(h && U && actions, "mppib_sample_smooth: null argument");
+    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_smooth: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
+    MPPIB_ON_DEVICE(h);
+    return launch_sample_smooth(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, actions, noise, (cudaStream_t)stream);
+}
+
 int32_t mppib_noise_library(MppibHandle h, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int32_t n_knots,
                             float* Z, void* stream) {
     MPPIB_REQUIRE(h && halton_tab && B && Z, "mppib_noise_library: null argument");
@@ -315,6 +332,12 @@ int32_t mppib_set_action_mirror(MppibHandle h, float* mirror) {
 int32_t mppib_set_distribution(MppibHandle h, float* dist) {
     MPPIB_REQUIRE(h != nullptr, "null handle");
     h->dist = dist;
+    return 0;
+}
+
+int32_t mppib_set_smooth_state(MppibHandle h, float* state) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    h->smooth = state;
     return 0;
 }
 

@@ -47,6 +47,7 @@ struct MppibContext {
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
     float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) or, with cov_full, (lambda, Sigma, L, Sigma^-1)
                                                // read by K1 / K3, updated by K4 (nullable)
+    float* smooth;                             // MODE_SMOOTH: device (a_prev[nu], A[T][nu]), read by K1, updated by K4 (nullable)
     // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
     float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
     float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
@@ -90,6 +91,7 @@ static inline int partial_row_capacity(const MppibParams& p, int nu) {
     return 2 + p.T * nu * (p.update_cov ? 2 : 1);
 }
 static inline bool cem_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_CEM; }
+static inline bool smooth_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_SMOOTH; }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
 static inline bool adaptive_horizon(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_horizon; }
@@ -118,6 +120,8 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s);
 int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                           const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s);
+int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                         const float* U, float* actions, float* noise, cudaStream_t s);
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s);
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,

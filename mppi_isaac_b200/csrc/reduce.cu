@@ -344,14 +344,62 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
     }
 }
 
+// K4 of mode smooth (smooth = (a_prev[nu], A[T][nu])): combine G rows (beta_g, eta_g, W_g) of stride P as finalize_rows does, the SIMPLE
+// update of the derivative U' = U + W/eta (U' = U when eta = 0), clamped to du_min / du_max; then one thread per j integrates it in t
+// order from a = a_prev: A_t = clamp(fmaf(U'_t, dt, a), u_min, u_max), U'_t := (A_t - a)/dt where that clamp bound, a = A_t.  U <- U',
+// A stored, the action, its mirror and a_prev <- A_0; stats = (beta, eta).  Thread j alone reads and writes column j of the state, and
+// every rank combines the same rows in the same order, so all write the same bits.  `un` = [T*nu + G] floats of shared memory.
+__device__ __forceinline__ void smooth_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
+                                            float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
+                                            float* __restrict__ smooth) {
+    const int T = p.T, NR = T * nu;
+    float* sg = un + NR;
+    const float inv_lambda = 1.0f / p.lambda_;
+    float b = INFINITY;
+    for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
+    for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
+        const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
+        sg[gidx] = eg > 0.f ? expf(-(__ldcg(&partials[(size_t)gidx * P]) - b) * inv_lambda) : 0.f;
+    }
+    __syncthreads();
+    float e = 0.f;
+    for (int gidx = 0; gidx < G; ++gidx) e += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 1]);
+    for (int r = threadIdx.x; r < NR; r += blockDim.x) {
+        float w = 0.f;
+        for (int gidx = 0; gidx < G; ++gidx) w += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + r]);
+        un[r] = U[r] + (e > 0.f ? w / e : 0.f);
+    }
+    __syncthreads();
+    const float dt = p.dt;
+    for (int j = threadIdx.x; j < nu; j += blockDim.x) {
+        const float lo = p.u_min[j], hi = p.u_max[j], dlo = p.du_min[j], dhi = p.du_max[j];
+        float a = smooth[j];
+        for (int t = 0; t < T; ++t) {
+            const int r = t * nu + j;
+            float v = fminf(fmaxf(un[r], dlo), dhi);
+            const float ah = fmaf(v, dt, a);
+            const float an = fminf(fmaxf(ah, lo), hi);
+            if (an != ah) v = (an - a) / dt;
+            U[r] = v;
+            smooth[nu + r] = an;
+            a = an;
+        }
+        const float first = smooth[nu + j];
+        smooth[j] = first;
+        action_out[j] = first;
+        if (action_mirror) action_mirror[j] = first;
+    }
+    if (threadIdx.x == 0 && stats) { stats[0] = b; stats[1] = e; }
+}
+
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
 // at least, `misc` = 8 floats.
-template <bool ADAPT, bool FULL = false>
+template <bool ADAPT, bool FULL = false, bool SMOOTH = false>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
-                                                float* __restrict__ dist) {
+                                                float* __restrict__ dist, float* __restrict__ smooth = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = (int)gridDim.x;
     float* sc = tiles;                   // [MAX_GRID] scale of every CTA partial (the ring is idle now)
@@ -424,7 +472,8 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             // cov -- in its prologue, before it took its ticket, so this CTA is the only reader left when it updates them.
             __threadfence();
             __syncthreads();
-            finalize_rows<ADAPT, FULL>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            if constexpr (SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
+            else finalize_rows<ADAPT, FULL>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
         }
     }
 }
@@ -449,9 +498,11 @@ constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
 // the fused K4 also keeps its covariance scratch there (full_fin_floats), which the ring stages of every accepted shape exceed.
 struct WsLayout {
     int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [NCONS][P4] warp partials | [8]
+    int us;                       // smooth: [NR4] U for the smoothness cost (no floats otherwise)
     int bar;                      // full[nstage], then empty[nstage] mbarriers
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
-    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W) {   // kind: what the shard row carries after W (RowKind)
+    // kind: what the shard row carries after W (RowKind)
+    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false) {
         const int NR = T * nu, P4 = (row_floats(T, nu, kind) + 3) & ~3;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
@@ -460,7 +511,8 @@ struct WsLayout {
         wk = gp + ((T + 3) & ~3);
         cpart = wk + 8 * WS_W;
         misc = cpart + WS_NCONS * P4;
-        bar = ((misc + 8) * 4 + 15) & ~15;
+        us = misc + 8;
+        bar = ((us + (smooth ? ((NR + 3) & ~3) : 0)) * 4 + 15) & ~15;
         bytes = bar + 2 * 8 * nstage + 128;
     }
 };
@@ -479,26 +531,28 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // HZN (update_cov with cov_horizon): the SIMPLE-mode g = lambda Sigma_H^-1 U is read from hz_g (mppib_shift computed it), phase B
 // stores every S_k (INFINITY for an invalid sample) to hz_S for the SYRK that follows, and the row this kernel writes is
 // (beta, eta, W[n]) only; the SYRK appends C.
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false>   // rows of W per lane: T*nu <= 32 * RPL
+// SMOOTH (mode smooth, x = the derivative noise): SIMPLE with gamma = 1, plus omega dt^2 sum_r (U_r + x_rk)^2 in phase A (U staged in
+// `us`, four chains in r order; skipped when omega = 0, so that the row is SIMPLE's), and the fused K4 integrates the state `smooth`.
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                        float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
-                       const float* __restrict__ hz_g) {
+                       const float* __restrict__ hz_g, float* __restrict__ smooth) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
-    const bool simple = p.mode == MPPIB_MODE_SIMPLE;
+    const bool simple = SMOOTH || p.mode == MPPIB_MODE_SIMPLE;
     const bool m2 = ADAPT && !FULL && !HZN && p.update_cov;
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
     const int P = 2 + (m2 ? 2 : 1) * NR + npairs;
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
-    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W);
+    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, SMOOTH);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -542,11 +596,12 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         }
         if (FULL && !simple && r < NR) acc = U[r];                            // phase A reads g in SIMPLE mode only
         g[r] = acc;
+        if (SMOOTH && r < NR) tiles[L.us + r] = U[r];
     }
     {
         // gamma^0 = 1 for every accepted gamma: log2f(0) * 0 would be NaN (validate refuses a negative or non-finite gamma)
         const float lg = log2f(p.gamma);
-        for (int t = tid; t < T4; t += NT) gp[t] = t == 0 ? 1.f : t < T ? exp2f(lg * (float)t) : 0.f;
+        for (int t = tid; t < T4; t += NT) gp[t] = t == 0 ? 1.f : t < T ? (SMOOTH ? 1.f : exp2f(lg * (float)t)) : 0.f;
     }
     __syncthreads();
 
@@ -605,7 +660,21 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                     a3 = fmaf(g4.w, xs[min(r + 3, NR - 1) * WS_W + lane], a3);
                 }
             }
-            const float sum = (a0 + a1) + (a2 + a3);
+            float sum = (a0 + a1) + (a2 + a3);
+            if constexpr (SMOOTH) {
+                if (p.smooth_weight != 0.f) {                                 // omega dt^2 sum_r (U_r + x_rk)^2
+                    const float* us = tiles + L.us;
+                    float q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
+                    int r = 0;
+                    for (; r + 4 <= NR; r += 4) {
+                        const float v0 = us[r] + xs[r * WS_W + lane], v1 = us[r + 1] + xs[(r + 1) * WS_W + lane];
+                        const float v2 = us[r + 2] + xs[(r + 2) * WS_W + lane], v3 = us[r + 3] + xs[(r + 3) * WS_W + lane];
+                        q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1); q2 = fmaf(v2, v2, q2); q3 = fmaf(v3, v3, q3);
+                    }
+                    for (; r < NR; ++r) { const float v = us[r] + xs[r * WS_W + lane]; q0 = fmaf(v, v, q0); }
+                    sum = fmaf(p.smooth_weight * p.dt * p.dt, (q0 + q1) + (q2 + q3), sum);
+                }
+            }
             // ---- B: tile minimum, weights, their sum
             const bool valid = (k0 + lane < K) && isfinite(sum);
             const float S = valid ? sum : INFINITY;
@@ -721,16 +790,17 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __syncthreads();
     if (!s_last_ws) return;
     __threadfence();
-    fold_and_finish<ADAPT, FULL>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist);
+    fold_and_finish<ADAPT, FULL, SMOOTH>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist,
+                                         smooth);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
-// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon).
-template <bool ADAPT, bool FULL = false, bool HZN = false>
+// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon); SMOOTH: smooth_rows.
+template <bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
-                float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig) {
+                float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const int T = p.T, NR = T * nu;
     int P = HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
@@ -759,7 +829,8 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
         partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
         P = peers.pcap;
     }
-    finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
+    if constexpr (SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
+    else finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
 }
 
@@ -953,27 +1024,27 @@ static PeerArgs reduce_peers(const MppibContext* c) {
     return a;
 }
 
-static int reduce_ws_stages(int T, int nu, int kind) {
+static int reduce_ws_stages(int T, int nu, int kind, bool smooth = false) {
     int ns = 8;
-    while (ns > 1 && WsLayout(T, nu, ns, kind).bytes > 224 * 1024) --ns;
+    while (ns > 1 && WsLayout(T, nu, ns, kind, smooth).bytes > 224 * 1024) --ns;
     return ns;
 }
 
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false>
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
     const int kind = FULL ? ROW_C : (ADAPT && c->params.update_cov) ? ROW_M2 : ROW_W;
-    const int nstage_max = reduce_ws_stages(T, nu, kind);
+    const int nstage_max = reduce_ws_stages(T, nu, kind, SMOOTH);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = WsLayout(T, nu, nstage, kind).bytes;
+    const size_t smem = WsLayout(T, nu, nstage, kind, SMOOTH).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -992,9 +1063,10 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
     PeerArgs peers = reduce_peers(c);
     if (HZN) peers.world = 0;                                                 // the row is complete only after the SYRK, which stores it
-    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch,
-                                                                    c->reduce_ticket, partial, peers, fin_U, fin_action, fin_stats,
-                                                                    fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g);
+    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
+                                                                            c->reduce_scratch, c->reduce_ticket, partial, peers, fin_U, fin_action,
+                                                                            fin_stats, fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g,
+                                                                            SMOOTH ? c->smooth : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1074,6 +1146,13 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(T, nu, ROW_C) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the covariance row of cov_full", T, nu);
     const int NR = T * nu;
+    if (smooth_mode(c)) {
+        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_reduce: mode smooth needs its state registered with mppib_set_smooth_state");
+        MPPIB_REQUIRE(reduce_ws_stages(T, nu, ROW_W, true) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages in mode smooth", T, nu);
+        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        return launch_reduce_ws_t<16, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
     if (adaptive_horizon(c)) {
         MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N, "mppib_reduce: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, NR);
         MPPIB_REQUIRE(c->hz_S != nullptr && c->hz_K == c->params.K && c->hz_n == NR, "mppib_reduce: cov_horizon buffers are not sized for K = %d, n = %d",
@@ -1100,7 +1179,11 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    if (adaptive_horizon(c)) {
+    if (smooth_mode(c)) {
+        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_finalize: mode smooth needs its state registered with mppib_set_smooth_state");
+        mppib_finalize_kernel<false, false, false, true><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats,
+                                                                                                peer_args(c), c->action_mirror, nullptr, nullptr, c->smooth);
+    } else if (adaptive_horizon(c)) {
         MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N && c->hz_sig != nullptr && c->hz_n == NR, "mppib_finalize: cov_horizon buffers are not sized for n = %d", NR);
         const int smem = hz_fin_smem(NR, G);
         MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: cov_horizon with n = %d and G = %d needs %d bytes of shared memory", NR, G, smem);
@@ -1111,18 +1194,18 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
             attr = smem;
         }
         mppib_finalize_kernel<true, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror,
-                                                                      c->dist, c->hz_sig);
+                                                                      c->dist, c->hz_sig, nullptr);
     } else if (adaptive_full(c)) {
         const size_t smem = (NR + G + full_fin_floats(c->params.T, c->model.nu)) * sizeof(float);
         mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                               nullptr);
+                                                               nullptr, nullptr);
     } else if (c->dist) {
         const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
         mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                         nullptr);
+                                                         nullptr, nullptr);
     } else {
         mppib_finalize_kernel<false><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                              c->action_mirror, nullptr, nullptr);
+                                                                              c->action_mirror, nullptr, nullptr, nullptr);
     }
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -229,6 +229,49 @@ int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
     return 0;
 }
 
+// SMOOTH (mppi_mode: smooth): the sampled derivative v = clamp(U + L0 z, du_min, du_max) is integrated over the horizon from the last
+// executed action a_prev = state[0..nu), a_t = clamp(fmaf(v_t, dt, a_{t-1}), u_min, u_max), and only actions and the applied derivative
+// noise = v - U (or (a_t - a_{t-1})/dt - U where the action clamp bound) are stored.  A CTA of 128 threads owns a tile of SM_S = 32
+// samples: all threads draw the tile's white draws into shared memory (the counters of the fixed-Sigma kernel), then lane = sample and
+// warp w carries the prefix of the controls j = w, w + 4, ... serially in t.  The colour sums i from 0 upwards as colour_clamp_store
+// does, so without a binding action clamp the noise is mppib_sample_kernel's bit for bit when that kernel clamps to du_min / du_max.
+constexpr int SM_S = 32;            // samples per CTA
+constexpr int SM_MAX_N = 512;       // T*nu: the tile's draws take SM_MAX_N * SM_S * 4 = 64 KB of shared memory
+
+__global__ void __launch_bounds__(128)
+mppib_sample_smooth_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+                           const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
+                           float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ state) {
+    extern __shared__ __align__(16) float zs[];
+    const int K = p.K, T = p.T;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int k0 = blockIdx.x * SM_S, k = k0 + lane;
+    stage_white_tile<SM_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
+    __syncthreads();
+    if (k >= K) return;
+    const bool is_null = p.sample_null_action && k_offset + (uint32_t)k == k_total - 1;
+    const float dt = p.dt;
+    const float* zl = zs + lane;
+    for (int j = warp; j < nu; j += 4) {
+        const float lo = p.u_min[j], hi = p.u_max[j], dlo = p.du_min[j], dhi = p.du_max[j];
+        const float* Lj = p.sigma_chol + j * nu;
+        float a = state[j];
+        for (int t = 0; t < T; ++t) {
+            const float* zr = zl + t * nu * SM_S;
+            float n = 0.f;
+            for (int i = 0; i <= j; ++i) n += Lj[i] * zr[i * SM_S];
+            const float u = U[t * nu + j];
+            const float v = is_null ? 0.f : fminf(fmaxf(u + n, dlo), dhi);
+            const float ah = fmaf(v, dt, a);
+            const float an = fminf(fmaxf(ah, lo), hi);
+            const size_t idx = ((size_t)t * nu + j) * K + k;
+            actions[idx] = an;
+            if (noise) noise[idx] = (an == ah ? v : (an - a) / dt) - u;
+            a = an;
+        }
+    }
+}
+
 // generalised Halton: radical inverse of `index` in base b with multiplicative digit scrambling (digit -> mult * digit mod b)
 __device__ __forceinline__ float halton(uint32_t index, uint32_t base, uint32_t mult) {
     const float inv_b = 1.0f / (float)base;
@@ -426,6 +469,7 @@ int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_noise_library: mode cem samples through mppib_sample_colored");
+    MPPIB_REQUIRE(!smooth_mode(c), "mppib_noise_library: mode smooth samples through mppib_sample_smooth");
     MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
     if (adaptive_cov(c))
@@ -439,6 +483,7 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,
                           float* actions, float* noise, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
+    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_library: mode smooth samples through mppib_sample_smooth");
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -456,6 +501,7 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
 int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample: mode cem samples through mppib_sample_colored (white noise: Lt = I)");
+    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample: mode smooth samples through mppib_sample_smooth");
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -476,6 +522,7 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
 int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                           const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu;
+    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_colored: mode smooth samples through mppib_sample_smooth");
     MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
     MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
                   CL_MAX_N, T, T * nu);
@@ -486,4 +533,23 @@ int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, con
     if (adaptive_full(c)) return launch_sample_colored_t<false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
     if (adaptive_cov(c)) return launch_sample_colored_t<true, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
     return launch_sample_colored_t<false, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+}
+
+int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                         const float* U, float* actions, float* noise, cudaStream_t s) {
+    const int K = c->params.K, T = c->params.T, nu = c->model.nu;
+    MPPIB_REQUIRE(smooth_mode(c), "mppib_sample_smooth: needs mode smooth (MPPIB_MODE_SMOOTH), the handle has mode %d", c->params.mode);
+    MPPIB_REQUIRE(c->smooth != nullptr, "mppib_sample_smooth: no smooth state registered (mppib_set_smooth_state)");
+    MPPIB_REQUIRE(T * nu <= SM_MAX_N, "mppib_sample_smooth: needs T*nu <= %d, got %d", SM_MAX_N, T * nu);
+    const int smem = (int)sizeof(float) * T * nu * SM_S;
+    static int smem_attr[64] = {0};
+    int& attr = smem_attr[c->device & 63];
+    if (smem > attr) {
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_smooth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr = smem;
+    }
+    mppib_sample_smooth_kernel<<<(K + SM_S - 1) / SM_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
+                                                                      k_offset, k_total, U, actions, noise, c->smooth);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }

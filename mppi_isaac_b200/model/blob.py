@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 17
+ABI_VERSION = 18
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -28,7 +28,7 @@ DRIVE_VELOCITY, DRIVE_EFFORT = 0, 1
 OBS_LINK_STATE, OBS_DOF_STATE, OBS_FREE_STATE, OBS_CONTACT = 0, 1, 2, 3
 SHAPE_BOX, SHAPE_SPHERE = 0, 1
 OWNER_STATIC, OWNER_LINK, OWNER_FREE = 0, 1, 2
-MODE_SIMPLE, MODE_MEAN, MODE_CEM = 0, 1, 2
+MODE_SIMPLE, MODE_MEAN, MODE_CEM, MODE_SMOOTH = 0, 1, 2, 3
 CEM_MAX_ELITES = 128
 
 f32, i32 = C.c_float, C.c_int32
@@ -77,6 +77,7 @@ class MppibParams(C.Structure):
         ("step_size_cov", f32), ("kappa", f32), ("lambda_mult", f32), ("cov_full", i32),
         ("cov_horizon", i32), ("sigma0", f32 * (MAX_NU * MAX_NU)),
         ("n_elites", i32), ("n_keep", i32), ("elite_alpha", f32),
+        ("du_min", f32 * MAX_NU), ("du_max", f32 * MAX_NU), ("smooth_weight", f32),
     ]
 
 
@@ -403,6 +404,34 @@ def _cem_params(p: MppibParams, mppi_cfg, nu: int) -> None:
     p.n_elites, p.n_keep, p.elite_alpha = E, keep, alpha
 
 
+def _smooth_params(p: MppibParams, mppi_cfg, nu: int, bc) -> None:
+    """The `mppi_mode: smooth` keys (DESIGN.md section 2, "Smooth MPPI"): the smoothness weight omega and the derivative bounds
+    du_min / du_max (length 1 broadcasts, None is unbounded); the refusals of the mode."""
+    w = float(getattr(mppi_cfg, "smooth_weight", 0.0))
+    if not (math.isfinite(w) and w >= 0.0):
+        raise ValueError(f"smooth_weight = {w} must be finite and >= 0")
+    dlo, dhi = bc(getattr(mppi_cfg, "du_min", None), -1e30), bc(getattr(mppi_cfg, "du_max", None), 1e30)
+    if len(dlo) != nu or len(dhi) != nu:
+        raise ValueError(f"du_min / du_max need 1 or nu = {nu} values, got {len(dlo)} / {len(dhi)}")
+    for j in range(nu):
+        if not float(np.float32(dlo[j])) <= float(np.float32(dhi[j])):
+            raise ValueError(f"du_min[{j}] = {dlo[j]} must not exceed du_max[{j}] = {dhi[j]}")
+    if not p.dt > 0.0:
+        raise ValueError(f"mppi_mode: smooth integrates the derivative over isaacgym.dt, which must be positive; dt = {p.dt}")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("mppi_mode: smooth excludes update_cov and update_lambda")
+    if p.filter_u:
+        raise ValueError("mppi_mode: smooth excludes filter_u: the actions are already smooth, switch filter_u off")
+    method = str(getattr(mppi_cfg, "sampling_method", "halton"))
+    if method != "random":
+        raise ValueError(f"mppi_mode: smooth samples its derivative with sampling_method random, not {method}")
+    if p.T > 256 or p.T * nu > 512:
+        raise ValueError(f"mppi_mode: smooth needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
+    p.smooth_weight = w
+    for j in range(nu):
+        p.du_min[j], p.du_max[j] = dlo[j], dhi[j]
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -415,6 +444,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         p.mode, p.gamma = MODE_MEAN, float(mppi_cfg.rollout_var_discount)
     elif mode == "cem":
         p.mode, p.gamma = MODE_CEM, float(mppi_cfg.rollout_var_discount)
+    elif mode == "smooth":
+        p.mode, p.gamma = MODE_SMOOTH, 1.0
     else:
         raise ValueError(f"unknown mppi_mode {mode}")
     if not (math.isfinite(p.gamma) and p.gamma >= 0.0):     # gamma = 0 is legal: score only the first step
@@ -472,6 +503,8 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
             p.sigma_chol[j * nu + i] = chol[j, i]
             p.sigma_inv[j * nu + i] = sinv[j, i]
             p.sigma0[j * nu + i] = sigma[j, i]
+    if p.mode == MODE_SMOOTH:
+        _smooth_params(p, mppi_cfg, nu, bc)
     if len(obs_items) > MAX_OBS:
         raise ValueError("too many observation items")
     p.k_offset = int(getattr(mppi_cfg, "_k_offset", 0))

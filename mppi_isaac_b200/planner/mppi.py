@@ -26,7 +26,7 @@ import os
 
 import torch
 
-from ..model.blob import MODE_SIMPLE
+from ..model.blob import MODE_SIMPLE, MODE_SMOOTH
 
 
 class _NoRange:
@@ -156,6 +156,13 @@ class MPPIPlanner:
         # both on the device; make_params checks the keys and refuses the combinations the mode excludes
         self.cem = str(getattr(cfg, "mppi_mode", "")) == "cem"
         self.cem_iterations = int(getattr(cfg, "cem_iterations", 3)) if self.cem else 1
+        # Smooth MPPI (DESIGN.md section 2, "Smooth MPPI"): U is the control derivative; K1 integrates it from the last executed action
+        # (the smooth state, a device buffer K4 updates), so the executed command changes by at most du_max * dt per plan
+        self.smooth = str(getattr(cfg, "mppi_mode", "")) == "smooth"
+        if self.smooth and bool(getattr(cfg, "use_priors", False)) and prior is not None:
+            raise ValueError("mppi_mode: smooth does not take a prior: the prior row would be an action, the samples are derivatives")
+        if self.smooth and self.u_per_command > 1:
+            raise ValueError("mppi_mode: smooth executes one action per plan (u_per_command = 1): U holds derivatives, not actions")
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))
@@ -176,6 +183,8 @@ class MPPIPlanner:
             raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
         if self.cem and not hasattr(self.backend, "set_distribution"):
             raise ValueError(f"mppi_mode: cem needs a backend with set_distribution ({type(self.backend).__name__} has none)")
+        if self.smooth and not hasattr(self.backend, "set_smooth_state"):
+            raise ValueError(f"mppi_mode: smooth needs a backend with set_smooth_state ({type(self.backend).__name__} has none)")
         self._peer_exchange = False
         self._peer_capable = (self.world > 1 and getattr(self.backend, "name", "") == "cuda"
                               and os.environ.get("MPPIB_EXCHANGE", "peer") == "peer")
@@ -293,6 +302,15 @@ class MPPIPlanner:
                 parts = [torch.diagonal(sigma)]
             self.dist = torch.cat([torch.tensor([self.lambda_], dtype=torch.float64), *parts]).to(**f32)
             self.backend.set_distribution(self.dist)
+        # Smooth MPPI: the state (a_prev[nu], A[T][nu]) starts at a_prev = clamp(0, u_min, u_max), A = a_prev at every step
+        self.smooth_state = None
+        if self.smooth:
+            p = self.backend.params
+            a0 = torch.tensor([min(max(0.0, p.u_min[j]), p.u_max[j]) for j in range(nu)], dtype=torch.float32)
+            self.smooth_state = a0.repeat(T + 1).to(dev)
+            self.backend.set_smooth_state(self.smooth_state)
+        elif hasattr(self.backend, "set_smooth_state"):
+            self.backend.set_smooth_state(None)          # a rebuilt planner in another mode must not keep the previous one's state
         self._graph = None
         self._graph_failed = False
         self._graph_epoch = -1
@@ -323,6 +341,8 @@ class MPPIPlanner:
         if self.cem:                                     # iteration i keys Philox with plan_idx = i << 32: iteration 0 draws what colored MPPI draws
             be.sample_colored(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise,
                               self.plan_ctr)
+        elif self.smooth:
+            be.sample_smooth(self.seed, 0, self.k_offset, self.K_total, self.U, self.actions, self.noise, self.plan_ctr)
         elif self.use_library:
             be.sample_library(self.k_offset, self.K_total, self.U, None, self.Z, self.actions, self.noise)
         elif self.use_colored:
@@ -332,7 +352,28 @@ class MPPIPlanner:
 
     @property
     def mean_action(self):
+        """(T, nu) device view of the nominal sequence U; with mppi_mode smooth that is the mean of the control DERIVATIVE (the
+        planned actions are ``action_sequence``)."""
         return self.U
+
+    @property
+    def action_sequence(self):
+        """(T, nu) device view of the action sequence A the last smooth plan integrated from ``previous_action`` (None unless
+        mppi_mode smooth); its first row is the action that plan returned."""
+        return None if self.smooth_state is None else self.smooth_state[self.nu:].view(self.T, self.nu)
+
+    @property
+    def previous_action(self):
+        """(nu,) device view of the last executed action a_prev that the next smooth plan integrates from (None unless mppi_mode
+        smooth).  Every plan sets it to the action it returns."""
+        return None if self.smooth_state is None else self.smooth_state[:self.nu]
+
+    def set_previous_action(self, a):
+        """mppi_mode smooth: the world executed `a` rather than the planned action (an operator override, a safety stop): the next
+        plan integrates from it, so the rate bound holds with respect to what was really executed."""
+        if self.smooth_state is None:
+            raise RuntimeError("set_previous_action needs mppi_mode: smooth")
+        self.smooth_state[:self.nu].copy_(torch.as_tensor(a, dtype=torch.float32).reshape(self.nu))
 
     @property
     def cov_action(self):
@@ -426,7 +467,7 @@ class MPPIPlanner:
             self.sim.rollout_all(self.actions)
         with _nvtx("mppi/objective cost"):
             cost = self._cost_batched()
-        x = self.noise if be.params.mode == MODE_SIMPLE else self.actions
+        x = self.noise if be.params.mode in (MODE_SIMPLE, MODE_SMOOTH) else self.actions
         with _nvtx("mppi/K3 reduce + exchange + K4 update"):
             if self.world == 1 and hasattr(be, "reduce_finalize"):
                 be.reduce_finalize(cost, x, self.U, self.partial, self._action, self.stats)      # K3 + K4 in one launch
@@ -460,7 +501,7 @@ class MPPIPlanner:
         if self.use_priors and prior_local:
             row = self.K_total - 2 - self.k_offset
             self.noise[:, :, row] = self.actions[:, :, row] - self.U
-        x = self.noise if be.params.mode == MODE_SIMPLE else self.actions
+        x = self.noise if be.params.mode in (MODE_SIMPLE, MODE_SMOOTH) else self.actions
         be.reduce(self.cost, x, self.U, self.partial)
         partials, G = self._exchange()
         be.finalize(partials, G, self.U, self._action, self.stats)
@@ -473,6 +514,7 @@ class MPPIPlanner:
             side.wait_stream(torch.cuda.current_stream(dev))
             u_keep, ctr_keep = self.U.clone(), self.plan_ctr.clone()
             dist_keep = None if self.dist is None else self.dist.clone()      # the warm-up plans adapt the distribution too
+            smooth_keep = None if self.smooth_state is None else self.smooth_state.clone()   # ... and move the smooth state
             with torch.cuda.stream(side):
                 for _ in range(2):                       # warm-up outside capture (allocator, lazy init)
                     self._plan_batched()
@@ -485,6 +527,8 @@ class MPPIPlanner:
             self.plan_ctr.copy_(ctr_keep)
             if dist_keep is not None:
                 self.dist.copy_(dist_keep)
+            if smooth_keep is not None:
+                self.smooth_state.copy_(smooth_keep)
             self._graph = g
             self._graph_epoch = getattr(self.sim, "model_epoch", 0)
         except Exception as e:  # capture is an optimisation; the eager path is the same kernels

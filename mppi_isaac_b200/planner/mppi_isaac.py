@@ -78,6 +78,8 @@ class MPPIisaacPlanner(object):
             self.mppi.U.copy_(old.U)           # the warm start survives a rebuilt simulator, as in the reference (mppi is not rebuilt there)
             if old.dist is not None and self.mppi.dist is not None and old.dist.shape == self.mppi.dist.shape:
                 self.mppi.dist.copy_(old.dist)         # and so does the adapted (lambda, cov) of adaptive MPPI
+            if old.smooth_state is not None and self.mppi.smooth_state is not None and old.smooth_state.shape == self.mppi.smooth_state.shape:
+                self.mppi.smooth_state.copy_(old.smooth_state)   # and the last executed action of mppi_mode smooth
 
     def _make_mppi(self):
         return MPPIPlanner(
@@ -170,4 +172,4 @@ class MPPIisaacPlanner(object):
 
     def update_mppi_params(self, params):
         self.cfg.mppi.noise_sigma = params["noise_sigma"]
-        self._build_mppi()                     # reference rebuilds MPPIPlanner (and so resets U), :129-138
+        self._build_mppi()                     # reference rebuilds MPPIPlanner (and so resets U and, mppi_mode smooth, a_prev), :129-138

@@ -28,7 +28,7 @@ BUILTIN_CONF = os.path.join(PKG_DIR, "conf")
 class MPPIConfig:
     num_samples: int = 100
     horizon: int = 30
-    mppi_mode: str = "halton-spline"     # halton-spline | simple | cem
+    mppi_mode: str = "halton-spline"     # halton-spline | simple | cem | smooth
     sampling_method: str = "halton"      # halton | random | colored
     noise_sigma: Optional[List[List[float]]] = None
     noise_mu: Optional[List[float]] = None
@@ -42,6 +42,9 @@ class MPPIConfig:
     elite_momentum: float = 0.1          # mppi_mode cem: momentum alpha of the mean and sigma updates, in [0, 1]
     keep_elites: float = 0.3             # mppi_mode cem: fraction xi of the elites carried into the next samples, floor(xi E) rows
     cem_iterations: int = 3              # mppi_mode cem: sample / roll out / update iterations per plan, at least 1
+    smooth_weight: float = 0.0           # mppi_mode smooth (DESIGN.md section 2): omega >= 0 of the cost omega sum_t |a_t - a_{t-1}|^2
+    du_min: Optional[List[float]] = None  # mppi_mode smooth: bounds of the action derivative (length 1 broadcasts; None: unbounded)
+    du_max: Optional[List[float]] = None
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0
