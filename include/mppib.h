@@ -52,7 +52,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 18
+#define MPPIB_ABI_VERSION 19
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -92,6 +92,7 @@ extern "C" {
 #define MPPIB_MODE_CEM    2   /* iCEM rule: the E best samples (elites) by discounted cost; U, sigma <- momentum step towards their mean / std */
 #define MPPIB_MODE_SMOOTH 3   /* Smooth MPPI: U is the control DERIVATIVE; actions are integrated from the last executed action (see below) */
 #define MPPIB_CEM_MAX_ELITES 128
+#define MPPIB_MAX_WORLDS 32   /* risk-aware MPPI: largest n_worlds (a group of worlds never straddles a 32-sample tile) */
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -223,6 +224,9 @@ typedef struct MppibParams {
     float   du_min[MPPIB_MAX_NU];
     float   du_max[MPPIB_MAX_NU];
     float   smooth_weight;     /* omega >= 0: S_k += omega sum_t |a_t - a_{t-1}|^2 (t = 0 against the last executed action)        */
+    /* risk-aware MPPI (see "Risk-aware MPPI" below); both are read only when n_worlds > 1, a zero block keeps today's planner      */
+    int32_t n_worlds;          /* R: rollouts per control sample, a power of two in 1 .. MPPIB_MAX_WORLDS; K and k_offset are multiples */
+    int32_t risk_tail;         /* m in 1 .. R: the score of a control is the mean of its m largest world costs (CVaR)              */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -420,6 +424,18 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
  * mppib_sample, mppib_sample_colored and the noise-library entry points refuse this mode; reduce and finalize refuse it while no
  * state is registered.  A distribution registered with mppib_set_distribution is ignored in this mode.                      */
 int32_t mppib_set_smooth_state(MppibHandle h, float* state);
+
+/* Risk-aware MPPI (n_worlds = R > 1, risk_tail = m; modes SIMPLE and MEAN, fixed, diagonal or full Sigma; not cov_horizon).  The K
+ * rollouts are Kc = K_total / R control samples of R rollouts each: global rollout kg = c*R + r runs control c in world r.
+ *   K1     every variant but smooth / horizon keys its Philox draws (or Halton index) and its null / prior tests by c against Kc
+ *          instead of kg against K_total, so the R rollouts of a control carry the same actions: the result is np.repeat of the
+ *          K1 at K_total = Kc, R times along k.  The null control is c = Kc - 1.
+ *   K2     the per-rollout size / mass / friction draws are keyed by the world r = kg % R instead of kg, so every control faces the
+ *          same R worlds (common random numbers), the same on every plan.
+ *   K3     S_k as before; then per aligned group of R lanes: a non-finite S_k becomes +inf, the group is sorted in descending order,
+ *          rho_c = (s_(0) + ... + s_(m-1)) / m (float32, summed left to right, one division) goes to lane r = 0 and +inf to the
+ *          others, and the rest of K3 runs unchanged: the shard row is the control-level row of a Kc-sample MPPI, beta = min rho.
+ *   K4, the shift and the peer exchange are unchanged.  The launchers refuse a shard whose K or k_offset is not a multiple of R. */
 int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset,
                             uint32_t k_total, const float* U, float* actions, float* noise, void* stream);
 

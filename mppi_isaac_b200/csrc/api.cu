@@ -65,6 +65,15 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         for (int j = 0; j < m->nu; ++j)
             for (int i = 0; i < m->nu; ++i) MPPIB_REQUIRE(i == j || p->sigma_chol[j * m->nu + i] == 0.f, "mode cem needs a diagonal noise_sigma");
     }
+    if (p->n_worlds > 1) {
+        const int R = p->n_worlds;
+        MPPIB_REQUIRE(R <= MPPIB_MAX_WORLDS && (R & (R - 1)) == 0, "n_worlds = %d must be a power of two in 1 .. %d", R, MPPIB_MAX_WORLDS);
+        MPPIB_REQUIRE(p->risk_tail >= 1 && p->risk_tail <= R, "risk_tail = %d out of range [1, n_worlds = %d]", p->risk_tail, R);
+        MPPIB_REQUIRE(p->K % R == 0 && p->k_offset % (uint32_t)R == 0, "n_worlds = %d: the shard K = %d, k_offset = %u must be multiples of it", R,
+                      p->K, p->k_offset);
+        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "n_worlds > 1 excludes mode cem and mode smooth");
+        MPPIB_REQUIRE(!p->cov_horizon, "n_worlds > 1 excludes cov_horizon");
+    }
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);

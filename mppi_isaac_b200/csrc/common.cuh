@@ -90,6 +90,11 @@ static inline int partial_row_capacity(const MppibParams& p, int nu) {
     if (p.update_cov && p.cov_horizon) return 2 + p.T * nu + p.T * nu * (p.T * nu + 1) / 2;
     return 2 + p.T * nu * (p.update_cov ? 2 : 1);
 }
+// Risk-aware MPPI (n_worlds = R > 1, a power of two): global rollout kg = c*R + r runs control sample c in world r.  K1 keys its draws
+// and its null / prior rows by c, K2 keys the per-rollout randomisation by r.  R <= 1 (and a zero-initialised block) keeps kg for both.
+__device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
+__device__ __forceinline__ uint32_t sample_world(uint32_t kg, int R) { return R > 1 ? kg & (uint32_t)(R - 1) : kg; }
+static inline bool risk_mode(const MppibContext* c) { return c->params.n_worlds > 1; }
 static inline bool cem_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_CEM; }
 static inline bool smooth_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_SMOOTH; }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }

@@ -46,6 +46,23 @@ __device__ __forceinline__ float warp_sum(float v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
+// Risk-aware MPPI: the CVaR score of the aligned group of R lanes (R a power of two <= 32) this lane belongs to.  The group's S (+inf
+// for an invalid or padding sample) is sorted in descending order by a bitonic network over __shfl_xor_sync -- every stage but the last
+// merges pairs of blocks of opposite order, the last one orders every group the same way -- then lane r = 0 of the group sums its m
+// largest values left to right, divides once by m and keeps the result; the other lanes get +inf and so weight 0.
+__device__ __forceinline__ float risk_score(float S, int R, int m, int lane) {
+    for (int k = 2; k <= R; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            const float o = __shfl_xor_sync(0xffffffffu, S, j);
+            const bool desc = k == R || (lane & k) == 0;                      // order of the block of k lanes this lane sorts into
+            S = (((lane & j) == 0) == desc) ? fmaxf(S, o) : fminf(S, o);
+        }
+    }
+    const int base = lane & ~(R - 1);
+    float acc = S;
+    for (int i = 1; i < m; ++i) acc += __shfl_sync(0xffffffffu, S, base + i);
+    return lane == base ? __fdiv_rn(acc, (float)m) : INFINITY;
+}
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -533,7 +550,9 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // (beta, eta, W[n]) only; the SYRK appends C.
 // SMOOTH (mode smooth, x = the derivative noise): SIMPLE with gamma = 1, plus omega dt^2 sum_r (U_r + x_rk)^2 in phase A (U staged in
 // `us`, four chains in r order; skipped when omega = 0, so that the row is SIMPLE's), and the fused K4 integrates the state `smooth`.
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>   // rows of W per lane: T*nu <= 32 * RPL
+// RISK (n_worlds = R > 1): phase B replaces the S of every aligned group of R samples by its CVaR score on the group's first lane and
+// +inf on the others (risk_score); a tile is 32 samples and every shard starts at a multiple of R, so no group straddles two tiles.
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
@@ -677,7 +696,8 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             }
             // ---- B: tile minimum, weights, their sum
             const bool valid = (k0 + lane < K) && isfinite(sum);
-            const float S = valid ? sum : INFINITY;
+            float S = valid ? sum : INFINITY;
+            if constexpr (RISK) S = risk_score(S, p.n_worlds, p.risk_tail, lane);
             if (HZN && k0 + lane < K) hz_S[k0 + lane] = S;
             const float b_c = warp_min(S);
             const float w = (S == INFINITY) ? 0.f : expf(-(S - b_c) * inv_lambda);
@@ -1030,7 +1050,7 @@ static int reduce_ws_stages(int T, int nu, int kind, bool smooth = false) {
     return ns;
 }
 
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
@@ -1044,7 +1064,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -1063,7 +1083,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
     PeerArgs peers = reduce_peers(c);
     if (HZN) peers.world = 0;                                                 // the row is complete only after the SYRK, which stores it
-    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
+    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
                                                                             c->reduce_scratch, c->reduce_ticket, partial, peers, fin_U, fin_action,
                                                                             fin_stats, fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g,
                                                                             SMOOTH ? c->smooth : nullptr);
@@ -1152,6 +1172,25 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
         if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
         if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
         return launch_reduce_ws_t<16, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
+    if (risk_mode(c)) {
+        const int R = c->params.n_worlds;
+        MPPIB_REQUIRE(c->params.K % R == 0 && c->params.k_offset % (uint32_t)R == 0, "mppib_reduce: n_worlds = %d needs K = %d and k_offset = %u to be multiples of it",
+                      R, c->params.K, c->params.k_offset);
+        MPPIB_REQUIRE(!adaptive_horizon(c), "mppib_reduce: n_worlds > 1 excludes cov_horizon");
+        if (adaptive_full(c)) {
+            if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+            if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+            return launch_reduce_ws_t<16, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        }
+        if (c->dist) {
+            if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+            if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+            return launch_reduce_ws_t<16, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        }
+        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        return launch_reduce_ws_t<16, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
     }
     if (adaptive_horizon(c)) {
         MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N, "mppib_reduce: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, NR);

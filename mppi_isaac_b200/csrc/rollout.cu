@@ -225,7 +225,7 @@ mppib_rollout_kernel(const __grid_constant__ MppibModel m, const __grid_constant
     }
     float* xs = sm + (size_t)nb * NSLOT * 32;             // free bodies / shapes / contacts (CONTACT kernels only)
     const contact::Layout L(nb, m.nfree, m.nshapes, m.max_contacts);
-    if (CONTACT) contact::init(m, p, L, xs, lane, p.k_offset + (uint32_t)k, root0, state, state0 != nullptr, K, k);
+    if (CONTACT) contact::init(m, p, L, xs, lane, sample_world(p.k_offset + (uint32_t)k, p.n_worlds), root0, state, state0 != nullptr, K, k);
     Frame base;
     const Quat bq = {m.base_quat[0], m.base_quat[1], m.base_quat[2], m.base_quat[3]};
     base.R = quat_to_R(bq);

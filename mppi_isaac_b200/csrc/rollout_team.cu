@@ -355,7 +355,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     // =====================================================================================================================
     // contact pipeline (team-parallel restatement of contact.cuh; the oracle's loop orders are kept)
     // =====================================================================================================================
-    const uint32_t kg = p.k_offset + (uint32_t)kc;
+    const uint32_t kg = sample_world(p.k_offset + (uint32_t)kc, p.n_worlds);   // key of the per-rollout randomisation
     // generalised coordinates of the contact solve held by this lane: coordinate sl * GC + ic = joint (< nb), else component of a free body
     constexpr int MAXS = NCS;
     constexpr int ncs = NCS;                                 // (== L.ncs, checked by the launcher)

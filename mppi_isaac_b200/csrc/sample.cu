@@ -68,7 +68,8 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
     }
 }
 
-// DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block).
+// DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block); with
+// n_worlds = R > 1 the control sample kg / R replaces the global sample in the counter and in the null / prior tests.
 template <bool DIAG, bool FULL = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
@@ -78,35 +79,35 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int t = blockIdx.y;
     if (k >= K) return;
-    const uint32_t kg = k_offset + (uint32_t)k;
+    const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds), kc_last = sample_control(k_total - 1, p.n_worlds);
     const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
     const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
     float z[MPPIB_MAX_NU];
 #pragma unroll
     for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk) {
         if (blk * 4 < nu) {
-            uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
+            uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
             box_muller(r.x, r.y, z[4 * blk], z[4 * blk + 1]);
             box_muller(r.z, r.w, z[4 * blk + 2], z[4 * blk + 3]);
         }
     }
-    const bool is_null = p.sample_null_action && kg == k_total - 1;
-    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
+    const bool is_null = p.sample_null_action && kc == kc_last;
+    const bool is_prior = prior_row != nullptr && kc + 1 == kc_last;
     colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, U, prior_row, actions, noise, dist);
 }
 
 // The white Philox draws of a tile of S samples [k0, k0 + S) to shared memory, zs[(t*nu + i) * S + sample]: the draws of the
-// fixed-Sigma kernel (counter (global sample, t, block)), spread over the CTA.
+// fixed-Sigma kernel (counter (control sample of n_worlds = R, t, block)), spread over the CTA.
 template <int S>
 __device__ __forceinline__ void stage_white_tile(float* zs, int T, int nu, int k0, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
-                                                 const uint32_t* __restrict__ plan_ctr, uint32_t k_offset) {
+                                                 const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, int R) {
     const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
     const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
     const int nblk = (nu + 3) / 4;
     for (int idx = threadIdx.x; idx < S * T * nblk; idx += blockDim.x) {
         const int sl = idx % S, rest = idx / S, blk = rest % nblk, t = rest / nblk;
-        const uint32_t kg = k_offset + (uint32_t)(k0 + sl);
-        const uint4 r = philox4x32_10(make_uint4(kg, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
+        const uint32_t kc = sample_control(k_offset + (uint32_t)(k0 + sl), R);
+        const uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
         float z[4];
         box_muller(r.x, r.y, z[0], z[1]);
         box_muller(r.z, r.w, z[2], z[3]);
@@ -166,11 +167,12 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const int K = p.K, T = p.T;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int k0 = blockIdx.x * CL_S, k = k0 + lane;
-    stage_white_tile<CL_S>(cs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
+    stage_white_tile<CL_S>(cs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, p.n_worlds);
     __syncthreads();
     const uint32_t kg = k_offset + (uint32_t)k;
-    const bool is_null = p.sample_null_action && kg == k_total - 1;
-    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
+    const uint32_t kc = sample_control(kg, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
+    const bool is_null = p.sample_null_action && kc == kc_total - 1;
+    const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
     const float* zl = cs + lane;
     for (int tl = warp; tl < (T + 1) / 2; tl += 4) {
         const int th = T - 1 - tl;                                            // th >= tl; th == tl for the middle row of an odd T
@@ -246,7 +248,7 @@ mppib_sample_smooth_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     const int K = p.K, T = p.T;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int k0 = blockIdx.x * SM_S, k = k0 + lane;
-    stage_white_tile<SM_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
+    stage_white_tile<SM_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, 1);
     __syncthreads();
     if (k >= K) return;
     const bool is_null = p.sample_null_action && k_offset + (uint32_t)k == k_total - 1;
@@ -296,8 +298,8 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     const int K = p.K, T = p.T;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= K) return;
-    const uint32_t kg = k_offset + (uint32_t)k;
-    const bool null_row = p.sample_null_action && kg == k_total - 1;
+    const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds);
+    const bool null_row = p.sample_null_action && kc == sample_control(k_total, p.n_worlds) - 1;
     const int nd = n_knots * nu;
     for (int j = 0; j < nu; ++j) {
         // coloured knots of control dimension j:  c[n] = sum_i L[j][i] z[n][i]
@@ -306,7 +308,7 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
             float acc = 0.f;
             for (int i = WHITE ? j : 0; i <= j; ++i) {
                 const int d = n * nu + i;
-                const float u = halton(kg + 1u, (uint32_t)tab[d], (uint32_t)tab[nd + d]);
+                const float u = halton(kc + 1u, (uint32_t)tab[d], (uint32_t)tab[nd + d]);
                 const float zn = 1.41421356237f * erfinvf(2.0f * u - 1.0f);
                 acc += WHITE ? zn : p.sigma_chol[j * nu + i] * zn;
             }
@@ -330,9 +332,9 @@ mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const int K = p.K;
     const int k = blockIdx.x * blockDim.x + threadIdx.x, t = blockIdx.y;
     if (k >= K) return;
-    const uint32_t kg = k_offset + (uint32_t)k;
-    const bool is_null = p.sample_null_action && kg == k_total - 1;
-    const bool is_prior = prior_row != nullptr && kg == k_total - 2;
+    const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
+    const bool is_null = p.sample_null_action && kc == kc_total - 1;
+    const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
     if constexpr (FULL) {
         const float* Ld = dist + 1 + nu * nu;
         float zc[MPPIB_MAX_NU];
@@ -398,7 +400,7 @@ mppib_sample_horizon_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             zs[idx] = k < K ? Z[(size_t)r * K + k] : 0.f;
         }
     } else {
-        stage_white_tile<HZ_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset);
+        stage_white_tile<HZ_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, 1);
     }
     const float* Ld = dist + 1 + (size_t)n * n;
     for (int r0 = 0; r0 < n; r0 += 32) {
@@ -464,12 +466,22 @@ int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
     return 0;
 }
 
+// Risk-aware MPPI: a K1 shard holds whole groups of n_worlds rollouts, so that the R rollouts of a control get the same draw
+int check_risk_shard(const MppibContext* c, const char* who, uint32_t k_offset, uint32_t k_total) {
+    const int R = c->params.n_worlds;
+    if (R <= 1) return 0;
+    MPPIB_REQUIRE(c->params.K % R == 0 && k_offset % (uint32_t)R == 0 && k_total % (uint32_t)R == 0,
+                  "%s: n_worlds = %d needs K = %d, k_offset = %u and k_total = %u to be multiples of it", who, R, c->params.K, k_offset, k_total);
+    return 0;
+}
+
 }  // namespace
 
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_noise_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_noise_library: mode smooth samples through mppib_sample_smooth");
+    if (int rc = check_risk_shard(c, "mppib_noise_library", k_offset, k_total)) return rc;
     MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
     if (adaptive_cov(c))
@@ -484,6 +496,7 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
                           float* actions, float* noise, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_library: mode smooth samples through mppib_sample_smooth");
+    if (int rc = check_risk_shard(c, "mppib_sample_library", k_offset, k_total)) return rc;
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -502,6 +515,7 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample: mode cem samples through mppib_sample_colored (white noise: Lt = I)");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample: mode smooth samples through mppib_sample_smooth");
+    if (int rc = check_risk_shard(c, "mppib_sample", k_offset, k_total)) return rc;
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -523,6 +537,7 @@ int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, con
                           const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_colored: mode smooth samples through mppib_sample_smooth");
+    if (int rc = check_risk_shard(c, "mppib_sample_colored", k_offset, k_total)) return rc;
     MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
     MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
                   CL_MAX_N, T, T * nu);

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 18
+ABI_VERSION = 19
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -30,6 +30,7 @@ SHAPE_BOX, SHAPE_SPHERE = 0, 1
 OWNER_STATIC, OWNER_LINK, OWNER_FREE = 0, 1, 2
 MODE_SIMPLE, MODE_MEAN, MODE_CEM, MODE_SMOOTH = 0, 1, 2, 3
 CEM_MAX_ELITES = 128
+MAX_WORLDS = 32                                 # risk-aware MPPI: largest n_worlds
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -78,6 +79,7 @@ class MppibParams(C.Structure):
         ("cov_horizon", i32), ("sigma0", f32 * (MAX_NU * MAX_NU)),
         ("n_elites", i32), ("n_keep", i32), ("elite_alpha", f32),
         ("du_min", f32 * MAX_NU), ("du_max", f32 * MAX_NU), ("smooth_weight", f32),
+        ("n_worlds", i32), ("risk_tail", i32),
     ]
 
 
@@ -432,6 +434,34 @@ def _smooth_params(p: MppibParams, mppi_cfg, nu: int, bc) -> None:
         p.du_min[j], p.du_max[j] = dlo[j], dhi[j]
 
 
+def risk_tail(n_worlds: int, alpha: float) -> int:
+    """m = ceil(alpha R) in float64: the number of worst worlds whose mean scores a control (1 .. R)."""
+    return min(max(int(math.ceil(float(alpha) * int(n_worlds))), 1), int(n_worlds))
+
+
+def _risk_params(p: MppibParams, mppi_cfg, K_local: int) -> None:
+    """The risk-aware MPPI keys (DESIGN.md section 2, "Risk-aware MPPI"): R = n_worlds rollouts per control sample, scored by the mean
+    of their m = ceil(cvar_alpha R) largest costs; the refusals of the mode.  n_worlds = 1 leaves the block as it was."""
+    R = int(getattr(mppi_cfg, "n_worlds", 1))
+    if R == 1:
+        return
+    alpha = float(getattr(mppi_cfg, "cvar_alpha", 1.0))
+    k_total = int(mppi_cfg.num_samples)
+    if not (1 <= R <= MAX_WORLDS and R & (R - 1) == 0):
+        raise ValueError(f"n_worlds = {R} must be a power of two in 1 .. {MAX_WORLDS}")
+    if not (math.isfinite(alpha) and 0.0 < alpha <= 1.0):
+        raise ValueError(f"cvar_alpha = {alpha} must lie in (0, 1]")
+    if k_total % R != 0 or k_total // R < 2:
+        raise ValueError(f"n_worlds = {R} needs num_samples = {k_total} to be a multiple of it with at least two control samples")
+    if K_local % R != 0:
+        raise ValueError(f"n_worlds = {R}: the shard of {K_local} samples must hold whole groups of worlds")
+    if p.mode in (MODE_CEM, MODE_SMOOTH):
+        raise ValueError("n_worlds > 1 excludes mppi_mode cem and smooth")
+    if p.cov_horizon:
+        raise ValueError("n_worlds > 1 excludes cov_type: horizon")
+    p.n_worlds, p.risk_tail = R, risk_tail(R, alpha)
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -508,6 +538,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     if len(obs_items) > MAX_OBS:
         raise ValueError("too many observation items")
     p.k_offset = int(getattr(mppi_cfg, "_k_offset", 0))
+    _risk_params(p, mppi_cfg, int(K_local))
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

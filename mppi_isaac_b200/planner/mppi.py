@@ -108,17 +108,24 @@ def colored_noise_chol(T: int, beta: float):
     return np.linalg.cholesky(colored_noise_cov(T, beta)).astype(np.float32)
 
 
-def shard_samples(k_total: int, rank: int, world: int):
-    """Split k_total samples over `world` ranks in units of 4 (128-bit loads need K_local % 4 == 0)."""
-    if k_total % 4 != 0:
-        raise ValueError(f"num_samples={k_total} must be a multiple of 4")
-    units = k_total // 4
+def shard_samples(k_total: int, rank: int, world: int, unit: int = 4):
+    """Split k_total samples over `world` ranks in units of `unit` samples (128-bit loads need K_local % 4 == 0; risk-aware MPPI
+    keeps the n_worlds rollouts of a control sample on one rank with unit = max(4, n_worlds))."""
+    if k_total % unit != 0:
+        raise ValueError(f"num_samples={k_total} must be a multiple of {unit}")
+    units = k_total // unit
     base, rem = divmod(units, world)
     mine = base + (1 if rank < rem else 0)
     off = rank * base + min(rank, rem)
     if mine == 0:
         raise ValueError(f"num_samples={k_total} is too small for {world} ranks")
-    return 4 * mine, 4 * off
+    return unit * mine, unit * off
+
+
+def _randomised(model) -> bool:
+    """True when K2 draws something per rollout: a free body's mass, or a shape's friction or size."""
+    return (any(model.free_mass_pct[f] != 0.0 for f in range(model.nfree))
+            or any(model.shape_fric_pct[s] != 0.0 or any(model.shape_size_sigma[s][i] != 0.0 for i in range(3)) for s in range(model.nshapes)))
 
 
 class MPPIPlanner:
@@ -163,6 +170,16 @@ class MPPIPlanner:
             raise ValueError("mppi_mode: smooth does not take a prior: the prior row would be an action, the samples are derivatives")
         if self.smooth and self.u_per_command > 1:
             raise ValueError("mppi_mode: smooth executes one action per plan (u_per_command = 1): U holds derivatives, not actions")
+        # risk-aware MPPI (DESIGN.md section 2, "Risk-aware MPPI"): the K rollouts are K / R control samples, each rolled out in the
+        # same R randomised worlds and scored by the CVaR of its R costs; make_params checks the keys against the mode
+        self.n_worlds = int(getattr(cfg, "n_worlds", 1))
+        self.control_samples = self.K_total // max(1, self.n_worlds)
+        if self.n_worlds > 1:
+            if bool(getattr(cfg, "use_priors", False)) and prior is not None:
+                raise ValueError("n_worlds > 1 does not take a prior: the prior row would have to fill a whole group of worlds")
+            if not _randomised(sim.scene.model):
+                raise ValueError("n_worlds > 1 needs a scene that randomises its rollouts (noise_percentage_mass, noise_percentage_friction "
+                                 "or noise_sigma_size on some actor): without it the worlds would be identical copies")
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))

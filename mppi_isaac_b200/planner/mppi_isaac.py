@@ -41,7 +41,7 @@ class MPPIisaacPlanner(object):
             rank = torch.distributed.get_rank(process_group)
             world = torch.distributed.get_world_size(process_group)
         self.k_total = int(cfg.mppi.num_samples)
-        self.k_local, self.k_offset = shard_samples(self.k_total, rank, world)
+        self.k_local, self.k_offset = shard_samples(self.k_total, rank, world, unit=max(4, int(getattr(cfg.mppi, "n_worlds", 1))))
 
         self.sim = RolloutSim(
             cfg.isaacgym,

@@ -45,6 +45,8 @@ class MPPIConfig:
     smooth_weight: float = 0.0           # mppi_mode smooth (DESIGN.md section 2): omega >= 0 of the cost omega sum_t |a_t - a_{t-1}|^2
     du_min: Optional[List[float]] = None  # mppi_mode smooth: bounds of the action derivative (length 1 broadcasts; None: unbounded)
     du_max: Optional[List[float]] = None
+    n_worlds: int = 1                    # risk-aware MPPI (DESIGN.md section 2): R rollouts per control sample in R fixed worlds, 1 .. 32
+    cvar_alpha: float = 1.0              # risk-aware MPPI: a control scores the mean of its ceil(alpha R) worst world costs, alpha in (0, 1]
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0

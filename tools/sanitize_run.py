@@ -3,7 +3,7 @@
 library), K2 (lanes-per-rollout chain kernel, team kernel on contact scenes of small and large robots, thread-per-rollout chain / tree /
 contact kernels), fused cost, K3 (warp-specialised
 ring, ragged last tile), K4, shift, the cov_type horizon kernels (horizon-colour K1, SYRK, its fused K4), the colored K1, the mppi_mode cem kernels (CEM K1, elite kernel with its last-CTA merge, CEM K4 and shift), the mppi_mode smooth kernels (smooth K1,
-K3 with the smoothness cost and the fused smooth K4), and whole plans (eager and CUDA-graph replay).  Sizes are
+K3 with the smoothness cost and the fused smooth K4), the risk-aware K1 / K2 / K3 (n_worlds), and whole plans (eager and CUDA-graph replay).  Sizes are
 small: the sanitizer serialises the GPU.  With WORLD_SIZE > 1 (torchrun) the plans also run the peer-memory exchange."""
 import os
 import sys
@@ -50,6 +50,8 @@ CASES = [
     ("panda reach, mppi_mode smooth (smooth K1: 32-sample tiles, ragged last tile, four warps over nu = 7; smooth K3 with the fused "
      "K4)", lambda: panda_cfg(K=1000 * world, T=31, device=dev, mppi_mode="smooth", sampling_method="random", filter_u=False,
                                  smooth_weight=0.5, du_min=[-1.0], du_max=[1.0]), PandaReachObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]),
+    ("heijn push, n_worlds 8 (K1 keyed by the control sample, team K2 keyed by the world, RISK K3 with the fused K4)",
+     lambda: push_cfg(K=256 * world, T=10, device=dev, n_worlds=8, cvar_alpha=0.25), PushObjective, [0.0, 0.0, 0.0]),
     ("panda pick (team K2: contacts, 16-lane articulation in 2 passes, compact layout)", lambda: pick_cfg(K=64 * world, T=9, device=dev), PandaPickObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0, 0.02, 0.02]),
 ]
 for name, mk, obj, q in CASES:
