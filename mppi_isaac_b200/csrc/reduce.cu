@@ -514,20 +514,22 @@ constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
 // region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.  With the C row (ROW_C)
 // the fused K4 also keeps its covariance scratch there (full_fin_floats), which the ring stages of every accepted shape exceed.
 struct WsLayout {
-    int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [NCONS][P4] warp partials | [8]
+    int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [nparts][P4] warp partials | [8]
     int us;                       // smooth: [NR4] U for the smoothness cost (no floats otherwise)
     int bar;                      // full[nstage], then empty[nstage] mbarriers
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
-    // kind: what the shard row carries after W (RowKind)
-    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false) {
+    // kind: what the shard row carries after W (RowKind); nparts: warp partials stored, by default one per consumer warp
+    // (min(nstage, WS_NCONS): the launch rounds the ring depth down to a multiple of the consumer count)
+    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false, int nparts = -1) {
         const int NR = T * nu, P4 = (row_floats(T, nu, kind) + 3) & ~3;
+        if (nparts < 0) nparts = nstage < WS_NCONS ? nstage : WS_NCONS;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
         if (kind == ROW_C && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
         gp = g + ((NR + 3) & ~3);
         wk = gp + ((T + 3) & ~3);
         cpart = wk + 8 * WS_W;
-        misc = cpart + WS_NCONS * P4;
+        misc = cpart + nparts * P4;
         us = misc + 8;
         bar = ((us + (smooth ? ((NR + 3) & ~3) : 0)) * 4 + 15) & ~15;
         bytes = bar + 2 * 8 * nstage + 128;
@@ -549,7 +551,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // stores every S_k (INFINITY for an invalid sample) to hz_S for the SYRK that follows, and the row this kernel writes is
 // (beta, eta, W[n]) only; the SYRK appends C.
 // SMOOTH (mode smooth, x = the derivative noise): SIMPLE with gamma = 1, plus omega dt^2 sum_r (U_r + x_rk)^2 in phase A (U staged in
-// `us`, four chains in r order; skipped when omega = 0, so that the row is SIMPLE's), and the fused K4 integrates the state `smooth`.
+// `us`, four chains in r order; with omega = 0 neither the term nor the `us` region exists, so that the ring, the consumers and the row
+// are SIMPLE's), and the fused K4 integrates the state `smooth`.
 // RISK (n_worlds = R > 1): phase B replaces the S of every aligned group of R samples by its CVaR score on the group's first lane and
 // +inf on the others (risk_score); a tile is 32 samples and every shard starts at a multiple of R, so no group straddles two tiles.
 template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false>   // rows of W per lane: T*nu <= 32 * RPL
@@ -571,7 +574,8 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
-    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, SMOOTH);
+    const bool smooth_term = SMOOTH && p.smooth_weight != 0.f;
+    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, smooth_term);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -615,7 +619,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         }
         if (FULL && !simple && r < NR) acc = U[r];                            // phase A reads g in SIMPLE mode only
         g[r] = acc;
-        if (SMOOTH && r < NR) tiles[L.us + r] = U[r];
+        if (smooth_term && r < NR) tiles[L.us + r] = U[r];
     }
     {
         // gamma^0 = 1 for every accepted gamma: log2f(0) * 0 would be NaN (validate refuses a negative or non-finite gamma)
@@ -681,7 +685,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             }
             float sum = (a0 + a1) + (a2 + a3);
             if constexpr (SMOOTH) {
-                if (p.smooth_weight != 0.f) {                                 // omega dt^2 sum_r (U_r + x_rk)^2
+                if (smooth_term) {                                            // omega dt^2 sum_r (U_r + x_rk)^2
                     const float* us = tiles + L.us;
                     float q0 = 0.f, q1 = 0.f, q2 = 0.f, q3 = 0.f;
                     int r = 0;
@@ -780,26 +784,25 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                 if (lane == 0) mine[2 + NR + q] = v;
             }
         }
-    } else {
-        // spare warp (fewer ring stages than warps): an empty partial
-        float* mine = cpart + (size_t)(warp - 1) * P4;
-        if (lane == 0) { mine[0] = INFINITY; mine[1] = 0.f; }
-        for (int r = lane; r < P - 2; r += 32) mine[2 + r] = 0.f;
     }
+    // (a spare warp -- fewer ring stages than warps -- has no partial: the layout stores the ncons consumers' only)
     __syncthreads();
     // ---- merge the warp partials into the CTA partial (global scratch), then ticket -> the last CTA folds all of them
     {
         float* mine = scratch + (size_t)blockIdx.x * P4;
         float bb = INFINITY;
 #pragma unroll
-        for (int c = 0; c < WS_NCONS; ++c) bb = fminf(bb, cpart[(size_t)c * P4]);
+        for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = fminf(bb, cpart[(size_t)c * P4]);
         float sc[WS_NCONS];
 #pragma unroll
-        for (int c = 0; c < WS_NCONS; ++c) { const float bc = cpart[(size_t)c * P4]; sc[c] = (bc == INFINITY) ? 0.f : expf(-(bc - bb) * inv_lambda); }
+        for (int c = 0; c < WS_NCONS; ++c) {
+            const float bc = c < ncons ? cpart[(size_t)c * P4] : INFINITY;
+            sc[c] = (bc == INFINITY) ? 0.f : expf(-(bc - bb) * inv_lambda);
+        }
         for (int e = tid; e < P; e += NT) {
             float v = 0.f;
 #pragma unroll
-            for (int c = 0; c < WS_NCONS; ++c) v += sc[c] * cpart[(size_t)c * P4 + e];
+            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) v += sc[c] * cpart[(size_t)c * P4 + e];
             mine[e] = e == 0 ? bb : v;
         }
     }
@@ -1044,9 +1047,12 @@ static PeerArgs reduce_peers(const MppibContext* c) {
     return a;
 }
 
+// The ring depth: the deepest ring (<= 8 stages) that fits next to seven warp partials, the depths every shape was tuned at.  Where
+// that leaves fewer than two stages (the second-moment row at T = 256, T*nu = 512), two stages fit next to their two consumers'.
 static int reduce_ws_stages(int T, int nu, int kind, bool smooth = false) {
     int ns = 8;
-    while (ns > 1 && WsLayout(T, nu, ns, kind, smooth).bytes > 224 * 1024) --ns;
+    while (ns > 1 && WsLayout(T, nu, ns, kind, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
+    if (ns < 2 && WsLayout(T, nu, 2, kind, smooth).bytes <= 224 * 1024) ns = 2;
     return ns;
 }
 
@@ -1057,10 +1063,11 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
     const int kind = FULL ? ROW_C : (ADAPT && c->params.update_cov) ? ROW_M2 : ROW_W;
-    const int nstage_max = reduce_ws_stages(T, nu, kind, SMOOTH);
+    const bool smooth_term = SMOOTH && c->params.smooth_weight != 0.f;    // the `us` region of the kernel's layout
+    const int nstage_max = reduce_ws_stages(T, nu, kind, smooth_term);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = WsLayout(T, nu, nstage, kind, SMOOTH).bytes;
+    const size_t smem = WsLayout(T, nu, nstage, kind, smooth_term).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {

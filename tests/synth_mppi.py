@@ -44,7 +44,8 @@ def row_floats(T, nu, kind):
     return 2 + NR + (NR if kind == "M2" else nu * (nu + 1) // 2 if kind == "C" else NR * (NR + 1) // 2 if kind == "H" else 0)
 
 
-def _ws_bytes(T, nu, nstage, kind):
+def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False):
+    """Bytes of ``WsLayout``: nparts warp partials (default one per consumer, min(nstage, 7)); smooth adds the [NR4] U region."""
     NR = T * nu
     P4 = (row_floats(T, nu, kind) + 3) & ~3
     ring, fold = nstage * (NR + T) * WS_W, MAX_GRID + 4 * P4
@@ -53,28 +54,33 @@ def _ws_bytes(T, nu, nstage, kind):
         g = max(g, NR + 1 + 2 * NR + nu * (nu + 1) // 2 + 3 * nu * nu)
     gp = g + ((NR + 3) & ~3)
     wk = gp + ((T + 3) & ~3)
-    misc = wk + 8 * WS_W + WS_NCONS * P4
-    bar = ((misc + 8) * 4 + 15) & ~15
+    misc = wk + 8 * WS_W + (min(nstage, WS_NCONS) if nparts is None else nparts) * P4
+    us = misc + 8
+    bar = ((us + (((NR + 3) & ~3) if smooth else 0)) * 4 + 15) & ~15
     return bar + 2 * 8 * nstage + 128
 
 
-def ws_stages(T, nu, kind):
+def ws_stages(T, nu, kind, smooth=False):
+    """The ring depth rule of ``reduce_ws_stages``: the deepest ring next to seven warp partials, else two stages next to two."""
     ns = 8
-    while ns > 1 and _ws_bytes(T, nu, ns, kind) > SMEM_CAP:
+    while ns > 1 and _ws_bytes(T, nu, ns, kind, WS_NCONS, smooth) > SMEM_CAP:
         ns -= 1
+    if ns < 2 and _ws_bytes(T, nu, 2, kind, None, smooth) <= SMEM_CAP:
+        ns = 2
     return ns
 
 
-def ws_layout(T, nu, kind):
-    """(rows of W per lane, consumer warps, ring stages, rows per x TMA box) of the K3 launch, or None if the shape is refused."""
+def ws_layout(T, nu, kind, smooth=False):
+    """(rows of W per lane, consumer warps, ring stages, rows per x TMA box) of the K3 launch, or None if the shape is refused.
+    `smooth`: the layout of mode smooth (row W, plus the U region of the smoothness cost)."""
     NR = T * nu
     if kind == "H":
         if NR > HZ_MAX_N:
             return None
         kind = "M2"                    # the host sizes the horizon K3 (row W only) with the update_cov rule's M2 layout
-    if NR > 512 or T > 256 or ws_stages(T, nu, "W") < 2 or ws_stages(T, nu, kind) < 2:
+    if NR > 512 or T > 256 or ws_stages(T, nu, "W") < 2 or ws_stages(T, nu, kind, smooth) < 2:
         return None
-    ns = ws_stages(T, nu, kind)
+    ns = ws_stages(T, nu, kind, smooth)
     ncons = min(ns, WS_NCONS)
     xbox = min(NR, 256)
     while NR % xbox:
@@ -82,9 +88,9 @@ def ws_layout(T, nu, kind):
     return (4 if NR <= 128 else 8 if NR <= 256 else 16), ncons, ncons * (ns // ncons), xbox
 
 
-def wrap_K(T, nu, kind, sms=NUM_SMS):
+def wrap_K(T, nu, kind, sms=NUM_SMS, smooth=False):
     """A ragged K (multiple of 4) whose every CTA streams more than three full rings of tiles."""
-    _, _, nstage, _ = ws_layout(T, nu, kind)
+    _, _, nstage, _ = ws_layout(T, nu, kind, smooth)
     return WS_W * sms * (3 * nstage + 1) - 12
 
 

@@ -12,8 +12,8 @@ import torch
 import adaptive_full_oracle as afo
 import adaptive_horizon_oracle as aho
 import adaptive_oracle as ada
-from synth_mppi import (NUM_SMS, hz_C, hz_id, hz_k1_f32, hz_k1_gate, k3_dS, k3_gate, k3_inputs, k3_restate, k3_S32, last4_K, make_case,
-                        nu_model, row_excess, syrk_split, ws_layout)
+from synth_mppi import (NUM_SMS, SMEM_CAP, WS_NCONS, _ws_bytes, hz_C, hz_id, hz_k1_f32, hz_k1_gate, k3_dS, k3_gate, k3_inputs, k3_restate,
+                        k3_S32, last4_K, make_case, nu_model, row_excess, syrk_split, ws_layout, ws_stages)
 from test_oracle_mppi import _torch_update
 
 SHAPES = [(32, 16), (256, 2), (256, 1)]
@@ -95,9 +95,12 @@ def test_make_params_refuses_a_negative_or_non_finite_gamma(gamma):
 
 
 def test_k3_layout_restatement():
-    """Consumer warps of the shapes the sweep uses for each count, and the refused shapes."""
+    """Consumer warps of the shapes the sweep uses for each count, and the refused shapes.  The second-moment row at T = 256, nu = 2
+    leaves room for two stages only next to their two consumers' partials; mode smooth's U region costs the ring a stage at 186 x 2."""
     assert [ws_layout(T, nu, "W")[1] for T, nu in [(1, 1), (125, 1), (146, 1), (174, 1), (216, 1), (187, 2)]] == [7, 6, 5, 4, 3, 2]
-    assert ws_layout(256, 2, "M2") is None and ws_layout(256, 2, "C") is not None
+    assert ws_layout(256, 2, "M2") == (16, 2, 2, 256) and ws_stages(256, 2, "M2") == 2 and ws_layout(256, 2, "C") is not None
+    assert _ws_bytes(256, 2, 2, "M2", WS_NCONS) > SMEM_CAP >= _ws_bytes(256, 2, 2, "M2")
+    assert ws_layout(186, 2, "W")[1:3] == (3, 3) and ws_layout(186, 2, "W", smooth=True)[1:3] == (2, 2)
     assert ws_layout(257, 1, "W") is None and ws_layout(57, 9, "W") is None
     assert [ws_layout(T, nu, "W")[3] for T, nu in [(37, 7), (251, 2), (129, 2), (32, 16)]] == [37, 251, 129, 256]
     assert [ws_layout(T, nu, k)[0] for T, nu, k in [(32, 4, "W"), (43, 3, "M2"), (16, 16, "C"), (129, 2, "C"), (32, 16, "C")]] == [4, 8, 8, 16, 16]
