@@ -140,13 +140,13 @@ class CudaBackend:
 
     def set_params(self, params: MppibParams):
         self._check_dist_fits(params, self.model, "mppib_set_params")
-        self.params = params
         self._check(self.lib.mppib_set_params(self.handle, C.byref(params)), "mppib_set_params")
+        self.params = params             # only once the library took it: a refused block leaves the handle as it was
 
     def set_model(self, model: MppibModel):
         self._check_dist_fits(self.params, model, "mppib_set_model")
-        self.model = model
         self._check(self.lib.mppib_set_model(self.handle, C.byref(model)), "mppib_set_model")
+        self.model = model
 
     def state_size(self) -> int:
         return int(self.lib.mppib_state_size(self.handle))

@@ -55,6 +55,7 @@ class MPPIisaacPlanner(object):
             assets_dirs=getattr(cfg, "assets_dirs", None) or None,
             backend=backend,
             observe=observe,
+            k_offset=self.k_offset,
         )
         # which rows does the Objective read?  (one dry run against dummy rows)
         self.sim.trace(lambda s: self.objective.compute_cost(s))

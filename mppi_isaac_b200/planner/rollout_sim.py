@@ -43,10 +43,11 @@ class RolloutSim:
     def __init__(self, cfg: IsaacGymConfig, actors: List[str], init_positions: Optional[List[List[float]]] = None,
                  num_envs: int = 1, viewer: bool = False, device: str = "cuda:0", interactive_goal: bool = True, *,
                  horizon: int = 1, mppi_cfg: Optional[MPPIConfig] = None, conf_dirs: Optional[Sequence[str]] = None,
-                 assets_dirs: Optional[Sequence[str]] = None, backend=None, observe="auto"):
+                 assets_dirs: Optional[Sequence[str]] = None, backend=None, observe="auto", k_offset: int = 0):
         if viewer or getattr(cfg, "viewer", False):
             raise NotImplementedError("the viewer is outside the rollout path (SURVEY.md section 2, row 12)")
         self.cfg = cfg
+        self.k_offset = int(k_offset)          # global index of this shard's first rollout (sharded plans)
         self.device = device
         self.num_envs = int(num_envs)
         self.interactive_goal = interactive_goal
@@ -119,6 +120,7 @@ class RolloutSim:
         mc = self._mppi_cfg if self._mppi_cfg is not None else self._default_mppi_cfg()
         mc = copy.copy(mc)
         mc.horizon = self._T
+        mc._k_offset = self.k_offset           # the kernels key per-rollout randomisation and CEM elite indices by the global index
         return make_params(mc, self.cfg, self.scene.nu, self.num_envs, self._obs_items)
 
     def _allocate(self):
