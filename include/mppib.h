@@ -42,6 +42,8 @@
  *                               over the whole control sequence, vectors ordered (t, j) like U
  *   partial  [2 + n + n(n+1)/2] (beta_g, eta_g, W_g, C_g[lower triangle of n x n]) with update_cov, cov_horizon and a registered
  *                               distribution
+ *   U, partial, dist with n_modes = M > 1: U[M][T][nu], partial [M][2 + T*nu] (one (beta, eta, W) block per mode), dist = the mode
+ *                               state [1 + M + T*nu] (see "Multi-modal MPPI" below)
  */
 #ifndef MPPIB_H
 #define MPPIB_H
@@ -52,7 +54,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 19
+#define MPPIB_ABI_VERSION 20
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -93,6 +95,7 @@ extern "C" {
 #define MPPIB_MODE_SMOOTH 3   /* Smooth MPPI: U is the control DERIVATIVE; actions are integrated from the last executed action (see below) */
 #define MPPIB_CEM_MAX_ELITES 128
 #define MPPIB_MAX_WORLDS 32   /* risk-aware MPPI: largest n_worlds (a group of worlds never straddles a 32-sample tile) */
+#define MPPIB_MAX_MODES 16    /* multi-modal MPPI: largest n_modes */
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -227,6 +230,10 @@ typedef struct MppibParams {
     /* risk-aware MPPI (see "Risk-aware MPPI" below); both are read only when n_worlds > 1, a zero block keeps today's planner      */
     int32_t n_worlds;          /* R: rollouts per control sample, a power of two in 1 .. MPPIB_MAX_WORLDS; K and k_offset are multiples */
     int32_t risk_tail;         /* m in 1 .. R: the score of a control is the mean of its m largest world costs (CVaR)              */
+    /* multi-modal MPPI (see "Multi-modal MPPI" below); read only when n_modes > 1, a zero block keeps today's planner               */
+    int32_t n_modes;           /* M in 1 .. MPPIB_MAX_MODES nominal sequences planned side by side                                   */
+    float   mode_margin;       /* >= 0: the executed mode is kept while its free energy is within this margin of the lowest          */
+    int32_t mode_samples;      /* Kc = K_total / M >= 32: global sample kg belongs to mode kg / Kc (the shard alone cannot tell K_total) */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -438,6 +445,27 @@ int32_t mppib_set_smooth_state(MppibHandle h, float* state);
  *   K4, the shift and the peer exchange are unchanged.  The launchers refuse a shard whose K or k_offset is not a multiple of R. */
 int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset,
                             uint32_t k_total, const float* U, float* actions, float* noise, void* stream);
+
+/* Multi-modal MPPI (n_modes = M > 1, mode_samples = Kc; modes SIMPLE and MEAN with the fixed Sigma; no update_cov / update_lambda,
+ * n_worlds, cem or smooth).  U is [M][T][nu], mode 0 first; global sample kg belongs to mode m(kg) = kg / Kc, a contiguous block, so a
+ * mode may span shards and a shard may hold several modes.  The mode state is a device buffer registered with mppib_set_distribution
+ * (caller-owned, initialised by the caller; only K4 writes it):
+ *   state    [1 + M + T*nu]  (active mode as a float, F[M], U_exec[T][nu])
+ *   K1     mppib_sample, mppib_sample_colored and mppib_sample_library draw sample kg around U + m(kg)*T*nu with the counters of the
+ *          global index: the columns of mode m equal today's K1 with U := U_m, bit for bit; k_total must be M * Kc
+ *   K3     one launch, CTAs (x, m): the shard row is M blocks of SIMPLE's / MEAN's row, [M][2 + T*nu], block m = (beta_m, eta_m, W_m)
+ *          over the shard's samples of mode m only (g_m = lambda Sigma^-1 U_m in SIMPLE mode); a mode without a sample on the shard
+ *          writes (+inf, 0, 0); a 32-sample tile straddling two modes is read by both modes' CTAs, each masking the other's lanes
+ *   K4     per mode: the G blocks m combined as today -> (beta_m, eta_m, W_m), the own step d_m = W_m/eta_m (SIMPLE) or
+ *          (1 - s) U_m + s W_m/eta_m - U_m (MEAN), d_m = 0 when eta_m = 0, F_m = beta_m - lambda ln(eta_m / Kc) (+inf when eta_m = 0);
+ *          then, from the U before the update, in float32 with every sum over j in ascending order:
+ *            D_ij = sum_t (U_it - U_jt)^T Sigma^-1 (U_it - U_jt),  h = lower median {D_ij : i < j} / ln(M + 1),  k_ij = exp(-D_ij / h),
+ *            U_i <- U_i + (sum_j k_ij d_j + (2/h) sum_j k_ij (U_i - U_j)) / sum_j k_ij   (k = 1 and no second term if h is 0 or not finite)
+ *          then Savitzky-Golay (filter_u) and the clamp to every mode; the executed mode p is kept while F_p <= min F + mode_margin,
+ *          otherwise it becomes argmin F (lowest index; all F infinite keeps p); the action, its mirror and stats = (beta_p, eta_p) come
+ *          from mode p, and the state receives (p, F, U_p).
+ *   shift  every mode as U is shifted today.
+ * Reduce and finalize refuse M > 1 while no mode state is registered.                                                             */
 
 #ifdef __cplusplus
 }

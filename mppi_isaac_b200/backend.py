@@ -60,6 +60,9 @@ def dist_floats(params, nu):
     """(floats, layout) of the distribution buffer that K1 / K3 / K4 read under `params` with `nu` inputs: 1 + 3 n^2 with cov_horizon
     (n = T*nu), 1 + 3 nu^2 with cov_full, 1 + nu otherwise (update_cov with a diagonal Sigma, or update_lambda alone)."""
     nu = int(nu)
+    if params.n_modes > 1:
+        M = int(params.n_modes)
+        return 1 + M + int(params.T) * nu, f"n_modes > 1 mode state (active mode, F[M], U_exec[T*nu], M = {M})"
     if params.mode == MODE_CEM:
         n, E = int(params.T) * nu, int(params.n_elites)
         return 2 + E + n + E * n, f"mppi_mode cem (carry offset, elites valid, S_elite[E], sigma[T*nu], elites[E][T*nu], E = {E})"
@@ -242,6 +245,8 @@ class CudaBackend:
         """Floats of one shard row K3 writes with a registered distribution: 2 + T*nu, + T*nu with update_cov, + nu(nu+1)/2
         with update_cov and cov_full, or + n(n+1)/2 with update_cov and cov_horizon (n = T*nu)."""
         T, nu = int(self.params.T), int(self.model.nu)
+        if self.params.n_modes > 1:
+            return int(self.params.n_modes) * (2 + T * nu)
         if self.params.mode == MODE_CEM:
             return cem_row_floats(T, nu, self.params.n_elites)
         if self._cov_horizon():
@@ -252,9 +257,9 @@ class CudaBackend:
         return 2 + T * nu * (2 if self.params.update_cov else 1)
 
     def _check_row(self, rows, what):
-        if ((self._cov_full() or self._cov_horizon() or self.params.mode == MODE_CEM) and self._dist_keepalive is not None and rows is not None
-                and rows.shape[-1] != self.partial_row_floats()):
-            kind = "mppi_mode cem" if self.params.mode == MODE_CEM else "cov_horizon" if self._cov_horizon() else "cov_full"
+        if ((self._cov_full() or self._cov_horizon() or self.params.mode == MODE_CEM or self.params.n_modes > 1) and self._dist_keepalive is not None
+                and rows is not None and rows.shape[-1] != self.partial_row_floats()):
+            kind = "n_modes > 1" if self.params.n_modes > 1 else "mppi_mode cem" if self.params.mode == MODE_CEM else "cov_horizon" if self._cov_horizon() else "cov_full"
             raise RuntimeError(f"{what}: {kind} shard rows hold {self.partial_row_floats()} floats, got {rows.shape[-1]}")
 
     def _check_dist_fits(self, params, model, what):
@@ -276,7 +281,7 @@ class CudaBackend:
     def set_distribution(self, dist):
         """Adaptive MPPI: register the device tensor (lambda, cov[nu]) -- with cov_full (lambda, Sigma, L, Sigma^-1), 1 + 3 nu^2
         floats, with cov_horizon (lambda, Sigma_H, L_H, Sigma_H^-1), 1 + 3 n^2 floats, n = T*nu -- that K1 / K3 read and K4 updates
-        (None switches it off).  With mppi_mode cem it is the CEM state (``dist_floats``)."""
+        (None switches it off).  With mppi_mode cem it is the CEM state, with n_modes > 1 the mode state (``dist_floats``)."""
         if dist is not None:
             need, layout = dist_floats(self.params, self.model.nu)
             if dist.numel() != need:

@@ -74,6 +74,19 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "n_worlds > 1 excludes mode cem and mode smooth");
         MPPIB_REQUIRE(!p->cov_horizon, "n_worlds > 1 excludes cov_horizon");
     }
+    MPPIB_REQUIRE(p->n_modes >= 0 && p->n_modes <= MPPIB_MAX_MODES, "n_modes = %d out of range [1, %d]", p->n_modes, MPPIB_MAX_MODES);
+    MPPIB_REQUIRE(isfinite(p->mode_margin) && p->mode_margin >= 0.f, "mode_margin = %g must be finite and >= 0", p->mode_margin);
+    if (p->n_modes > 1) {
+        const int M = p->n_modes;
+        MPPIB_REQUIRE(p->mode_samples >= 32, "n_modes = %d: mode_samples = %d must be at least 32 (a 32-sample tile straddles at most two modes)", M,
+                      p->mode_samples);
+        MPPIB_REQUIRE((uint64_t)p->k_offset + (uint64_t)p->K <= (uint64_t)M * (uint64_t)p->mode_samples,
+                      "n_modes = %d: the shard [%u, +%d) exceeds n_modes * mode_samples = %d", M, p->k_offset, p->K, M * p->mode_samples);
+        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "n_modes > 1 excludes mode cem and mode smooth");
+        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "n_modes > 1 excludes update_cov and update_lambda (the adapted distribution belongs to one mean)");
+        MPPIB_REQUIRE(p->n_worlds <= 1, "n_modes > 1 excludes n_worlds > 1");
+        MPPIB_REQUIRE(p->T * m->nu <= 512, "n_modes > 1 needs T*nu <= 512, got %d", p->T * m->nu);
+    }
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);

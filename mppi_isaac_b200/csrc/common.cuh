@@ -85,6 +85,7 @@ struct DeviceGuard {
 __host__ __device__ static inline int cem_row_floats(int T, int nu, int E) { return (2 * E + E * T * nu + 3) & ~3; }
 static inline int cem_state_floats(int T, int nu, int E) { return 2 + E + T * nu + E * T * nu; }
 static inline int partial_row_capacity(const MppibParams& p, int nu) {
+    if (p.n_modes > 1) return p.n_modes * (2 + p.T * nu);
     if (p.mode == MPPIB_MODE_CEM) return cem_row_floats(p.T, nu, p.n_elites);
     if (p.update_cov && p.cov_full) return 2 + p.T * nu + nu * (nu + 1) / 2;
     if (p.update_cov && p.cov_horizon) return 2 + p.T * nu + p.T * nu * (p.T * nu + 1) / 2;
@@ -95,6 +96,10 @@ static inline int partial_row_capacity(const MppibParams& p, int nu) {
 __device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
 __device__ __forceinline__ uint32_t sample_world(uint32_t kg, int R) { return R > 1 ? kg & (uint32_t)(R - 1) : kg; }
 static inline bool risk_mode(const MppibContext* c) { return c->params.n_worlds > 1; }
+// Multi-modal MPPI (n_modes = M > 1): global sample kg is drawn around mode kg / Kc of U[M][T][nu], Kc = mode_samples.  M <= 1 (and a
+// zero-initialised block) keeps mode 0 for every sample.
+__device__ __forceinline__ int sample_mode(uint32_t kg, const MppibParams& p) { return p.n_modes > 1 ? (int)(kg / (uint32_t)p.mode_samples) : 0; }
+static inline bool modes_on(const MppibContext* c) { return c->params.n_modes > 1; }
 static inline bool cem_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_CEM; }
 static inline bool smooth_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_SMOOTH; }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }

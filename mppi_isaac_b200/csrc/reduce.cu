@@ -15,6 +15,8 @@
 // Algorithmic bytes per launch: 4*K*T*(nu+1) + 4*(T*nu+2)   (BASELINE.md section 3).
 #include <cuda.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {
@@ -35,6 +37,11 @@ __host__ __device__ __forceinline__ int full_fin_floats(int T, int nu) { return 
 __host__ __device__ __forceinline__ int hz_row_floats(int n) { return 2 + n + n * (n + 1) / 2; }
 __host__ __device__ __forceinline__ int hz_fin_floats(int n) { return 4 * n + n * (n + 1) / 2; }
 __device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }     // offset of row i in a packed lower triangle
+// n_modes = M > 1: the shared floats modes_rows needs with G shard rows: d[M*T*nu], Sigma^-1 U then the coupled U [M*T*nu], U[M*T*nu],
+// Sigma^-1, the G scales of every mode, (beta, eta, F, sum_j k_ij)[M], D[M][M], k[M][M] and 4 floats
+__host__ __device__ __forceinline__ int modes_fin_floats(int NR, int M, int G) {
+    return 3 * M * NR + MPPIB_MAX_NU * MPPIB_MAX_NU + M * G + 4 * M + 2 * M * M + 4;
+}
 
 __device__ __forceinline__ float warp_min(float v) {
 #pragma unroll
@@ -409,6 +416,226 @@ __device__ __forceinline__ void smooth_rows(const MppibParams& p, int nu, const 
     if (threadIdx.x == 0 && stats) { stats[0] = b; stats[1] = e; }
 }
 
+// K4 of multi-modal MPPI (n_modes = M > 1, include/mppib.h "Multi-modal MPPI"; state = (active mode, F[M], U_exec[T][nu])): combine
+// the G blocks of every mode as finalize_rows does, form the own steps d_m and free energies F_m, couple the modes (SVGD step with the
+// RBF kernel in the Sigma^-1 metric, median bandwidth), Savitzky-Golay and clamp every mode, select the executed mode and write the
+// action, stats and state from it.  U[M][T][nu] and Sigma^-1 are staged in shared memory first; D_ij = sum_r (U_i - U_j)_r (V_i - V_j)_r
+// with V_m = Sigma^-1 U_m per step, one warp per pair (lane = row, then the warp's butterfly sum); every other sum runs in a fixed
+// order on one thread, so every rank, which combines the same rows in the same order, writes the same bits.  `sm` = modes_fin_floats.
+__device__ __noinline__ void modes_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
+                                        float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* sm,
+                                        float* __restrict__ state) {
+    const int T = p.T, NR = T * nu, M = p.n_modes, P1 = 2 + NR, MN = M * NR;
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
+    float* dd = sm;                  // [M*NR] own steps, then the final sequences
+    float* un = dd + MN;             // [M*NR] V = Sigma^-1 U per step, then the coupled sequences before Savitzky-Golay
+    float* us = un + MN;             // [M*NR] U as it was
+    float* si = us + MN;             // [nu*nu] Sigma^-1
+    float* sg = si + MPPIB_MAX_NU * MPPIB_MAX_NU;   // [M][G]
+    float* bm = sg + M * G;
+    float* em = bm + M;
+    float* fm = em + M;
+    float* ks = fm + M;
+    float* Dm = ks + M;              // [M][M]
+    float* km = Dm + M * M;          // [M][M]
+    float* misc = km + M * M;        // h, executed mode
+    const float lam = p.lambda_, inv_lambda = 1.0f / lam;
+    const bool simple = p.mode == MPPIB_MODE_SIMPLE;
+    for (int q = tid; q < MN; q += nt) us[q] = U[q];
+    for (int q = tid; q < nu * nu; q += nt) si[q] = p.sigma_inv[q];
+    for (int m = tid; m < M; m += nt) {
+        float b = INFINITY;
+        for (int g = 0; g < G; ++g) {
+            const float* row = partials + (size_t)g * P + (size_t)m * P1;
+            if (__ldcg(row + 1) > 0.f) b = fminf(b, __ldcg(row));
+        }
+        bm[m] = b;
+    }
+    __syncthreads();
+    for (int q = tid; q < M * G; q += nt) {
+        const int m = q / G, g = q % G;
+        const float* row = partials + (size_t)g * P + (size_t)m * P1;
+        const float eg = __ldcg(row + 1);
+        sg[q] = eg > 0.f ? expf(-(__ldcg(row) - bm[m]) * inv_lambda) : 0.f;
+    }
+    __syncthreads();
+    for (int m = tid; m < M; m += nt) {
+        float e = 0.f;
+        for (int g = 0; g < G; ++g) e += sg[m * G + g] * __ldcg(partials + (size_t)g * P + (size_t)m * P1 + 1);
+        em[m] = e;
+        fm[m] = e > 0.f ? bm[m] - lam * logf(e / (float)p.mode_samples) : INFINITY;
+    }
+    __syncthreads();
+    for (int q = tid; q < MN; q += nt) {                                      // own MPPI step of every mode
+        const int m = q / NR, r = q % NR;
+        float w = 0.f;
+        for (int g = 0; g < G; ++g) w += sg[m * G + g] * __ldcg(partials + (size_t)g * P + (size_t)m * P1 + 2 + r);
+        const float e = em[m], u = us[q];
+        float d = 0.f;
+        if (e > 0.f) {
+            const float wm = w / e;
+            d = simple ? wm : (1.0f - p.step_size_mean) * u + p.step_size_mean * wm - u;
+        }
+        dd[q] = d;
+        const int t = r / nu, a = r % nu;
+        const float* ut = us + (size_t)m * NR + t * nu;
+        float v = 0.f;
+        for (int b = 0; b < nu; ++b) v += si[a * nu + b] * ut[b];
+        un[q] = v;
+    }
+    __syncthreads();
+    const int npairs = M * (M - 1) / 2;
+    for (int q = warp; q < npairs; q += nw) {                                 // D_ij, i < j: one warp per pair
+        int i = 0, rem = q;
+        while (rem >= M - 1 - i) { rem -= M - 1 - i; ++i; }
+        const int j = i + 1 + rem;
+        const float* Ui = us + (size_t)i * NR;
+        const float* Uj = us + (size_t)j * NR;
+        const float* Vi = un + (size_t)i * NR;
+        const float* Vj = un + (size_t)j * NR;
+        float acc = 0.f;
+        for (int r = lane; r < NR; r += 32) acc += (Ui[r] - Uj[r]) * (Vi[r] - Vj[r]);
+        acc = warp_sum(acc);
+        if (lane == 0) { Dm[i * M + j] = acc; Dm[j * M + i] = acc; }
+    }
+    for (int i = tid; i < M; i += nt) Dm[i * M + i] = 0.f;
+    if (tid == 0) misc[0] = NAN;                                              // no pair of that rank (a NaN distance): k = 1
+    __syncthreads();
+    for (int q = tid; q < npairs; q += nt) {                                  // the lower median: the pair of rank (npairs - 1) / 2
+        int i = 0, rem = q;
+        while (rem >= M - 1 - i) { rem -= M - 1 - i; ++i; }
+        const float v = Dm[i * M + i + 1 + rem];
+        int rank = 0;
+        for (int q2 = 0, i2 = 0, j2 = 1; q2 < npairs; ++q2) {
+            const float v2 = Dm[i2 * M + j2];
+            rank += (v2 < v || (v2 == v && q2 < q)) ? 1 : 0;
+            if (++j2 == M) { ++i2; j2 = i2 + 1; }
+        }
+        if (rank == (npairs - 1) / 2) misc[0] = v / logf((float)(M + 1));
+    }
+    __syncthreads();
+    const float h = misc[0];
+    const bool kern = h > 0.f && isfinite(h);
+    for (int q = tid; q < M * M; q += nt) km[q] = kern ? expf(-Dm[q] / h) : 1.0f;
+    __syncthreads();
+    for (int i = tid; i < M; i += nt) {
+        float sk = 0.f;
+        for (int j = 0; j < M; ++j) sk += km[i * M + j];
+        ks[i] = sk;
+    }
+    __syncthreads();
+    const float c2 = kern ? 2.0f / h : 0.f;
+    for (int q = tid; q < MN; q += nt) {                                      // the coupled step, j ascending
+        const int i = q / NR, r = q % NR;
+        const float ui = us[q];
+        float a1 = 0.f, a2 = 0.f;
+        for (int j = 0; j < M; ++j) {
+            const float k = km[i * M + j];
+            a1 += k * dd[j * NR + r];
+            a2 += k * (ui - us[(size_t)j * NR + r]);
+        }
+        un[q] = ui + (kern ? a1 + c2 * a2 : a1) / ks[i];
+    }
+    __syncthreads();
+    for (int q = tid; q < MN; q += nt) {                                      // Savitzky-Golay (filter_u) and the clamp, every mode
+        const int m = q / NR, r = q % NR, t = r / nu, j = r % nu;
+        const float* u = un + (size_t)m * NR;
+        float out = u[r];
+        if (p.filter_u) {
+            float s = 0.f;
+            if (t < 4) {
+#pragma unroll
+                for (int i = 0; i < 9; ++i) s += c_sg_edge[t][i] * u[i * nu + j];
+                s *= (1.0f / 1155.0f);
+            } else if (t >= T - 4) {
+                const int ee = T - 1 - t;
+#pragma unroll
+                for (int i = 0; i < 9; ++i) s += c_sg_edge[ee][i] * u[(T - 1 - i) * nu + j];
+                s *= (1.0f / 1155.0f);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 9; ++i) s += c_sg_mid[i] * u[(t - 4 + i) * nu + j];
+                s *= (1.0f / 231.0f);
+            }
+            out = s;
+        }
+        out = fminf(fmaxf(out, p.u_min[j]), p.u_max[j]);
+        dd[q] = out;
+        U[q] = out;
+    }
+    if (tid == 0) {                                                           // the executed mode
+        int pm = (int)state[0];
+        pm = pm < 0 ? 0 : pm >= M ? M - 1 : pm;
+        int a = 0;
+        for (int m = 1; m < M; ++m) if (fm[m] < fm[a]) a = m;
+        if (isfinite(fm[a]) && !(fm[pm] <= fm[a] + p.mode_margin)) pm = a;
+        misc[1] = (float)pm;
+        state[0] = (float)pm;
+        if (stats) { stats[0] = bm[pm]; stats[1] = em[pm]; }
+    }
+    __syncthreads();
+    const int pe = (int)misc[1];
+    for (int m = tid; m < M; m += nt) state[1 + m] = fm[m];
+    for (int r = tid; r < NR; r += nt) {
+        const float v = dd[(size_t)pe * NR + r];
+        state[1 + M + r] = v;
+        if (r < nu) { action_out[r] = v; if (action_mirror) action_mirror[r] = v; }
+    }
+}
+
+// n_modes = M > 1, the last CTA of K3: the gridDim.x CTA partials of every mode m (scratch rows m*gx .. m*gx + gx - 1, stride P4 of the
+// mode's row P1 = 2 + T*nu) fold into block m of the shard row [M][P1] in CTA order; the row goes into the peer windows as
+// fold_and_finish stores it and, for single-GPU plans, modes_rows does K4's work in place.
+__device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int nu, int P1, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
+                                                      float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U,
+                                                      float* __restrict__ fin_action, float* __restrict__ fin_stats, float* __restrict__ fin_mirror,
+                                                      float* tiles, float inv_lambda, float* __restrict__ state) {
+    const int tid = threadIdx.x, M = (int)gridDim.y, gx = (int)gridDim.x, nrow = M * gx, P = M * P1, P4 = (P1 + 3) & ~3;
+    float* sc = tiles;               // [M*gx] CTA beta, then scale
+    float* bb = tiles + nrow;        // [M] mode minimum
+    for (int q = tid; q < nrow; q += NT) sc[q] = __ldcg(scratch + (size_t)q * P4);
+    __syncthreads();
+    for (int m = tid; m < M; m += NT) {
+        float b = INFINITY;
+        for (int g = 0; g < gx; ++g) b = fminf(b, sc[m * gx + g]);
+        bb[m] = b;
+    }
+    __syncthreads();
+    for (int q = tid; q < nrow; q += NT) {
+        const float b = sc[q];
+        sc[q] = b == INFINITY ? 0.f : expf(-(b - bb[q / gx]) * inv_lambda);
+    }
+    __syncthreads();
+    uint32_t seq = 0;
+    if (peers.world > 1) seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
+    const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
+    for (int q = tid; q < P; q += NT) {
+        const int m = q / P1, e = q % P1;
+        const float* src = scratch + (size_t)m * gx * P4 + e;
+        const float* scm = sc + m * gx;
+        float v = 0.f;
+#pragma unroll 4
+        for (int g = 0; g < gx; ++g) v += scm[g] * __ldcg(src + (size_t)g * P4);
+        if (e == 0) v = bb[m];
+        partial[q] = v;
+        for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + q] = v;
+    }
+    if (peers.world > 1) {
+        __threadfence_system();
+        __syncthreads();
+        if (tid < peers.world) {
+            uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
+            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
+        }
+    }
+    if (tid == 0) *ticket = 0u;
+    if (fin_U != nullptr) {
+        __threadfence();
+        __syncthreads();
+        modes_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, state);
+    }
+}
+
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
 // at least, `misc` = 8 floats.
@@ -520,12 +747,13 @@ struct WsLayout {
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
     // kind: what the shard row carries after W (RowKind); nparts: warp partials stored, by default one per consumer warp
     // (min(nstage, WS_NCONS): the launch rounds the ring depth down to a multiple of the consumer count)
-    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false, int nparts = -1) {
+    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false, int nparts = -1, int modes = 1) {
         const int NR = T * nu, P4 = (row_floats(T, nu, kind) + 3) & ~3;
         if (nparts < 0) nparts = nstage < WS_NCONS ? nstage : WS_NCONS;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
         if (kind == ROW_C && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
+        if (modes > 1 && g < modes_fin_floats(NR, modes, 1)) g = modes_fin_floats(NR, modes, 1);   // the fused K4 of n_modes > 1
         gp = g + ((NR + 3) & ~3);
         wk = gp + ((T + 3) & ~3);
         cpart = wk + 8 * WS_W;
@@ -555,7 +783,10 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // are SIMPLE's), and the fused K4 integrates the state `smooth`.
 // RISK (n_worlds = R > 1): phase B replaces the S of every aligned group of R samples by its CVaR score on the group's first lane and
 // +inf on the others (risk_score); a tile is 32 samples and every shard starts at a multiple of R, so no group straddles two tiles.
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false>   // rows of W per lane: T*nu <= 32 * RPL
+// MODES (n_modes = M > 1): the grid is (gx, M) and CTA (x, m) walks only the tiles that hold samples of mode m, with g = lambda Sigma^-1
+// U_m; the lanes of a straddling tile that belong to the other mode are masked (weight 0, not in the minimum).  Its partial is scratch
+// row m*gx + x, and the last CTA folds every mode into block m of the row [M][2 + T*nu] (fold_modes_and_finish).
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false, bool MODES = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
@@ -565,6 +796,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if constexpr (MODES) U += (size_t)blockIdx.y * NR;                       // this CTA's mode
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
     const bool simple = SMOOTH || p.mode == MPPIB_MODE_SIMPLE;
@@ -575,7 +807,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
     const bool smooth_term = SMOOTH && p.smooth_weight != 0.f;
-    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, smooth_term);
+    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, smooth_term, -1, MODES ? p.n_modes : 1);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -585,13 +817,20 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + L.bar);           // [nstage]
     uint64_t* empty = full + nstage;                                          // [nstage]
 
-    const int ntiles = (K + WS_W - 1) / WS_W;
+    int ntiles = (K + WS_W - 1) / WS_W, tile0 = 0, lo = 0, hi = K;            // MODES: the local samples [lo, hi) of this CTA's mode
+    if constexpr (MODES) {
+        const int m = (int)blockIdx.y, kc = p.mode_samples, ko = (int)p.k_offset;
+        lo = max(0, m * kc - ko);
+        hi = min(K, (m + 1) * kc - ko);
+        tile0 = lo / WS_W;
+        ntiles = hi > lo ? (hi + WS_W - 1) / WS_W - tile0 : 0;
+    }
     const int my_tiles = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const uint32_t tile_bytes = (uint32_t)tile_floats * 4u;
 
     auto issue_tile = [&](int i) {   // elected producer lane: TMA tile i of this CTA into ring stage i % nstage
         const int s = i % nstage;
-        const int k0 = ((int)blockIdx.x + i * (int)gridDim.x) * WS_W;
+        const int k0 = (tile0 + (int)blockIdx.x + i * (int)gridDim.x) * WS_W;
         float* dst = tiles + (size_t)s * tile_floats;
         mbar_expect_tx(&full[s], tile_bytes);
         for (int r0 = 0; r0 < NR; r0 += xbox_rows) tma_load_2d(dst + (size_t)r0 * WS_W, &tm_x, k0, r0, &full[s]);
@@ -660,7 +899,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         }
         for (int i = c; i < my_tiles; i += ncons) {
             const int s = i % nstage;
-            const int k0 = ((int)blockIdx.x + i * (int)gridDim.x) * WS_W;
+            const int k0 = (tile0 + (int)blockIdx.x + i * (int)gridDim.x) * WS_W;
             const float* xs = tiles + (size_t)s * tile_floats;                // [NR][32]
             const float* cs = xs + (size_t)NR * WS_W;                         // [T][32]
             mbar_wait(&full[s], (uint32_t)((i / nstage) & 1));
@@ -699,7 +938,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                 }
             }
             // ---- B: tile minimum, weights, their sum
-            const bool valid = (k0 + lane < K) && isfinite(sum);
+            const bool valid = (k0 + lane < K) && isfinite(sum) && (!MODES || (k0 + lane >= lo && k0 + lane < hi));
             float S = valid ? sum : INFINITY;
             if constexpr (RISK) S = risk_score(S, p.n_worlds, p.risk_tail, lane);
             if (HZN && k0 + lane < K) hz_S[k0 + lane] = S;
@@ -789,7 +1028,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __syncthreads();
     // ---- merge the warp partials into the CTA partial (global scratch), then ticket -> the last CTA folds all of them
     {
-        float* mine = scratch + (size_t)blockIdx.x * P4;
+        float* mine = scratch + (size_t)(blockIdx.x + (MODES ? blockIdx.y * gridDim.x : 0u)) * P4;
         float bb = INFINITY;
 #pragma unroll
         for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = fminf(bb, cpart[(size_t)c * P4]);
@@ -809,24 +1048,29 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __threadfence();
     __syncthreads();
     __shared__ unsigned int s_last_ws;
-    if (tid == 0) s_last_ws = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1u : 0u;
+    if (tid == 0) s_last_ws = atomicAdd(ticket, 1u) == (MODES ? gridDim.x * gridDim.y : gridDim.x) - 1 ? 1u : 0u;
     __syncthreads();
     if (!s_last_ws) return;
     __threadfence();
+    if constexpr (MODES) {
+        fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
+        return;
+    }
     fold_and_finish<ADAPT, FULL, SMOOTH>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist,
                                          smooth);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
-// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon); SMOOTH: smooth_rows.
-template <bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false>
+// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon); SMOOTH: smooth_rows;
+// MODES: modes_rows (n_modes > 1, dist = the mode state).
+template <bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool MODES = false>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
                 float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const int T = p.T, NR = T * nu;
-    int P = HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
+    int P = MODES ? p.n_modes * (2 + NR) : HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
     const float* partials = partials_in;
     uint32_t seq = 0;
     if (partials_in == nullptr) {
@@ -852,7 +1096,8 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
         partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
         P = peers.pcap;
     }
-    if constexpr (SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
+    if constexpr (MODES) modes_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
+    else if constexpr (SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
     else finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
 }
@@ -1009,6 +1254,16 @@ __global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu
     }
 }
 
+// n_modes = M > 1: every mode of U[M][T][nu] shifts as U does (the appended step is u_init)
+__global__ void mppib_shift_modes_kernel(const __grid_constant__ MppibParams p, int nu, float* __restrict__ U, uint32_t* __restrict__ plan_ctr) {
+    extern __shared__ float tmp[];
+    const int NR = p.T * nu, MN = p.n_modes * NR;
+    for (int q = threadIdx.x; q < MN; q += blockDim.x) tmp[q] = q % NR + nu < NR ? U[q + nu] : p.u_init[q % nu];
+    __syncthreads();
+    for (int q = threadIdx.x; q < MN; q += blockDim.x) U[q] = tmp[q];
+    if (threadIdx.x == 0 && plan_ctr) *plan_ctr += 1u;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1056,7 +1311,7 @@ static int reduce_ws_stages(int T, int nu, int kind, bool smooth = false) {
     return ns;
 }
 
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false>
+template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false, bool MODES = false>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
@@ -1067,11 +1322,12 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     const int nstage_max = reduce_ws_stages(T, nu, kind, smooth_term);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const size_t smem = WsLayout(T, nu, nstage, kind, smooth_term).bytes;
+    const int modes = MODES ? c->params.n_modes : 1;
+    const size_t smem = WsLayout(T, nu, nstage, kind, smooth_term, -1, modes).bytes;
     static size_t smem_attr[64] = {0};
     size_t& attr = smem_attr[c->device & 63];
     if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK, MODES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr = smem;
     }
     int xbox_rows = NR < 256 ? NR : 256;
@@ -1087,10 +1343,22 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     const int ntiles = (K + WS_W - 1) / WS_W;
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
     if (grid > MAX_GRID) grid = MAX_GRID;
+    if (MODES) {
+        // gx CTAs per mode, about one per SM over all modes, no more than the tiles of the largest mode's local range
+        int tmax = 0;
+        for (int m = 0; m < modes; ++m) {
+            const long long lo = std::max(0LL, (long long)m * c->params.mode_samples - c->params.k_offset);
+            const long long hi = std::min((long long)K, (long long)(m + 1) * c->params.mode_samples - c->params.k_offset);
+            if (hi > lo) tmax = std::max(tmax, (int)((hi + WS_W - 1) / WS_W - lo / WS_W));
+        }
+        grid = std::max(1, std::min(tmax, c->num_sms / modes));
+        MPPIB_REQUIRE((long long)grid * modes * ((2 + NR + 3) & ~3) <= (long long)c->reduce_max_ctas * (((long long)partial_row_capacity(c->params, nu) + 3) & ~3LL),
+                      "mppib_reduce: scratch too small");
+    }
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
     PeerArgs peers = reduce_peers(c);
     if (HZN) peers.world = 0;                                                 // the row is complete only after the SYRK, which stores it
-    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK><<<grid, NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
+    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK, MODES><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
                                                                             c->reduce_scratch, c->reduce_ticket, partial, peers, fin_U, fin_action,
                                                                             fin_stats, fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g,
                                                                             SMOOTH ? c->smooth : nullptr);
@@ -1173,6 +1441,12 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(T, nu, ROW_C) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the covariance row of cov_full", T, nu);
     const int NR = T * nu;
+    if (modes_on(c)) {
+        MPPIB_REQUIRE(c->dist != nullptr, "mppib_reduce: n_modes > 1 needs its mode state registered with mppib_set_distribution");
+        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        return launch_reduce_ws_t<16, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    }
     if (smooth_mode(c)) {
         MPPIB_REQUIRE(c->smooth != nullptr, "mppib_reduce: mode smooth needs its state registered with mppib_set_smooth_state");
         MPPIB_REQUIRE(reduce_ws_stages(T, nu, ROW_W, true) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages in mode smooth", T, nu);
@@ -1225,7 +1499,19 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    if (smooth_mode(c)) {
+    if (modes_on(c)) {
+        MPPIB_REQUIRE(c->dist != nullptr, "mppib_finalize: n_modes > 1 needs its mode state registered with mppib_set_distribution");
+        const int smem = (int)sizeof(float) * modes_fin_floats(NR, c->params.n_modes, G);
+        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: n_modes = %d with T*nu = %d and G = %d needs %d bytes of shared memory", c->params.n_modes, NR, G, smem);
+        static int smem_attr[64] = {0};
+        int& attr = smem_attr[c->device & 63];
+        if (smem > attr) {
+            MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_finalize_kernel<false, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            attr = smem;
+        }
+        mppib_finalize_kernel<false, false, false, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
+                                                                                   c->action_mirror, c->dist, nullptr, nullptr);
+    } else if (smooth_mode(c)) {
         MPPIB_REQUIRE(c->smooth != nullptr, "mppib_finalize: mode smooth needs its state registered with mppib_set_smooth_state");
         mppib_finalize_kernel<false, false, false, true><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats,
                                                                                                 peer_args(c), c->action_mirror, nullptr, nullptr, c->smooth);
@@ -1259,6 +1545,11 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
 
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
+    if (modes_on(c)) {
+        mppib_shift_modes_kernel<<<1, 256, c->params.n_modes * NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr);
+        MPPIB_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
     float* hz_g = adaptive_horizon(c) && c->params.mode == MPPIB_MODE_SIMPLE ? c->hz_g : nullptr;
     mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g);
     MPPIB_CHECK_CUDA(cudaGetLastError());

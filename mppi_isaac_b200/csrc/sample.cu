@@ -69,7 +69,9 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
 }
 
 // DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block); with
-// n_worlds = R > 1 the control sample kg / R replaces the global sample in the counter and in the null / prior tests.
+// n_worlds = R > 1 the control sample kg / R replaces the global sample in the counter and in the null / prior tests.  With n_modes > 1
+// the sample is drawn around its mode's sequence (sample_mode), the counter stays the global sample; n_modes > 1 excludes update_cov,
+// so only the fixed-Sigma instantiations (not DIAG / FULL) carry the mode offset.
 template <bool DIAG, bool FULL = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
@@ -93,7 +95,9 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
     }
     const bool is_null = p.sample_null_action && kc == kc_last;
     const bool is_prior = prior_row != nullptr && kc + 1 == kc_last;
-    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+    const float* Um = U;
+    if constexpr (!DIAG && !FULL) Um += (size_t)sample_mode(k_offset + (uint32_t)k, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
+    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
 }
 
 // The white Philox draws of a tile of S samples [k0, k0 + S) to shared memory, zs[(t*nu + i) * S + sample]: the draws of the
@@ -173,6 +177,8 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const uint32_t kc = sample_control(kg, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
     const bool is_null = p.sample_null_action && kc == kc_total - 1;
     const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
+    const float* Um = U;
+    if constexpr (!DIAG && !FULL && !CEM) Um += (size_t)sample_mode(kg, p) * (T * nu);   // n_modes > 1 (fixed Sigma only)
     const float* zl = cs + lane;
     for (int tl = warp; tl < (T + 1) / 2; tl += 4) {
         const int th = T - 1 - tl;                                            // th >= tl; th == tl for the middle row of an odd T
@@ -207,8 +213,8 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             cem_clamp_store(p, nu, wl, tl, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
             if (th != tl) cem_clamp_store(p, nu, wh, th, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
         } else {
-            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, U, prior_row, actions, noise, dist);
-            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, U, prior_row, actions, noise, dist);
+            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
+            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
         }
     }
 }
@@ -335,6 +341,7 @@ mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
     const bool is_null = p.sample_null_action && kc == kc_total - 1;
     const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
+    if constexpr (!DIAG && !FULL) U += (size_t)sample_mode(k_offset + (uint32_t)k, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
     if constexpr (FULL) {
         const float* Ld = dist + 1 + nu * nu;
         float zc[MPPIB_MAX_NU];
@@ -475,6 +482,15 @@ int check_risk_shard(const MppibContext* c, const char* who, uint32_t k_offset, 
     return 0;
 }
 
+// Multi-modal MPPI: the modes' blocks of Kc samples cover exactly the k_total samples of the plan
+int check_modes_total(const MppibContext* c, const char* who, uint32_t k_total) {
+    if (!modes_on(c)) return 0;
+    MPPIB_REQUIRE((uint64_t)k_total == (uint64_t)c->params.n_modes * (uint64_t)c->params.mode_samples,
+                  "%s: n_modes = %d with mode_samples = %d needs k_total = %d, got %u", who, c->params.n_modes, c->params.mode_samples,
+                  c->params.n_modes * c->params.mode_samples, k_total);
+    return 0;
+}
+
 }  // namespace
 
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
@@ -497,6 +513,7 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_library: mode smooth samples through mppib_sample_smooth");
     if (int rc = check_risk_shard(c, "mppib_sample_library", k_offset, k_total)) return rc;
+    if (int rc = check_modes_total(c, "mppib_sample_library", k_total)) return rc;
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -516,6 +533,7 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample: mode cem samples through mppib_sample_colored (white noise: Lt = I)");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample: mode smooth samples through mppib_sample_smooth");
     if (int rc = check_risk_shard(c, "mppib_sample", k_offset, k_total)) return rc;
+    if (int rc = check_modes_total(c, "mppib_sample", k_total)) return rc;
     const int K = c->params.K, T = c->params.T;
     dim3 block(128), grid((K + 127) / 128, T);
     if (adaptive_horizon(c))
@@ -538,6 +556,7 @@ int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, con
     const int T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_colored: mode smooth samples through mppib_sample_smooth");
     if (int rc = check_risk_shard(c, "mppib_sample_colored", k_offset, k_total)) return rc;
+    if (int rc = check_modes_total(c, "mppib_sample_colored", k_total)) return rc;
     MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
     MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
                   CL_MAX_N, T, T * nu);

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 19
+ABI_VERSION = 20
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -31,6 +31,7 @@ OWNER_STATIC, OWNER_LINK, OWNER_FREE = 0, 1, 2
 MODE_SIMPLE, MODE_MEAN, MODE_CEM, MODE_SMOOTH = 0, 1, 2, 3
 CEM_MAX_ELITES = 128
 MAX_WORLDS = 32                                 # risk-aware MPPI: largest n_worlds
+MAX_MODES = 16                                  # multi-modal MPPI: largest n_modes
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -80,6 +81,7 @@ class MppibParams(C.Structure):
         ("n_elites", i32), ("n_keep", i32), ("elite_alpha", f32),
         ("du_min", f32 * MAX_NU), ("du_max", f32 * MAX_NU), ("smooth_weight", f32),
         ("n_worlds", i32), ("risk_tail", i32),
+        ("n_modes", i32), ("mode_margin", f32), ("mode_samples", i32),
     ]
 
 
@@ -462,6 +464,29 @@ def _risk_params(p: MppibParams, mppi_cfg, K_local: int) -> None:
     p.n_worlds, p.risk_tail = R, risk_tail(R, alpha)
 
 
+def _modes_params(p: MppibParams, mppi_cfg) -> None:
+    """The multi-modal MPPI keys (DESIGN.md section 2, "Multi-modal MPPI"): M = n_modes nominal sequences, each drawn around by its
+    block of Kc = K_total / M samples, and the switching margin; the refusals of the mode.  n_modes = 1 leaves the block as it was."""
+    M = int(getattr(mppi_cfg, "n_modes", 1))
+    margin = float(getattr(mppi_cfg, "mode_switch_margin", 0.0))
+    if not 1 <= M <= MAX_MODES:
+        raise ValueError(f"n_modes = {M} must lie in 1 .. {MAX_MODES}")
+    if not (math.isfinite(margin) and margin >= 0.0):
+        raise ValueError(f"mode_switch_margin = {margin} must be finite and >= 0")
+    if M == 1:
+        return
+    k_total = int(mppi_cfg.num_samples)
+    if k_total % M != 0 or k_total // M < 32:
+        raise ValueError(f"n_modes = {M} needs num_samples = {k_total} to be a multiple of it with at least 32 samples per mode")
+    if p.mode in (MODE_CEM, MODE_SMOOTH):
+        raise ValueError("n_modes > 1 excludes mppi_mode cem and smooth")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("n_modes > 1 excludes update_cov and update_lambda: the adapted distribution belongs to one mean")
+    if p.n_worlds > 1:
+        raise ValueError("n_modes > 1 excludes n_worlds > 1")
+    p.n_modes, p.mode_margin, p.mode_samples = M, margin, k_total // M
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -539,6 +564,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
         raise ValueError("too many observation items")
     p.k_offset = int(getattr(mppi_cfg, "_k_offset", 0))
     _risk_params(p, mppi_cfg, int(K_local))
+    _modes_params(p, mppi_cfg)
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

@@ -122,6 +122,21 @@ def shard_samples(k_total: int, rank: int, world: int, unit: int = 4):
     return unit * mine, unit * off
 
 
+def mode_starts(params, nu: int, U0, M: int, seed: int):
+    """(M - 1, T, nu) float32 starts of modes 1 .. M-1 of multi-modal MPPI: clamp(U0 + L0 z_m[t], u_min, u_max) with L0 the lower
+    Cholesky factor of noise_sigma (the parameter block's float32 copy) and z one (M - 1, T, nu) float64 standard-normal draw of
+    numpy.random.default_rng(seed), rounded to float32; the sums in float64, the result rounded once.  Identical modes would stay
+    identical under the coupling, so this start breaks the symmetry."""
+    import numpy as np
+    T = int(params.T)
+    z = np.random.default_rng(int(seed)).standard_normal((M - 1, T, nu)).astype(np.float32).astype(np.float64)
+    L0 = np.array(params.sigma_chol[:nu * nu], np.float32).astype(np.float64).reshape(nu, nu)
+    lo = np.array(params.u_min[:nu], np.float32).astype(np.float64)
+    hi = np.array(params.u_max[:nu], np.float32).astype(np.float64)
+    U = np.asarray(U0, np.float32).astype(np.float64).reshape(1, T, nu) + np.einsum("ji,mti->mtj", L0, z)
+    return np.clip(U, lo, hi).astype(np.float32)
+
+
 def _randomised(model) -> bool:
     """True when K2 draws something per rollout: a free body's mass, or a shape's friction or size."""
     return (any(model.free_mass_pct[f] != 0.0 for f in range(model.nfree))
@@ -180,6 +195,15 @@ class MPPIPlanner:
             if not _randomised(sim.scene.model):
                 raise ValueError("n_worlds > 1 needs a scene that randomises its rollouts (noise_percentage_mass, noise_percentage_friction "
                                  "or noise_sigma_size on some actor): without it the worlds would be identical copies")
+        # multi-modal MPPI (DESIGN.md section 2, "Multi-modal MPPI"): M nominal sequences side by side, each sampled by its block of
+        # K_total / M samples and coupled by a Stein-variational step on the device; the mode state (active mode, F[M], U_exec) is a device
+        # buffer K4 writes; make_params checks the keys against the mode
+        self.n_modes = int(getattr(cfg, "n_modes", 1))
+        if self.n_modes > 1:
+            if bool(getattr(cfg, "use_priors", False)) and prior is not None:
+                raise ValueError("n_modes > 1 does not take a prior: the prior row would belong to no mode")
+            if not hasattr(sim.backend, "set_distribution"):
+                raise ValueError(f"n_modes > 1 needs a backend with set_distribution ({type(sim.backend).__name__} has none)")
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))
@@ -266,12 +290,16 @@ class MPPIPlanner:
     def _alloc(self):
         dev, T, nu, K = self.device, self.T, self.nu, self.K
         f32 = dict(dtype=torch.float32, device=dev)
-        self.U = torch.zeros((T, nu), **f32)
+        M = self.n_modes
+        self.U = torch.zeros((T, nu), **f32) if M == 1 else torch.zeros((M, T, nu), **f32)
+        U0 = self.U if M == 1 else self.U[0]
         U_init = getattr(self.cfg, "U_init", None)
         if U_init is not None:
-            self.U.copy_(torch.as_tensor(U_init, dtype=torch.float32).reshape(T, nu))
+            U0.copy_(torch.as_tensor(U_init, dtype=torch.float32).reshape(T, nu))
         else:
-            self.U += torch.as_tensor(self.backend.params.u_init[:nu], dtype=torch.float32).to(dev)
+            U0 += torch.as_tensor(self.backend.params.u_init[:nu], dtype=torch.float32).to(dev)
+        if M > 1:
+            self.U[1:].copy_(torch.from_numpy(mode_starts(self.backend.params, nu, U0.cpu().numpy(), M, self.seed)))
         self.actions = torch.zeros((T, nu, K), **f32)       # [T][nu][K]
         self.noise = torch.zeros((T, nu, K), **f32)
         self.cost = torch.zeros((T, K), **f32)
@@ -283,6 +311,8 @@ class MPPIPlanner:
         if self.cem:
             E = int(self.backend.params.n_elites)
             P = (2 * E + E * T * nu + 3) & ~3                 # (S, index)[E] + actions[E][T*nu] of mppi_mode cem, padded to 4
+        if M > 1:
+            P = M * (2 + T * nu)                              # (beta_m, eta_m, W_m[T*nu]) of every mode
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
@@ -298,6 +328,7 @@ class MPPIPlanner:
         # adaptive MPPI: dist = (lambda, cov[nu]) from lambda_ and diag(noise_sigma), or with cov_type full (lambda, Sigma, L, Sigma^-1)
         # (horizon: the same of Sigma_H = I_T (x) Sigma, n = T*nu) computed in float64 and rounded; registered before the noise library is built (update_cov makes it white)
         self.dist = None
+        self.mode_state = None
         if self.cem:
             # the CEM state (carry offset, elites valid, S_elite[E], sigma[T][nu], elites[E][T][nu]): sigma starts at sqrt(diag(Sigma))
             E = int(self.backend.params.n_elites)
@@ -306,6 +337,10 @@ class MPPIPlanner:
             state[2 + E:2 + E + T * nu] = sigma0.repeat(T)
             self.dist = state.to(**f32)
             self.backend.set_distribution(self.dist)
+        elif M > 1:
+            # the mode state (active mode, F[M], U_exec[T][nu]): mode 0 executed, no free energy yet, U_exec = mode 0
+            self.mode_state = torch.cat([torch.zeros(1), torch.full((M,), float("inf")), U0.detach().cpu().reshape(-1)]).to(**f32)
+            self.backend.set_distribution(self.mode_state)
         elif not self.adaptive and hasattr(self.backend, "set_distribution"):
             self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
         if self.adaptive:
@@ -370,8 +405,26 @@ class MPPIPlanner:
     @property
     def mean_action(self):
         """(T, nu) device view of the nominal sequence U; with mppi_mode smooth that is the mean of the control DERIVATIVE (the
-        planned actions are ``action_sequence``)."""
+        planned actions are ``action_sequence``); with n_modes > 1 the sequence of the executed mode after the last plan."""
+        if self.mode_state is not None:
+            return self.mode_state[1 + self.n_modes:].view(self.T, self.nu)
         return self.U
+
+    @property
+    def modes(self):
+        """(M, T, nu) device view of the nominal sequences of multi-modal MPPI (None unless n_modes > 1)."""
+        return self.U if self.n_modes > 1 else None
+
+    @property
+    def mode_free_energy(self):
+        """(M,) device view of the free energies F_m = beta_m - lambda ln(eta_m / Kc) of the last plan (+inf where a mode had no valid
+        sample or before the first plan; None unless n_modes > 1)."""
+        return None if self.mode_state is None else self.mode_state[1:1 + self.n_modes]
+
+    @property
+    def active_mode(self):
+        """Index of the mode the last plan executed (an int, read from the device; None unless n_modes > 1)."""
+        return None if self.mode_state is None else int(self.mode_state[0].item())
 
     @property
     def action_sequence(self):
@@ -532,6 +585,7 @@ class MPPIPlanner:
             u_keep, ctr_keep = self.U.clone(), self.plan_ctr.clone()
             dist_keep = None if self.dist is None else self.dist.clone()      # the warm-up plans adapt the distribution too
             smooth_keep = None if self.smooth_state is None else self.smooth_state.clone()   # ... and move the smooth state
+            modes_keep = None if self.mode_state is None else self.mode_state.clone()       # ... and the mode state
             with torch.cuda.stream(side):
                 for _ in range(2):                       # warm-up outside capture (allocator, lazy init)
                     self._plan_batched()
@@ -546,6 +600,8 @@ class MPPIPlanner:
                 self.dist.copy_(dist_keep)
             if smooth_keep is not None:
                 self.smooth_state.copy_(smooth_keep)
+            if modes_keep is not None:
+                self.mode_state.copy_(modes_keep)
             self._graph = g
             self._graph_epoch = getattr(self.sim, "model_epoch", 0)
         except Exception as e:  # capture is an optimisation; the eager path is the same kernels
@@ -574,4 +630,4 @@ class MPPIPlanner:
         self._plans += 1
         if self.u_per_command == 1:
             return self._action
-        return self.U[: self.u_per_command]
+        return self.mean_action[: self.u_per_command]

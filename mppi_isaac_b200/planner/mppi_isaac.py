@@ -81,6 +81,8 @@ class MPPIisaacPlanner(object):
                 self.mppi.dist.copy_(old.dist)         # and so does the adapted (lambda, cov) of adaptive MPPI
             if old.smooth_state is not None and self.mppi.smooth_state is not None and old.smooth_state.shape == self.mppi.smooth_state.shape:
                 self.mppi.smooth_state.copy_(old.smooth_state)   # and the last executed action of mppi_mode smooth
+            if old.mode_state is not None and self.mppi.mode_state is not None and old.mode_state.shape == self.mppi.mode_state.shape:
+                self.mppi.mode_state.copy_(old.mode_state)       # and, with n_modes > 1, the executed mode and its free energies
 
     def _make_mppi(self):
         return MPPIPlanner(

@@ -47,6 +47,8 @@ class MPPIConfig:
     du_max: Optional[List[float]] = None
     n_worlds: int = 1                    # risk-aware MPPI (DESIGN.md section 2): R rollouts per control sample in R fixed worlds, 1 .. 32
     cvar_alpha: float = 1.0              # risk-aware MPPI: a control scores the mean of its ceil(alpha R) worst world costs, alpha in (0, 1]
+    n_modes: int = 1                     # multi-modal MPPI (DESIGN.md section 2): M nominal sequences planned side by side, 1 .. 16, K / M >= 32 samples each
+    mode_switch_margin: float = 0.0      # multi-modal MPPI: keep the executed mode while its free energy is within this margin (cost units) of the lowest
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0
