@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 20
+#define MPPIB_ABI_VERSION 21
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -96,6 +96,7 @@ extern "C" {
 #define MPPIB_CEM_MAX_ELITES 128
 #define MPPIB_MAX_WORLDS 32   /* risk-aware MPPI: largest n_worlds (a group of worlds never straddles a 32-sample tile) */
 #define MPPIB_MAX_MODES 16    /* multi-modal MPPI: largest n_modes */
+#define MPPIB_MAX_ANNEAL 16   /* annealed MPPI: largest number of MPPI iterations per plan */
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -466,6 +467,26 @@ int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  *          from mode p, and the state receives (p, F, U_p).
  *   shift  every mode as U is shifted today.
  * Reduce and finalize refuse M > 1 while no mode state is registered.                                                             */
+
+/* Annealed MPPI (N MPPI iterations per plan with a noise schedule over iterations and horizon; modes SIMPLE and MEAN with the fixed
+ * Sigma, Gaussian or colored K1, any n_worlds; no update_cov / update_lambda, cem, smooth, n_modes > 1 or Halton library).  The schedule
+ * is a device buffer registered with mppib_set_anneal (caller-owned, initialised by the caller; N = n_iterations in 1 .. MPPIB_MAX_ANNEAL):
+ *   state    [1 + 2*N*T]  (iteration counter as a float, s[N][T], r[N][T]); the host fills s[i][t] = c_i^i c_h^(T-1-t) and
+ *                         r[i][t] = 1 / s[i][t]^2, both from float64 rounded once; iteration i reads row min(counter, N - 1)
+ * One plan is mppib_shift, then N times K1 -> K2 -> cost -> K3 -> (exchange) -> K4; nothing on the host changes between iterations but
+ * plan_idx = i << 32, so a batched plan is one CUDA graph.
+ *   K1     mppib_sample and mppib_sample_colored (fixed Sigma, with their n_worlds keying): the draw and colour of today's K1, then
+ *          noise_j = s[i][t] (L z)_j with one float32 multiplication, a = clamp(U + noise) with the null / prior rows, noise := a - U
+ *   K3     SIMPLE mode: g_r = (lambda (Sigma^-1 U)_r) r[i][t], the importance-sampling term under N(U, s^2 Sigma), one multiplication
+ *          after the lambda product; MEAN mode is unchanged (only its samples are annealed).  Every RPL / RISK instantiation, split or fused.
+ *   K4     today's update (Savitzky-Golay, clamp, action, mirror, stats), then counter := counter + 1 (split and fused tail); the action and
+ *          stats of a plan are those of its last iteration
+ *   shift  as today, then counter := 0
+ * With s = 1 every added operation multiplies by 1.0f: a registered schedule of ones with N = 1 reproduces the plain plan bit for bit.
+ * Registration refuses N outside 1 .. MPPIB_MAX_ANNEAL and the excluded modes; the library records T there and refuses every launch once
+ * mppib_set_params has changed T (or switched to an excluded mode) without a new registration.  mppib_sample_library, mppib_noise_library,
+ * mppib_sample_smooth and the cem path refuse a registered schedule.  NULL switches it off: every launch is then today's.             */
+int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations);
 
 #ifdef __cplusplus
 }

@@ -24,7 +24,7 @@ SYMBOLS = [
     "mppib_set_model", "mppib_state_size", "mppib_obs_size", "mppib_sample", "mppib_rollout",
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
-    "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth",
+    "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth", "mppib_set_anneal",
 ]
 
 
@@ -79,6 +79,11 @@ def smooth_state_floats(T, nu):
     return int(nu) + int(T) * int(nu)
 
 
+def anneal_state_floats(T, n_iterations):
+    """Floats of the schedule of annealed MPPI: (counter, s[N][T], r[N][T])."""
+    return 1 + 2 * int(n_iterations) * int(T)
+
+
 def cem_row_floats(T, nu, E):
     """Floats of one shard row of mppi_mode cem: (S, index bits)[E], actions[E][T*nu], padded to a multiple of 4."""
     return (2 * int(E) + int(E) * int(T) * int(nu) + 3) & ~3
@@ -113,6 +118,7 @@ class CudaBackend:
         self._mirror_keepalive = None
         self._dist_keepalive = None
         self._smooth_keepalive = None
+        self._anneal_keepalive = None     # (state, N)
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -132,6 +138,10 @@ class CudaBackend:
             self.set_distribution(self._dist_keepalive)
         if self._smooth_keepalive is not None:           # ... and the planner's smooth state
             self.set_smooth_state(self._smooth_keepalive)
+        if self._anneal_keepalive is not None:           # ... and its annealing schedule, while it still fits the horizon (a planner
+            state, n = self._anneal_keepalive            # rebuilt for another horizon or mode registers its own)
+            if not (state.numel() == anneal_state_floats(params.T, n) and self.lib.mppib_set_anneal(self.handle, _ptr(state), C.c_int32(n)) == 0):
+                self._anneal_keepalive = None
 
     def destroy(self):
         if self.handle:
@@ -297,6 +307,17 @@ class CudaBackend:
                 raise RuntimeError(f"mppib_set_smooth_state: (a_prev[nu], A[T][nu]) = nu + T*nu = {need} floats, got {state.numel()}")
         self._smooth_keepalive = state
         self._check(self.lib.mppib_set_smooth_state(self.handle, _ptr(state)), "mppib_set_smooth_state")
+
+    def set_anneal(self, state, n_iterations=0):
+        """Annealed MPPI: register the device tensor (counter, s[N][T], r[N][T]) of N = n_iterations MPPI iterations per plan that K1 / K3
+        read, K4 advances and the shift resets (None switches it off).  The library records T and refuses launches once it changes."""
+        if state is not None:
+            need = anneal_state_floats(self.params.T, n_iterations)
+            if state.numel() != need or state.dtype != torch.float32 or not state.is_contiguous():
+                raise RuntimeError(f"mppib_set_anneal: (counter, s[N][T], r[N][T]) = 1 + 2*N*T = {need} contiguous float32 values, got "
+                                   f"{state.dtype} {state.numel()}")
+        self._check(self.lib.mppib_set_anneal(self.handle, _ptr(state), C.c_int32(0 if state is None else int(n_iterations))), "mppib_set_anneal")
+        self._anneal_keepalive = None if state is None else (state, int(n_iterations))
 
     def reduce(self, cost, x, U, partial):
         self._check_row(partial, "mppib_reduce")

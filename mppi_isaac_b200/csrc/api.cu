@@ -116,6 +116,22 @@ static int alloc_scratch(MppibContext* c) {
     return 0;
 }
 
+// Annealed MPPI: what a parameter block must leave out while a schedule is registered (checked at registration and at every launch,
+// so that a later mppib_set_params cannot slip past it)
+static int anneal_excludes(const MppibParams& p, const char* who) {
+    MPPIB_REQUIRE(p.mode == MPPIB_MODE_SIMPLE || p.mode == MPPIB_MODE_MEAN, "%s: annealed MPPI excludes mode cem (it has its own sigma) and mode smooth", who);
+    MPPIB_REQUIRE(!p.update_cov && !p.update_lambda, "%s: annealed MPPI excludes update_cov and update_lambda", who);
+    MPPIB_REQUIRE(p.n_modes <= 1, "%s: annealed MPPI excludes n_modes > 1 (the Stein coupling's Sigma^-1 metric would need the schedule)", who);
+    return 0;
+}
+
+int check_anneal(const MppibContext* c, const char* who) {
+    if (!c->anneal) return 0;
+    MPPIB_REQUIRE(c->params.T == c->anneal_T, "%s: the annealing schedule was registered for T = %d, the parameter block has T = %d; register a schedule "
+                  "for the new horizon (mppib_set_anneal)", who, c->anneal_T, c->params.T);
+    return anneal_excludes(c->params, who);
+}
+
 extern "C" {
 
 int32_t mppib_abi_version(void) { return MPPIB_ABI_VERSION; }
@@ -251,6 +267,7 @@ int32_t mppib_obs_size(MppibHandle h) { return h ? h->obs_rows : -1; }
 int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total, const float* U,
                      const float* prior_row, float* actions, float* noise, void* stream) {
     MPPIB_REQUIRE(h && U && actions, "mppib_sample: null argument");
+    if (int rc = check_anneal(h, "mppib_sample")) return rc;
     MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
     MPPIB_ON_DEVICE(h);
     return launch_sample(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, actions, noise, (cudaStream_t)stream);
@@ -259,6 +276,7 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
 int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                              const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, void* stream) {
     MPPIB_REQUIRE(h && U && Lt && actions, "mppib_sample_colored: null argument");
+    if (int rc = check_anneal(h, "mppib_sample_colored")) return rc;
     MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_colored: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
     MPPIB_ON_DEVICE(h);
     return launch_sample_colored(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, (cudaStream_t)stream);
@@ -299,6 +317,7 @@ int32_t mppib_rollout(MppibHandle h, const float* state0, const float* root0, fl
 
 int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const float* U, float* partial, void* stream) {
     MPPIB_REQUIRE(h && cost && x && U && partial, "mppib_reduce: null argument");
+    if (int rc = check_anneal(h, "mppib_reduce")) return rc;
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
     if (cem_mode(h)) return launch_elite(h, cost, x, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
@@ -307,6 +326,7 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
 
 int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, float* U, float* partial, float* action_out, float* stats, void* stream) {
     MPPIB_REQUIRE(h && cost && x && U && partial && action_out, "mppib_reduce_finalize: null argument");
+    if (int rc = check_anneal(h, "mppib_reduce_finalize")) return rc;
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
     if (cem_mode(h)) return launch_elite(h, cost, x, partial, U, action_out, stats, (cudaStream_t)stream);
@@ -315,6 +335,7 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
 
 int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U, float* action_out, float* stats, void* stream) {
     MPPIB_REQUIRE(h && U && action_out && G >= 1, "mppib_finalize: bad argument");
+    if (int rc = check_anneal(h, "mppib_finalize")) return rc;
     if (!partials) {
         MPPIB_REQUIRE(h->peer_world >= 2 && G == h->peer_world, "mppib_finalize: partials == NULL needs an open peer window and G == world (G=%d, world=%d)", G, h->peer_world);
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
@@ -363,8 +384,22 @@ int32_t mppib_set_smooth_state(MppibHandle h, float* state) {
     return 0;
 }
 
+int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    if (state == nullptr) {
+        h->anneal = nullptr; h->anneal_n = 0; h->anneal_T = 0;
+        return 0;
+    }
+    MPPIB_REQUIRE(n_iterations >= 1 && n_iterations <= MPPIB_MAX_ANNEAL, "mppib_set_anneal: n_iterations = %d out of range [1, %d]", n_iterations,
+                  MPPIB_MAX_ANNEAL);
+    if (int rc = anneal_excludes(h->params, "mppib_set_anneal")) return rc;
+    h->anneal = state; h->anneal_n = n_iterations; h->anneal_T = h->params.T;
+    return 0;
+}
+
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream) {
     MPPIB_REQUIRE(h && U, "mppib_shift: null argument");
+    if (int rc = check_anneal(h, "mppib_shift")) return rc;
     MPPIB_ON_DEVICE(h);
     if (cem_mode(h)) return launch_cem_shift(h, U, plan_ctr, (cudaStream_t)stream);
     return launch_shift(h, U, plan_ctr, (cudaStream_t)stream);

@@ -48,6 +48,8 @@ struct MppibContext {
     float* dist;                               // adaptive MPPI: device (lambda, cov[nu]) or, with cov_full, (lambda, Sigma, L, Sigma^-1)
                                                // read by K1 / K3, updated by K4 (nullable)
     float* smooth;                             // MODE_SMOOTH: device (a_prev[nu], A[T][nu]), read by K1, updated by K4 (nullable)
+    float* anneal;                             // annealed MPPI: device (counter, s[N][T], r[N][T]), read by K1 / K3, counter set by K4 / shift (nullable)
+    int anneal_n, anneal_T;                    // N iterations and the horizon T the schedule was registered for
     // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
     float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
     float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
@@ -105,7 +107,15 @@ static inline bool smooth_mode(const MppibContext* c) { return c->params.mode ==
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
 static inline bool adaptive_horizon(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_horizon; }
-#define MPPIB_HZ_MAX_N 256                     // cov_horizon: largest n = T*nu (the packed n x n triangle K4 factors in shared memory)
+// Annealed MPPI: the row of the registered schedule a (counter, s[N][T], r[N][T]) that iteration min(counter, N - 1) reads -- the noise
+// scale s (recip = false) or r = 1 / s^2 (recip = true).  The counter is a float that K4 advances and the shift resets.
+__device__ __forceinline__ const float* anneal_row(const float* __restrict__ a, int n, int T, bool recip) {
+    const int i = min(max((int)a[0], 0), n - 1);
+    return a + 1 + (size_t)((recip ? n : 0) + i) * T;
+}
+// the launch-time refusals of a registered schedule (api.cu)
+int check_anneal(const MppibContext* c, const char* who);
+#define MPPIB_HZ_MAX_N 256                    // cov_horizon: largest n = T*nu (the packed n x n triangle K4 factors in shared memory)
 #define HZ_TILE 64                             // SYRK output tile
 #define HZ_MAX_TILES 10                        // lower-triangle tiles of a 256 x 256 C
 

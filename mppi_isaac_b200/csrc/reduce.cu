@@ -643,7 +643,7 @@ template <bool ADAPT, bool FULL = false, bool SMOOTH = false>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
-                                                float* __restrict__ dist, float* __restrict__ smooth = nullptr) {
+                                                float* __restrict__ dist, float* __restrict__ smooth = nullptr, float* __restrict__ anneal = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = (int)gridDim.x;
     float* sc = tiles;                   // [MAX_GRID] scale of every CTA partial (the ring is idle now)
@@ -718,6 +718,7 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             __syncthreads();
             if constexpr (SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
             else finalize_rows<ADAPT, FULL>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            if (tid == 0 && anneal) anneal[0] += 1.0f;                        // annealed MPPI: the next iteration's row (every CTA read it)
         }
     }
 }
@@ -786,13 +787,15 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // MODES (n_modes = M > 1): the grid is (gx, M) and CTA (x, m) walks only the tiles that hold samples of mode m, with g = lambda Sigma^-1
 // U_m; the lanes of a straddling tile that belong to the other mode are masked (weight 0, not in the minimum).  Its partial is scratch
 // row m*gx + x, and the last CTA folds every mode into block m of the row [M][2 + T*nu] (fold_modes_and_finish).
+// anneal (annealed MPPI, nullable): the registered schedule of anneal_n iterations; SIMPLE mode scales g_r by r[t] = 1 / s[t]^2 of the
+// iteration's row after the lambda product (a schedule of ones changes no bit), and the fused K4 advances the counter.
 template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false, bool MODES = false>   // rows of W per lane: T*nu <= 32 * RPL
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                        float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
-                       const float* __restrict__ hz_g, float* __restrict__ smooth) {
+                       const float* __restrict__ hz_g, float* __restrict__ smooth, float* __restrict__ anneal, int anneal_n) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -842,6 +845,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         for (int i = 0; i < nstage && i < my_tiles; ++i) issue_tile(i);   // the first ring fill is in flight while the prologue below runs
     }
+    const float* rrow = anneal ? anneal_row(anneal, anneal_n, T, true) : nullptr;
     for (int r = tid; r < NR4; r += NT) {
         float acc = 0.f;
         if (HZN && simple && r < NR) {
@@ -855,6 +859,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             else
                 for (int j = 0; j < nu; ++j) acc += p.sigma_inv[i * nu + j] * U[t * nu + j];
             acc *= lam;
+            if (rrow) acc = __fmul_rn(acc, rrow[t]);                          // annealed MPPI: importance term under N(U, s^2 Sigma)
         }
         if (FULL && !simple && r < NR) acc = U[r];                            // phase A reads g in SIMPLE mode only
         g[r] = acc;
@@ -1057,17 +1062,19 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         return;
     }
     fold_and_finish<ADAPT, FULL, SMOOTH>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist,
-                                         smooth);
+                                         smooth, anneal);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
 // distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon); SMOOTH: smooth_rows;
-// MODES: modes_rows (n_modes > 1, dist = the mode state).
+// MODES: modes_rows (n_modes > 1, dist = the mode state).  anneal (annealed MPPI, nullable): the counter of the registered schedule is
+// advanced by one after the update.
 template <bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool MODES = false>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
-                float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth) {
+                float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth,
+                float* __restrict__ anneal) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const int T = p.T, NR = T * nu;
     int P = MODES ? p.n_modes * (2 + NR) : HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
@@ -1100,6 +1107,7 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
     else if constexpr (SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
     else finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
     if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
+    if (threadIdx.x == 0 && anneal) anneal[0] += 1.0f;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1233,15 +1241,17 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
 }
 
 // hz_g (cov_horizon with a registered distribution, SIMPLE mode): g = lambda Sigma_H^-1 U of the shifted U, once per plan, for K3's
-// control cost (a row of Sigma_H^-1 per thread, summed in column order).
+// control cost (a row of Sigma_H^-1 per thread, summed in column order).  anneal (annealed MPPI, nullable): the plan starts at
+// iteration 0, so the counter of the registered schedule is reset.
 __global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu, float* __restrict__ U, uint32_t* __restrict__ plan_ctr,
-                                   const float* __restrict__ dist, float* __restrict__ hz_g) {
+                                   const float* __restrict__ dist, float* __restrict__ hz_g, float* __restrict__ anneal) {
     extern __shared__ float tmp[];
     const int NR = p.T * nu;
     for (int r = threadIdx.x; r < NR; r += blockDim.x) tmp[r] = r + nu < NR ? U[r + nu] : p.u_init[r % nu];
     __syncthreads();
     for (int r = threadIdx.x; r < NR; r += blockDim.x) U[r] = tmp[r];
     if (threadIdx.x == 0 && plan_ctr) *plan_ctr += 1u;
+    if (threadIdx.x == 0 && anneal) anneal[0] = 0.f;
     if (hz_g != nullptr) {
         const float lam = dist[0];
         const float* sinv = dist + 1 + 2 * (size_t)NR * NR;
@@ -1361,7 +1371,8 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK, MODES><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
                                                                             c->reduce_scratch, c->reduce_ticket, partial, peers, fin_U, fin_action,
                                                                             fin_stats, fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g,
-                                                                            SMOOTH ? c->smooth : nullptr);
+                                                                            SMOOTH ? c->smooth : nullptr, MODES || HZN || SMOOTH ? nullptr : c->anneal,
+                                                                            c->anneal_n);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1510,11 +1521,11 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
             attr = smem;
         }
         mppib_finalize_kernel<false, false, false, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                                   c->action_mirror, c->dist, nullptr, nullptr);
+                                                                                   c->action_mirror, c->dist, nullptr, nullptr, nullptr);
     } else if (smooth_mode(c)) {
         MPPIB_REQUIRE(c->smooth != nullptr, "mppib_finalize: mode smooth needs its state registered with mppib_set_smooth_state");
         mppib_finalize_kernel<false, false, false, true><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats,
-                                                                                                peer_args(c), c->action_mirror, nullptr, nullptr, c->smooth);
+                                                                                                peer_args(c), c->action_mirror, nullptr, nullptr, c->smooth, nullptr);
     } else if (adaptive_horizon(c)) {
         MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N && c->hz_sig != nullptr && c->hz_n == NR, "mppib_finalize: cov_horizon buffers are not sized for n = %d", NR);
         const int smem = hz_fin_smem(NR, G);
@@ -1526,18 +1537,18 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
             attr = smem;
         }
         mppib_finalize_kernel<true, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror,
-                                                                      c->dist, c->hz_sig, nullptr);
+                                                                      c->dist, c->hz_sig, nullptr, nullptr);
     } else if (adaptive_full(c)) {
         const size_t smem = (NR + G + full_fin_floats(c->params.T, c->model.nu)) * sizeof(float);
         mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                               nullptr, nullptr);
+                                                               nullptr, nullptr, c->anneal);
     } else if (c->dist) {
         const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
         mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                         nullptr, nullptr);
+                                                         nullptr, nullptr, c->anneal);
     } else {
         mppib_finalize_kernel<false><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                              c->action_mirror, nullptr, nullptr, nullptr);
+                                                                              c->action_mirror, nullptr, nullptr, nullptr, c->anneal);
     }
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -1551,7 +1562,7 @@ int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) 
         return 0;
     }
     float* hz_g = adaptive_horizon(c) && c->params.mode == MPPIB_MODE_SIMPLE ? c->hz_g : nullptr;
-    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g);
+    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g, c->anneal);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

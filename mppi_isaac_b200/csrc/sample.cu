@@ -35,11 +35,13 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
 // The control-space colour, clamp and store of one (t, k) of every Philox K1: noise_j = sum_{i <= j} L0[j][i] z_i with the fixed
 // Sigma's Cholesky factor, summed from i = 0 upwards; DIAG (adaptive MPPI with update_cov): sqrt(cov_j) z_j with cov = dist[1..nu],
 // the live diagonal covariance; FULL (update_cov with cov_full): the live lower Cholesky factor L = dist[1 + nu*nu ..] in the same
-// order.  a = clamp(U + noise) with the null / prior rows, noise := a - U.
+// order.  a = clamp(U + noise) with the null / prior rows, noise := a - U.  Annealed MPPI (srow = the s row of the iteration, fixed Sigma
+// only): noise_j := s[t] noise_j, one rounded multiplication, so a schedule of ones changes no bit.
 template <bool DIAG, bool FULL>
 __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int t, int k, bool is_null,
                                                    bool is_prior, const float* __restrict__ U, const float* __restrict__ prior_row,
-                                                   float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
+                                                   float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist,
+                                                   const float* __restrict__ srow = nullptr) {
     const int K = p.K;
 #pragma unroll
     for (int j = 0; j < MPPIB_MAX_NU; ++j) {
@@ -56,6 +58,7 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
 #pragma unroll
             for (int i = 0; i < MPPIB_MAX_NU; ++i)
                 if (i <= j) n += p.sigma_chol[j * nu + i] * z[i];
+            if (srow) n = __fmul_rn(srow[t], n);
         }
         const float u = U[t * nu + j];
         float a = u + n;
@@ -71,12 +74,13 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
 // DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block); with
 // n_worlds = R > 1 the control sample kg / R replaces the global sample in the counter and in the null / prior tests.  With n_modes > 1
 // the sample is drawn around its mode's sequence (sample_mode), the counter stays the global sample; n_modes > 1 excludes update_cov,
-// so only the fixed-Sigma instantiations (not DIAG / FULL) carry the mode offset.
+// so only the fixed-Sigma instantiations (not DIAG / FULL) carry the mode offset.  anneal (annealed MPPI, fixed Sigma only; nullable): the
+// registered schedule of anneal_n iterations, whose s row scales the noise.
 template <bool DIAG, bool FULL = false>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
               const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
-              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist) {
+              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist, const float* __restrict__ anneal, int anneal_n) {
     const int K = p.K;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int t = blockIdx.y;
@@ -97,7 +101,8 @@ mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0
     const bool is_prior = prior_row != nullptr && kc + 1 == kc_last;
     const float* Um = U;
     if constexpr (!DIAG && !FULL) Um += (size_t)sample_mode(k_offset + (uint32_t)k, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
-    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
+    const float* srow = (!DIAG && !FULL && anneal) ? anneal_row(anneal, anneal_n, p.T, false) : nullptr;
+    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
 }
 
 // The white Philox draws of a tile of S samples [k0, k0 + S) to shared memory, zs[(t*nu + i) * S + sample]: the draws of the
@@ -161,12 +166,14 @@ constexpr int CL_S = 32;            // samples per CTA
 constexpr int CL_MAX_T = 256;
 constexpr int CL_MAX_N = 512;       // T*nu: the tile's draws take CL_MAX_N * CL_S * 4 = 64 KB of shared memory
 
+// The fixed-Sigma instantiation asks for 8 CTAs per SM: with the annealing scale it takes 64 registers (78 unbounded, 63 without the
+// scale) and spills nothing; 0 leaves the other instantiations as the compiler allocates them.
 template <bool DIAG, bool FULL, bool CEM = false>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(128, (DIAG || FULL || CEM) ? 0 : 8)
 mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
                             const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
                             const float* __restrict__ prior_row, const float* __restrict__ Lt, float* __restrict__ actions,
-                            float* __restrict__ noise, const float* __restrict__ dist) {
+                            float* __restrict__ noise, const float* __restrict__ dist, const float* __restrict__ anneal, int anneal_n) {
     extern __shared__ __align__(16) float cs[];
     const int K = p.K, T = p.T;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -179,6 +186,7 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
     const float* Um = U;
     if constexpr (!DIAG && !FULL && !CEM) Um += (size_t)sample_mode(kg, p) * (T * nu);   // n_modes > 1 (fixed Sigma only)
+    const float* srow = (!DIAG && !FULL && !CEM && anneal) ? anneal_row(anneal, anneal_n, T, false) : nullptr;   // annealed MPPI
     const float* zl = cs + lane;
     for (int tl = warp; tl < (T + 1) / 2; tl += 4) {
         const int th = T - 1 - tl;                                            // th >= tl; th == tl for the middle row of an odd T
@@ -213,8 +221,8 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             cem_clamp_store(p, nu, wl, tl, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
             if (th != tl) cem_clamp_store(p, nu, wh, th, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
         } else {
-            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
-            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, Um, prior_row, actions, noise, dist);
+            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
+            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
         }
     }
 }
@@ -232,7 +240,8 @@ int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
     }
     mppib_sample_colored_kernel<DIAG, FULL, CEM><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
                                                                                           plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
-                                                                                          DIAG || FULL || CEM ? c->dist : nullptr);
+                                                                                          DIAG || FULL || CEM ? c->dist : nullptr,
+                                                                                          DIAG || FULL || CEM ? nullptr : c->anneal, c->anneal_n);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -497,6 +506,8 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
                          float* Z, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_noise_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_noise_library: mode smooth samples through mppib_sample_smooth");
+    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_noise_library: annealed MPPI excludes the noise library (every iteration would reuse the same directions); "
+                  "register no schedule (mppib_set_anneal(h, NULL, 0))");
     if (int rc = check_risk_shard(c, "mppib_noise_library", k_offset, k_total)) return rc;
     MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
@@ -512,6 +523,8 @@ int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, 
                           float* actions, float* noise, cudaStream_t s) {
     MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
     MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_library: mode smooth samples through mppib_sample_smooth");
+    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_sample_library: annealed MPPI excludes the noise library (every iteration would reuse the same directions); "
+                  "register no schedule (mppib_set_anneal(h, NULL, 0))");
     if (int rc = check_risk_shard(c, "mppib_sample_library", k_offset, k_total)) return rc;
     if (int rc = check_modes_total(c, "mppib_sample_library", k_total)) return rc;
     const int K = c->params.K, T = c->params.T;
@@ -540,13 +553,13 @@ int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint3
         return launch_sample_horizon_t<false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, nullptr, actions, noise, s);
     if (adaptive_full(c))
         mppib_sample_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset,
-                                                                k_total, U, prior_row, actions, noise, c->dist);
+                                                                k_total, U, prior_row, actions, noise, c->dist, nullptr, 0);
     else if (adaptive_cov(c))
         mppib_sample_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
-                                                         prior_row, actions, noise, c->dist);
+                                                         prior_row, actions, noise, c->dist, nullptr, 0);
     else
         mppib_sample_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
-                                                          prior_row, actions, noise, nullptr);
+                                                          prior_row, actions, noise, nullptr, c->anneal, c->anneal_n);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -574,6 +587,7 @@ int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, cons
     const int K = c->params.K, T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(smooth_mode(c), "mppib_sample_smooth: needs mode smooth (MPPIB_MODE_SMOOTH), the handle has mode %d", c->params.mode);
     MPPIB_REQUIRE(c->smooth != nullptr, "mppib_sample_smooth: no smooth state registered (mppib_set_smooth_state)");
+    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_sample_smooth: annealed MPPI excludes mode smooth");
     MPPIB_REQUIRE(T * nu <= SM_MAX_N, "mppib_sample_smooth: needs T*nu <= %d, got %d", SM_MAX_N, T * nu);
     const int smem = (int)sizeof(float) * T * nu * SM_S;
     static int smem_attr[64] = {0};

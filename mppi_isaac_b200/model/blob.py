@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 20
+ABI_VERSION = 21
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -32,6 +32,8 @@ MODE_SIMPLE, MODE_MEAN, MODE_CEM, MODE_SMOOTH = 0, 1, 2, 3
 CEM_MAX_ELITES = 128
 MAX_WORLDS = 32                                 # risk-aware MPPI: largest n_worlds
 MAX_MODES = 16                                  # multi-modal MPPI: largest n_modes
+MAX_ANNEAL = 16                                 # annealed MPPI: largest anneal_iterations
+ANNEAL_MIN_SCALE = 2.0 ** -20                   # annealed MPPI: smallest noise scale, so that r = 1 / s^2 stays finite in float32
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -487,6 +489,55 @@ def _modes_params(p: MppibParams, mppi_cfg) -> None:
     p.n_modes, p.mode_margin, p.mode_samples = M, margin, k_total // M
 
 
+def anneal_schedule(n_iterations: int, iter_decay: float, horizon_decay: float, T: int):
+    """(s, r) float64 (N, T) arrays of annealed MPPI (DESIGN.md section 2, "Annealed MPPI"): s[i][t] = c_i^i c_h^(T-1-t), r = 1 / s^2.
+    The caller rounds each once to float32."""
+    i = np.arange(int(n_iterations), dtype=np.float64)[:, None]
+    t = np.arange(int(T), dtype=np.float64)[None, :]
+    s = float(iter_decay) ** i * float(horizon_decay) ** (int(T) - 1 - t)
+    return s, 1.0 / (s * s)
+
+
+def anneal_config(mppi_cfg):
+    """(N, c_i, c_h) of the annealed-MPPI keys, defaults (1, 1.0, 1.0): one MPPI iteration at unit noise, today's planner."""
+    return (int(getattr(mppi_cfg, "anneal_iterations", 1)), float(getattr(mppi_cfg, "anneal_iter_decay", 1.0)),
+            float(getattr(mppi_cfg, "anneal_horizon_decay", 1.0)))
+
+
+def anneal_on(mppi_cfg) -> bool:
+    """True when the annealed-MPPI keys ask for more than today's planner: N > 1 or a decay below 1."""
+    n, ci, ch = anneal_config(mppi_cfg)
+    return n > 1 or ci < 1.0 or ch < 1.0
+
+
+def _anneal_params(p: MppibParams, mppi_cfg) -> None:
+    """The refusals of annealed MPPI (DESIGN.md section 2, "Annealed MPPI").  The schedule itself is a device buffer the planner registers
+    (mppib_set_anneal), so the parameter block does not change."""
+    n, ci, ch = anneal_config(mppi_cfg)
+    if not 1 <= n <= MAX_ANNEAL:
+        raise ValueError(f"anneal_iterations = {n} must lie in 1 .. {MAX_ANNEAL}")
+    for name, c in (("anneal_iter_decay", ci), ("anneal_horizon_decay", ch)):
+        if not (math.isfinite(c) and 0.0 < c <= 1.0):
+            raise ValueError(f"{name} = {c} must lie in (0, 1]")
+    if not anneal_on(mppi_cfg):
+        return
+    s, _ = anneal_schedule(n, ci, ch, p.T)
+    if s.min() < ANNEAL_MIN_SCALE:
+        raise ValueError(f"annealed MPPI: the smallest noise scale c_i^(N-1) c_h^(T-1) = {s.min():.3g} is below 2^-20 (anneal_iterations = {n}, "
+                         f"anneal_iter_decay = {ci}, anneal_horizon_decay = {ch}, horizon = {p.T})")
+    if p.mode == MODE_CEM:
+        raise ValueError("annealed MPPI excludes mppi_mode cem, which has its own sigma")
+    if p.mode == MODE_SMOOTH:
+        raise ValueError("annealed MPPI excludes mppi_mode smooth")
+    if str(getattr(mppi_cfg, "sampling_method", "halton")) == "halton":
+        raise ValueError("annealed MPPI excludes sampling_method halton: the library is drawn once, so every iteration would reuse the same "
+                         "directions; use random or colored")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("annealed MPPI excludes update_cov and update_lambda (and so every cov_type)")
+    if p.n_modes > 1:
+        raise ValueError("annealed MPPI excludes n_modes > 1: the Stein coupling's Sigma^-1 metric would need the schedule")
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -565,6 +616,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     p.k_offset = int(getattr(mppi_cfg, "_k_offset", 0))
     _risk_params(p, mppi_cfg, int(K_local))
     _modes_params(p, mppi_cfg)
+    _anneal_params(p, mppi_cfg)
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

@@ -26,7 +26,7 @@ import os
 
 import torch
 
-from ..model.blob import MODE_SIMPLE, MODE_SMOOTH
+from ..model.blob import ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule
 
 
 class _NoRange:
@@ -178,6 +178,12 @@ class MPPIPlanner:
         # both on the device; make_params checks the keys and refuses the combinations the mode excludes
         self.cem = str(getattr(cfg, "mppi_mode", "")) == "cem"
         self.cem_iterations = int(getattr(cfg, "cem_iterations", 3)) if self.cem else 1
+        # annealed MPPI (DESIGN.md section 2, "Annealed MPPI"): N MPPI iterations per plan, the noise of iteration i at step t scaled by
+        # s[i][t] = c_i^i c_h^(T-1-t); the schedule is a device buffer K1 / K3 read and K4 / the shift count through.  make_params checks
+        # the keys and refuses the combinations the mode excludes; with the defaults nothing is registered and every launch is today's.
+        self.annealed = anneal_on(cfg)
+        self.anneal_iterations = anneal_config(cfg)[0] if self.annealed else 1
+        self.iterations = self.cem_iterations if self.cem else self.anneal_iterations
         # Smooth MPPI (DESIGN.md section 2, "Smooth MPPI"): U is the control derivative; K1 integrates it from the last executed action
         # (the smooth state, a device buffer K4 updates), so the executed command changes by at most du_max * dt per plan
         self.smooth = str(getattr(cfg, "mppi_mode", "")) == "smooth"
@@ -224,6 +230,8 @@ class MPPIPlanner:
             raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
         if self.cem and not hasattr(self.backend, "set_distribution"):
             raise ValueError(f"mppi_mode: cem needs a backend with set_distribution ({type(self.backend).__name__} has none)")
+        if self.annealed and not hasattr(self.backend, "set_anneal"):
+            raise ValueError(f"annealed MPPI needs a backend with set_anneal ({type(self.backend).__name__} has none)")
         if self.smooth and not hasattr(self.backend, "set_smooth_state"):
             raise ValueError(f"mppi_mode: smooth needs a backend with set_smooth_state ({type(self.backend).__name__} has none)")
         self._peer_exchange = False
@@ -363,6 +371,17 @@ class MPPIPlanner:
             self.backend.set_smooth_state(self.smooth_state)
         elif hasattr(self.backend, "set_smooth_state"):
             self.backend.set_smooth_state(None)          # a rebuilt planner in another mode must not keep the previous one's state
+        # annealed MPPI: the schedule (counter, s[N][T], r[N][T]) from float64, each rounded once; a planner rebuilt with the keys at their
+        # defaults registers none, as set_distribution(None) above
+        self.anneal_state = None
+        if self.annealed:
+            N, ci, ch = anneal_config(self.cfg)
+            s, r = anneal_schedule(N, ci, ch, T)
+            self.anneal_state = torch.cat([torch.zeros(1), torch.from_numpy(s.astype("float32")).reshape(-1),
+                                           torch.from_numpy(r.astype("float32")).reshape(-1)]).to(**f32)
+            self.backend.set_anneal(self.anneal_state, N)
+        elif hasattr(self.backend, "set_anneal"):
+            self.backend.set_anneal(None)
         self._graph = None
         self._graph_failed = False
         self._graph_epoch = -1
@@ -390,7 +409,8 @@ class MPPIPlanner:
 
     def _sample(self, iteration=0):
         be = self.backend
-        if self.cem:                                     # iteration i keys Philox with plan_idx = i << 32: iteration 0 draws what colored MPPI draws
+        # iteration i of a plan (cem, or annealed MPPI) keys Philox with plan_idx = i << 32: iteration 0 draws what a one-iteration plan draws
+        if self.cem:
             be.sample_colored(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise,
                               self.plan_ctr)
         elif self.smooth:
@@ -398,9 +418,33 @@ class MPPIPlanner:
         elif self.use_library:
             be.sample_library(self.k_offset, self.K_total, self.U, None, self.Z, self.actions, self.noise)
         elif self.use_colored:
-            be.sample_colored(self.seed, 0, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise, self.plan_ctr)
+            be.sample_colored(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise,
+                              self.plan_ctr)
         else:
-            be.sample(self.seed, 0, self.k_offset, self.K_total, self.U, None, self.actions, self.noise, self.plan_ctr)
+            be.sample(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self.actions, self.noise, self.plan_ctr)
+
+    @property
+    def noise_schedule(self):
+        """(N, T) device view of the noise scales s[i][t] of annealed MPPI (None with the feature off); ``set_noise_schedule`` replaces it."""
+        if self.anneal_state is None:
+            return None
+        n = self.anneal_iterations * self.T
+        return self.anneal_state[1:1 + n].view(self.anneal_iterations, self.T)
+
+    def set_noise_schedule(self, s):
+        """Annealed MPPI: replace the noise scales by the (N, T) array `s` (each in [2^-20, inf)); s and r = 1 / s^2 are computed in float64
+        from the values given and each rounded once, as the planner builds the configured schedule.  Both are written into the registered buffer, so a captured plan graph follows without a re-capture."""
+        import numpy as np
+        if self.anneal_state is None:
+            raise RuntimeError("set_noise_schedule needs annealed MPPI (anneal_iterations > 1 or a decay below 1)")
+        s = np.asarray(s.detach().cpu() if isinstance(s, torch.Tensor) else s, np.float64)
+        N, T = self.anneal_iterations, self.T
+        if s.shape != (N, T):
+            raise ValueError(f"set_noise_schedule: s must have shape (anneal_iterations, horizon) = ({N}, {T}), got {s.shape}")
+        if not (np.all(np.isfinite(s)) and s.min() >= ANNEAL_MIN_SCALE):
+            raise ValueError("set_noise_schedule: every s[i][t] must be finite and at least 2^-20")
+        vals = np.concatenate([s.reshape(-1), (1.0 / (s * s)).reshape(-1)]).astype(np.float32)
+        self.anneal_state[1:].copy_(torch.from_numpy(vals))
 
     @property
     def mean_action(self):
@@ -526,7 +570,7 @@ class MPPIPlanner:
         be = self.backend
         with _nvtx("mppi/shift"):
             be.shift(self.U, self.plan_ctr)
-        for i in range(self.cem_iterations):             # cem_iterations with mppi_mode cem, one otherwise
+        for i in range(self.iterations):                 # cem_iterations with mppi_mode cem, anneal_iterations otherwise
             self._iterate_batched(i)
 
     def _iterate_batched(self, iteration):
@@ -548,7 +592,7 @@ class MPPIPlanner:
 
     def _plan_stepwise(self, state):
         self.backend.shift(self.U, self.plan_ctr)
-        for i in range(self.cem_iterations):             # cem_iterations with mppi_mode cem, one otherwise
+        for i in range(self.iterations):                 # cem_iterations with mppi_mode cem, anneal_iterations otherwise
             state = self._iterate_stepwise(state, i)
 
     def _iterate_stepwise(self, state, iteration):

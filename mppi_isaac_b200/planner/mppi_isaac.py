@@ -83,6 +83,7 @@ class MPPIisaacPlanner(object):
                 self.mppi.smooth_state.copy_(old.smooth_state)   # and the last executed action of mppi_mode smooth
             if old.mode_state is not None and self.mppi.mode_state is not None and old.mode_state.shape == self.mppi.mode_state.shape:
                 self.mppi.mode_state.copy_(old.mode_state)       # and, with n_modes > 1, the executed mode and its free energies
+            # the annealing schedule is rebuilt from the config, not carried over: a keep_U rebuild starts from the configured decays
 
     def _make_mppi(self):
         return MPPIPlanner(

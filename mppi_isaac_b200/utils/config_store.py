@@ -49,6 +49,9 @@ class MPPIConfig:
     cvar_alpha: float = 1.0              # risk-aware MPPI: a control scores the mean of its ceil(alpha R) worst world costs, alpha in (0, 1]
     n_modes: int = 1                     # multi-modal MPPI (DESIGN.md section 2): M nominal sequences planned side by side, 1 .. 16, K / M >= 32 samples each
     mode_switch_margin: float = 0.0      # multi-modal MPPI: keep the executed mode while its free energy is within this margin (cost units) of the lowest
+    anneal_iterations: int = 1           # annealed MPPI (DESIGN.md section 2): N MPPI iterations per plan, 1 .. 16
+    anneal_iter_decay: float = 1.0       # annealed MPPI: c_i in (0, 1], the noise std factor per iteration
+    anneal_horizon_decay: float = 1.0    # annealed MPPI: c_h in (0, 1], the noise std factor per step towards the start of the horizon
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0

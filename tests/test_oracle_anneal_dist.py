@@ -1,0 +1,33 @@
+"""Annealed MPPI sharded over two gloo ranks on the checker backend, three iterations per plan: every rank ends every plan with the same
+actions, U and counter, and the sharded plan reproduces the single-process one."""
+import os
+import socket
+import sys
+
+import numpy as np
+import pytest
+import torch.multiprocessing as mp
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+
+def _free_port():
+    with socket.socket() as s:
+        s.bind(("127.0.0.1", 0))
+        return s.getsockname()[1]
+
+
+@pytest.mark.timeout(300)
+def test_sharded_annealed_plan_matches_single_process(tmp_path):
+    sys.path.insert(0, HERE)
+    import anneal_dist_worker as w
+    world, K = 2, 136
+    mp.spawn(w.run, args=(world, _free_port(), str(tmp_path), K), nprocs=world, join=True)
+    single, ref, ref_ctr = w.plan(K)
+    for name in ("act", "ctr", "U"):
+        a0 = np.load(tmp_path / f"{name}_0.npy")
+        np.testing.assert_array_equal(np.load(tmp_path / f"{name}_1.npy"), a0)   # both ranks hold the same bits
+    np.testing.assert_array_equal(np.load(tmp_path / "ctr_0.npy"), ref_ctr)
+    assert list(ref_ctr) == [3.0, 3.0, 3.0]
+    np.testing.assert_allclose(np.load(tmp_path / "act_0.npy"), ref, rtol=0, atol=2e-5)   # == the unsharded plan (fp32 reassociation only)
+    np.testing.assert_allclose(np.load(tmp_path / "U_0.npy"), single.mppi.U.numpy(), rtol=0, atol=2e-5)
