@@ -74,6 +74,24 @@ def dist_floats(params, nu):
     return 1 + nu, "(lambda, cov[nu])"
 
 
+def shard_row_floats(params, nu):
+    """Floats of one shard row that K3 (or the elite kernel of mppi_mode cem) writes under `params` with `nu` inputs once a
+    distribution is registered, as the library sizes its buffers (shard_row_floats in csrc/common.cuh): 2 + T*nu, + T*nu with
+    update_cov, + nu(nu+1)/2 with cov_full, + n(n+1)/2 with cov_horizon (n = T*nu); n_modes * (2 + T*nu) with n_modes > 1;
+    cem_row_floats with mppi_mode cem."""
+    T, nu = int(params.T), int(nu)
+    n = T * nu
+    if params.mode == MODE_CEM:
+        return cem_row_floats(T, nu, params.n_elites)
+    if params.n_modes > 1:
+        return int(params.n_modes) * (2 + n)
+    if params.update_cov and params.cov_horizon:
+        return 2 + n + n * (n + 1) // 2
+    if params.update_cov and params.cov_full:
+        return 2 + n + nu * (nu + 1) // 2
+    return 2 + n * (2 if params.update_cov else 1)
+
+
 def smooth_state_floats(T, nu):
     """Floats of the smooth state of mppi_mode smooth: (a_prev[nu], A[T][nu])."""
     return int(nu) + int(T) * int(nu)
@@ -252,19 +270,8 @@ class CudaBackend:
         return bool(self.params.update_cov) and bool(self.params.cov_horizon)
 
     def partial_row_floats(self) -> int:
-        """Floats of one shard row K3 writes with a registered distribution: 2 + T*nu, + T*nu with update_cov, + nu(nu+1)/2
-        with update_cov and cov_full, or + n(n+1)/2 with update_cov and cov_horizon (n = T*nu)."""
-        T, nu = int(self.params.T), int(self.model.nu)
-        if self.params.n_modes > 1:
-            return int(self.params.n_modes) * (2 + T * nu)
-        if self.params.mode == MODE_CEM:
-            return cem_row_floats(T, nu, self.params.n_elites)
-        if self._cov_horizon():
-            n = T * nu
-            return 2 + n + n * (n + 1) // 2
-        if self._cov_full():
-            return 2 + T * nu + nu * (nu + 1) // 2
-        return 2 + T * nu * (2 if self.params.update_cov else 1)
+        """Floats of one shard row K3 writes with a registered distribution (``shard_row_floats``)."""
+        return shard_row_floats(self.params, self.model.nu)
 
     def _check_row(self, rows, what):
         if ((self._cov_full() or self._cov_horizon() or self.params.mode == MODE_CEM or self.params.n_modes > 1) and self._dist_keepalive is not None

@@ -320,7 +320,6 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
     if (int rc = check_anneal(h, "mppib_reduce")) return rc;
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
-    if (cem_mode(h)) return launch_elite(h, cost, x, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
     return launch_reduce(h, cost, x, U, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
@@ -329,7 +328,6 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
     if (int rc = check_anneal(h, "mppib_reduce_finalize")) return rc;
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
-    if (cem_mode(h)) return launch_elite(h, cost, x, partial, U, action_out, stats, (cudaStream_t)stream);
     return launch_reduce(h, cost, x, U, partial, U, action_out, stats, (cudaStream_t)stream);
 }
 
@@ -341,7 +339,6 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
     }
     MPPIB_ON_DEVICE(h);
-    if (cem_mode(h)) return launch_cem_finalize(h, partials, G, U, action_out, stats, (cudaStream_t)stream);
     return launch_finalize(h, partials, G, U, action_out, stats, (cudaStream_t)stream);
 }
 
@@ -401,7 +398,6 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream) {
     MPPIB_REQUIRE(h && U, "mppib_shift: null argument");
     if (int rc = check_anneal(h, "mppib_shift")) return rc;
     MPPIB_ON_DEVICE(h);
-    if (cem_mode(h)) return launch_cem_shift(h, U, plan_ctr, (cudaStream_t)stream);
     return launch_shift(h, U, plan_ctr, (cudaStream_t)stream);
 }
 

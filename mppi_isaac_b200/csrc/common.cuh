@@ -37,11 +37,11 @@ struct MppibContext {
     int state_rows;          // NS
     int num_sms;
     // K3 scratch: per-CTA partials + ticket counter (device memory owned by the handle)
-    float* reduce_scratch;   // [max_ctas][partial_row_floats(), padded to 4]
+    float* reduce_scratch;   // [max_ctas][partial_row_capacity(), padded to 4]
     unsigned int* reduce_ticket;
     int reduce_max_ctas;
     // peer window (multi-GPU exchange over NVLink peer memory), see include/mppib.h
-    int peer_world, peer_rank, peer_pcap;      // pcap: floats per row (>= partial_row_floats(), multiple of 4)
+    int peer_world, peer_rank, peer_pcap;      // pcap: floats per row (>= partial_row_capacity(), multiple of 4)
     void* peer_win[MPPIB_MAX_PEERS];           // window base of every rank (own entry = local allocation)
     unsigned long long peer_timeout_ns;
     float* action_mirror;                      // pinned host mirror of the action written by K4 (nullable)
@@ -80,33 +80,67 @@ struct DeviceGuard {
     DeviceGuard _guard((h)->device);                                                        \
     MPPIB_CHECK_CUDA(_guard.err)
 
-// Floats of one shard row (beta, eta, W[T*nu] and, with update_cov, M2[T*nu], or with cov_full too C[nu(nu+1)/2]).  Buffers are
-// sized by the flags alone, so that registering a distribution never needs a reallocation; the kernels append M2 / C only when a
-// distribution is registered too.
-// MODE_CEM: the shard row (S, index bits)[E] + actions[E][T*nu], padded to 4 floats; the CEM state (include/mppib.h)
-__host__ __device__ static inline int cem_row_floats(int T, int nu, int E) { return (2 * E + E * T * nu + 3) & ~3; }
-static inline int cem_state_floats(int T, int nu, int E) { return 2 + E + T * nu + E * T * nu; }
-static inline int partial_row_capacity(const MppibParams& p, int nu) {
-    if (p.n_modes > 1) return p.n_modes * (2 + p.T * nu);
-    if (p.mode == MPPIB_MODE_CEM) return cem_row_floats(p.T, nu, p.n_elites);
-    if (p.update_cov && p.cov_full) return 2 + p.T * nu + nu * (nu + 1) / 2;
-    if (p.update_cov && p.cov_horizon) return 2 + p.T * nu + p.T * nu * (p.T * nu + 1) / 2;
-    return 2 + p.T * nu * (p.update_cov ? 2 : 1);
+// The update rule a plan runs: which K3 (or elite kernel), K4 and shift, and what their shard row carries.  Risk-aware MPPI is not a
+// rule but a K3 flag (risk_mode) that combines with PLAIN, DIST and FULL.
+enum Rule { RULE_PLAIN, RULE_DIST, RULE_FULL, RULE_HORIZON, RULE_SMOOTH, RULE_MODES, RULE_CEM };
+// Floats of one shard row:
+//   PLAIN, SMOOTH  (beta, eta, W[T*nu])
+//   DIST           (beta, eta, W[T*nu]), + M2[T*nu] with update_cov
+//   FULL           (beta, eta, W[T*nu], C[nu(nu+1)/2])
+//   HORIZON        (beta, eta, W[n], C[n(n+1)/2]), n = T*nu
+//   MODES          (beta, eta, W[T*nu]) of every mode
+//   CEM            (S, index bits)[E] + actions[E][T*nu], padded to 4 floats, E = n_elites
+// The kernels pass the parts they already hold (T, update_cov, ...); the host passes the parameter block.
+__host__ __device__ inline int shard_row_floats(Rule r, int T, int nu, bool update_cov, int n_modes, int E) {
+    const int NR = T * nu;
+    switch (r) {
+    case RULE_DIST: return 2 + NR + (update_cov ? NR : 0);
+    case RULE_FULL: return 2 + NR + nu * (nu + 1) / 2;
+    case RULE_HORIZON: return 2 + NR + NR * (NR + 1) / 2;
+    case RULE_MODES: return n_modes * (2 + NR);
+    case RULE_CEM: return (2 * E + E * T * nu + 3) & ~3;
+    default: return 2 + NR;
+    }
 }
-// Risk-aware MPPI (n_worlds = R > 1, a power of two): global rollout kg = c*R + r runs control sample c in world r.  K1 keys its draws
-// and its null / prior rows by c, K2 keys the per-rollout randomisation by r.  R <= 1 (and a zero-initialised block) keeps kg for both.
-__device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
-__device__ __forceinline__ uint32_t sample_world(uint32_t kg, int R) { return R > 1 ? kg & (uint32_t)(R - 1) : kg; }
+__host__ __device__ inline int shard_row_floats(Rule r, const MppibParams& p, int nu) {
+    return shard_row_floats(r, p.T, nu, p.update_cov, p.n_modes, p.n_elites);
+}
 static inline bool risk_mode(const MppibContext* c) { return c->params.n_worlds > 1; }
-// Multi-modal MPPI (n_modes = M > 1): global sample kg is drawn around mode kg / Kc of U[M][T][nu], Kc = mode_samples.  M <= 1 (and a
-// zero-initialised block) keeps mode 0 for every sample.
-__device__ __forceinline__ int sample_mode(uint32_t kg, const MppibParams& p) { return p.n_modes > 1 ? (int)(kg / (uint32_t)p.mode_samples) : 0; }
 static inline bool modes_on(const MppibContext* c) { return c->params.n_modes > 1; }
 static inline bool cem_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_CEM; }
 static inline bool smooth_mode(const MppibContext* c) { return c->params.mode == MPPIB_MODE_SMOOTH; }
 static inline bool adaptive_cov(const MppibContext* c) { return c->dist != nullptr && c->params.update_cov; }
 static inline bool adaptive_full(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_full; }
 static inline bool adaptive_horizon(const MppibContext* c) { return adaptive_cov(c) && c->params.cov_horizon; }
+// the rule of the handle as it stands: the adaptive rules need a registered distribution
+static inline Rule update_rule(const MppibContext* c) {
+    if (cem_mode(c)) return RULE_CEM;
+    if (modes_on(c)) return RULE_MODES;
+    if (smooth_mode(c)) return RULE_SMOOTH;
+    if (adaptive_horizon(c)) return RULE_HORIZON;
+    if (adaptive_full(c)) return RULE_FULL;
+    if (c->dist) return RULE_DIST;
+    return RULE_PLAIN;
+}
+// the rule the flags select once a distribution is registered: buffers are sized by it, so that registering a distribution never
+// needs a reallocation
+static inline Rule configured_rule(const MppibParams& p) {
+    if (p.mode == MPPIB_MODE_CEM) return RULE_CEM;
+    if (p.n_modes > 1) return RULE_MODES;
+    if (p.mode == MPPIB_MODE_SMOOTH) return RULE_SMOOTH;
+    if (p.update_cov && p.cov_horizon) return RULE_HORIZON;
+    if (p.update_cov && p.cov_full) return RULE_FULL;
+    if (p.update_cov || p.update_lambda) return RULE_DIST;
+    return RULE_PLAIN;
+}
+static inline int partial_row_capacity(const MppibParams& p, int nu) { return shard_row_floats(configured_rule(p), p, nu); }
+// Risk-aware MPPI (n_worlds = R > 1, a power of two): global rollout kg = c*R + r runs control sample c in world r.  K1 keys its draws
+// and its null / prior rows by c, K2 keys the per-rollout randomisation by r.  R <= 1 (and a zero-initialised block) keeps kg for both.
+__device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
+__device__ __forceinline__ uint32_t sample_world(uint32_t kg, int R) { return R > 1 ? kg & (uint32_t)(R - 1) : kg; }
+// Multi-modal MPPI (n_modes = M > 1): global sample kg is drawn around mode kg / Kc of U[M][T][nu], Kc = mode_samples.  M <= 1 (and a
+// zero-initialised block) keeps mode 0 for every sample.
+__device__ __forceinline__ int sample_mode(uint32_t kg, const MppibParams& p) { return p.n_modes > 1 ? (int)(kg / (uint32_t)p.mode_samples) : 0; }
 // Annealed MPPI: the row of the registered schedule a (counter, s[N][T], r[N][T]) that iteration min(counter, N - 1) reads -- the noise
 // scale s (recip = false) or r = 1 / s^2 (recip = true).  The counter is a float that K4 advances and the shift resets.
 __device__ __forceinline__ const float* anneal_row(const float* __restrict__ a, int n, int T, bool recip) {
@@ -133,6 +167,80 @@ static inline PeerArgs peer_args(const MppibContext* c) {
     PeerArgs a; a.world = c->peer_world; a.rank = c->peer_rank; a.pcap = c->peer_pcap; a.timeout_ns = c->peer_timeout_ns;
     for (int g = 0; g < MPPIB_MAX_PEERS; ++g) a.win[g] = c->peer_win[g];
     return a;
+}
+// the windows K3 (or the elite kernel, or the SYRK) publishes its row into: only when every peer is mapped (otherwise single-GPU
+// behaviour, world = 0)
+static inline PeerArgs reduce_peers(const MppibContext* c) {
+    PeerArgs a = peer_args(c);
+    for (int g = 0; g < a.world; ++g) if (!a.win[g]) { a.world = 0; break; }
+    if (a.world < 2) a.world = 0;
+    return a;
+}
+
+// The exchange protocol.  Publish: a rank stores its row of exchange seq = (its own window's consumed counter) + 1 into slot
+// (seq & 1, rank) of every window (remote stores over NVLink), then, after a system fence, release-stores seq into flag (seq & 1, rank)
+// of every window.  Acquire: K4 waits until the G flags of exchange seq in its own window hold seq, reads the rows and stores seq into
+// the counter (consume).  Two slots let the next exchange's rows land while K4 still reads this one's.
+struct PeerRow { uint32_t seq; size_t off; };   // off: in floats from the window base
+__device__ __forceinline__ PeerRow peer_row(const PeerArgs& peers) {
+    uint32_t seq = 0;
+    if (peers.world > 1) seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
+    return {seq, MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap};
+}
+// element e of this rank's row into every window (none without peers)
+__device__ __forceinline__ void peer_store(const PeerArgs& peers, const PeerRow& row, int e, float v) {
+    for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row.off + e] = v;
+}
+// after every thread's peer_store: the row is complete, tell every rank (a CTA-wide call, with peers only: world > 1)
+__device__ __forceinline__ void peer_release(const PeerArgs& peers, const PeerRow& row) {
+    __threadfence_system();
+    __syncthreads();
+    const int tid = threadIdx.x;
+    if (tid < peers.world) {
+        uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (row.seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
+        asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(row.seq) : "memory");
+    }
+}
+// wait until every rank's row of the next exchange has landed in this rank's window (a CTA-wide call); rows[g * stride] is rank g's
+struct PeerRows { const float* rows; int stride; uint32_t seq; };
+__device__ __forceinline__ PeerRows peer_acquire(const PeerArgs& peers, int G) {
+    char* win = reinterpret_cast<char*>(peers.win[peers.rank]);
+    const uint32_t seq = *reinterpret_cast<const volatile uint32_t*>(win) + 1u;
+    if ((int)threadIdx.x < G) {
+        const uint32_t* flag = reinterpret_cast<const uint32_t*>(win + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + threadIdx.x;
+        unsigned long long t0, now;
+        uint32_t got;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+        while (true) {
+            asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(got) : "l"(flag) : "memory");
+            if (got == seq) break;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+            if (now - t0 > peers.timeout_ns) {
+                printf("mppib_finalize: rank %d waited %.1f s for rank %d (exchange %u, flag %u): peer lost\n", peers.rank, (double)peers.timeout_ns * 1e-9, (int)threadIdx.x, seq, got);
+                __trap();
+            }
+            __nanosleep(64);
+        }
+    }
+    __syncthreads();
+    return {reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap, peers.pcap, seq};
+}
+// exchange `seq` is consumed: its slot may take the rows of exchange seq + 2 (one thread)
+__device__ __forceinline__ void peer_consume(const PeerArgs& peers, uint32_t seq) {
+    *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;
+}
+
+// Raise KERNEL's dynamic shared-memory limit to `bytes` on `device` where it is lower: the attribute belongs to the function on one
+// device, so the high-water mark is kept per device.
+template <auto KERNEL>
+int ensure_smem(int device, size_t bytes) {
+    static size_t attr[64] = {0};
+    size_t& a = attr[device & 63];
+    if (bytes > a) {
+        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        a = bytes;
+    }
+    return 0;
 }
 
 // kernel launchers (defined in the .cu files)

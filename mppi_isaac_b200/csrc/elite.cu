@@ -135,7 +135,7 @@ mppib_elite_kernel(const __grid_constant__ MppibParams p, int nu, const float* _
     __shared__ float un[EL_MAX_NR];
     __shared__ unsigned int s_last;
     const int K = p.K, T = p.T, NR = T * nu, E = p.n_elites, tid = threadIdx.x;
-    const int P = cem_row_floats(T, nu, E);
+    const int P = shard_row_floats(RULE_CEM, T, nu, false, 0, E);
     {
         const float lg = log2f(p.gamma);                                      // gamma^t as K3 computes it
         for (int t = tid; t < T; t += EL_NT) gp[t] = t == 0 ? 1.f : exp2f(lg * (float)t);
@@ -177,9 +177,7 @@ mppib_elite_kernel(const __grid_constant__ MppibParams p, int nu, const float* _
     }
     if (tid == 0) *ticket = 0u;
     // the shard row: (S, index bits)[E], actions[E][T*nu] gathered from x[T*nu][K]; missing entries (+inf, 0xFFFFFFFF, 0)
-    uint32_t seq = 0;
-    if (peers.world > 1) seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
-    const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
+    const PeerRow row = peer_row(peers);
     for (int q = tid; q < P; q += EL_NT) {
         float v = 0.f;
         if (q < 2 * E) {
@@ -192,16 +190,9 @@ mppib_elite_kernel(const __grid_constant__ MppibParams p, int nu, const float* _
             if (key != KEY_NONE) v = __ldg(x + (size_t)r * K + ((uint32_t)key - p.k_offset));
         }
         partial[q] = v;
-        for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + q] = v;
+        peer_store(peers, row, q, v);
     }
-    if (peers.world > 1) {
-        __threadfence_system();
-        __syncthreads();
-        if (tid < peers.world) {
-            uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
-            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
-        }
-    }
+    if (peers.world > 1) peer_release(peers, row);
     if (fin_U != nullptr) {
         // single-GPU plans: K4 on the row just written (the same code as mppib_finalize with G = 1, so the same bits); K1 read U and
         // the CEM state before this launch, so nothing else reads them now
@@ -217,35 +208,17 @@ mppib_cem_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const f
                           float* __restrict__ mirror, float* __restrict__ state) {
     __shared__ unsigned long long keys[FIN_MAX_KEYS];
     __shared__ float un[EL_MAX_NR];
-    int P = cem_row_floats(p.T, nu, p.n_elites);
     const float* partials = partials_in;
+    int P = shard_row_floats(RULE_CEM, p, nu);
     uint32_t seq = 0;
-    if (partials_in == nullptr) {
-        // rows come from this rank's peer window: wait until every rank's row of exchange `seq` has landed (as mppib_finalize_kernel)
-        char* win = reinterpret_cast<char*>(peers.win[peers.rank]);
-        seq = *reinterpret_cast<const volatile uint32_t*>(win) + 1u;
-        if ((int)threadIdx.x < G) {
-            const uint32_t* flag = reinterpret_cast<const uint32_t*>(win + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + threadIdx.x;
-            unsigned long long t0, now;
-            uint32_t got;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-            while (true) {
-                asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(got) : "l"(flag) : "memory");
-                if (got == seq) break;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-                if (now - t0 > peers.timeout_ns) {
-                    printf("mppib_finalize: rank %d waited %.1f s for rank %d (exchange %u, flag %u): peer lost\n", peers.rank, (double)peers.timeout_ns * 1e-9, (int)threadIdx.x, seq, got);
-                    __trap();
-                }
-                __nanosleep(64);
-            }
-        }
-        __syncthreads();
-        partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
-        P = peers.pcap;
+    if (partials_in == nullptr) {                                             // rows come from this rank's peer window
+        const PeerRows w = peer_acquire(peers, G);
+        partials = w.rows;
+        P = w.stride;
+        seq = w.seq;
     }
     cem_update(p, nu, partials, G, P, U, action_out, stats, mirror, state, keys, un);
-    if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
+    if (threadIdx.x == 0 && partials_in == nullptr) peer_consume(peers, seq);
 }
 
 // U[t] <- U[t+1], U[T-1] <- u_init; sigma[t][j] <- sigma0_j (the diagonal of sigma_chol); carry offset <- 1; *plan_ctr += 1
@@ -267,14 +240,6 @@ __global__ void mppib_cem_shift_kernel(const __grid_constant__ MppibParams p, in
     }
 }
 
-// K3 writes into the windows only when every peer is mapped (as reduce.cu's reduce_peers)
-PeerArgs elite_peers(const MppibContext* c) {
-    PeerArgs a = peer_args(c);
-    for (int g = 0; g < a.world; ++g) if (!a.win[g]) { a.world = 0; break; }
-    if (a.world < 2) a.world = 0;
-    return a;
-}
-
 int cem_checks(const MppibContext* c, const char* what) {
     const int NR = c->params.T * c->model.nu, E = c->params.n_elites;
     MPPIB_REQUIRE(c->dist != nullptr, "%s: mppi_mode cem needs its state registered with mppib_set_distribution", what);
@@ -293,7 +258,7 @@ int launch_elite(MppibContext* c, const float* cost, const float* x, float* part
     int grid = (K + EL_NEW - 1) / EL_NEW;
     if (grid > c->num_sms) grid = c->num_sms;
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
-    mppib_elite_kernel<<<grid, EL_NT, 0, s>>>(c->params, c->model.nu, cost, x, partial, c->reduce_scratch, c->reduce_ticket, elite_peers(c), fin_U,
+    mppib_elite_kernel<<<grid, EL_NT, 0, s>>>(c->params, c->model.nu, cost, x, partial, c->reduce_scratch, c->reduce_ticket, reduce_peers(c), fin_U,
                                               fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;

@@ -25,16 +25,14 @@ constexpr int NT = 256;         // threads per CTA
 constexpr int MAX_GRID = 512;   // persistent CTAs (<= scratch rows)
 constexpr int MAX_PAIRS = MPPIB_MAX_NU * (MPPIB_MAX_NU + 1) / 2;   // lower triangle of a full nu x nu covariance
 
-// what a shard row carries after (beta, eta, W[T*nu]): nothing, M2[T*nu] (update_cov) or C[nu(nu+1)/2] (update_cov with cov_full)
-enum RowKind { ROW_W = 0, ROW_M2 = 1, ROW_C = 2 };
-__host__ __device__ __forceinline__ int row_floats(int T, int nu, int kind) {
-    return 2 + T * nu + (kind == ROW_M2 ? T * nu : kind == ROW_C ? nu * (nu + 1) / 2 : 0);
-}
-// shared floats finalize_rows<true, true> needs after un[T*nu] and the G scales: m1[T*nu], d[T*nu], C[nu(nu+1)/2], Sigma, L, L^-1
+// the rules that read lambda (and Sigma) from a registered distribution and update it in K4
+__host__ __device__ constexpr bool rule_adapts(Rule r) { return r == RULE_DIST || r == RULE_FULL || r == RULE_HORIZON; }
+// The row a K3 CTA accumulates: the shard row, but one mode's block with MODES and (beta, eta, W[n]) with HORIZON (the SYRK appends C)
+__host__ __device__ constexpr Rule k3_row_rule(Rule r) { return r == RULE_MODES || r == RULE_HORIZON ? RULE_PLAIN : r; }
+// shared floats finalize_rows<RULE_FULL> needs after un[T*nu] and the G scales: m1[T*nu], d[T*nu], C[nu(nu+1)/2], Sigma, L, L^-1
 __host__ __device__ __forceinline__ int full_fin_floats(int T, int nu) { return 2 * T * nu + nu * (nu + 1) / 2 + 3 * nu * nu; }
-// cov_horizon, n = T*nu: the shard row (beta, eta, W[n], C[n(n+1)/2]) and the shared floats finalize_rows<true, false, true> needs
-// after un[n] and the G scales: m1[n], d[n], the packed lower triangle A[n(n+1)/2] it factors, pivots[n], a column buffer[n]
-__host__ __device__ __forceinline__ int hz_row_floats(int n) { return 2 + n + n * (n + 1) / 2; }
+// cov_horizon, n = T*nu: the shared floats finalize_rows<RULE_HORIZON> needs after un[n] and the G scales: m1[n], d[n], the packed lower
+// triangle A[n(n+1)/2] it factors, pivots[n], a column buffer[n]
 __host__ __device__ __forceinline__ int hz_fin_floats(int n) { return 4 * n + n * (n + 1) / 2; }
 __device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }     // offset of row i in a packed lower triangle
 // n_modes = M > 1: the shared floats modes_rows needs with G shard rows: d[M*T*nu], Sigma^-1 U then the coupled U [M*T*nu], U[M*T*nu],
@@ -212,10 +210,11 @@ __device__ __noinline__ void horizon_update(const MppibParams& p, int nu, const 
 // Sigma^-1 as they were.  The diagonal equals the diagonal rule above without its clamp at 0.
 // HZN (update_cov with cov_horizon): the rows carry C_g[n(n+1)/2] over the whole sequence; m1 and d are kept as n-vectors and
 // horizon_update does the rest.
-template <bool ADAPT, bool FULL = false, bool HZN = false>
+template <Rule R>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
                                               float* __restrict__ dist, float* __restrict__ hz_sig = nullptr) {
+    constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON;
     const int T = p.T, NR = T * nu;
     float* sg = un + NR;
     const float lam = ADAPT ? dist[0] : p.lambda_;
@@ -606,9 +605,7 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
         sc[q] = b == INFINITY ? 0.f : expf(-(b - bb[q / gx]) * inv_lambda);
     }
     __syncthreads();
-    uint32_t seq = 0;
-    if (peers.world > 1) seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
-    const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
+    const PeerRow row = peer_row(peers);
     for (int q = tid; q < P; q += NT) {
         const int m = q / P1, e = q % P1;
         const float* src = scratch + (size_t)m * gx * P4 + e;
@@ -618,16 +615,9 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
         for (int g = 0; g < gx; ++g) v += scm[g] * __ldcg(src + (size_t)g * P4);
         if (e == 0) v = bb[m];
         partial[q] = v;
-        for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + q] = v;
+        peer_store(peers, row, q, v);
     }
-    if (peers.world > 1) {
-        __threadfence_system();
-        __syncthreads();
-        if (tid < peers.world) {
-            uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
-            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
-        }
-    }
+    if (peers.world > 1) peer_release(peers, row);
     if (tid == 0) *ticket = 0u;
     if (fin_U != nullptr) {
         __threadfence();
@@ -639,7 +629,7 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
 // at least, `misc` = 8 floats.
-template <bool ADAPT, bool FULL = false, bool SMOOTH = false>
+template <Rule R>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
@@ -692,23 +682,14 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
         __syncthreads();
         // fused exchange: this rank's row goes straight into the window of every rank (remote stores over NVLink),
         // then one release-store of the arrival flag per peer; K4 on each rank acquires its own flags
-        uint32_t seq = 0;
-        if (peers.world > 1) seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
-        const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
+        const PeerRow row = peer_row(peers);
         for (int e = tid; e < P; e += NT) {
             const float v0 = fold[e] + fold[PP + e] + fold[2 * PP + e] + fold[3 * PP + e];
             const float v = e == 0 ? bb : v0;
             partial[e] = v;
-            for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + e] = v;
+            peer_store(peers, row, e, v);
         }
-        if (peers.world > 1) {
-            __threadfence_system();
-            __syncthreads();
-            if (tid < peers.world) {
-                uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
-                asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
-            }
-        }
+        if (peers.world > 1) peer_release(peers, row);
         if (tid == 0) *ticket = 0u;
         if (fin_U != nullptr) {
             // single-GPU plans: this CTA is the last one alive and holds the shard row -> do K4's work here (U update, savgol,
@@ -716,8 +697,8 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             // cov -- in its prologue, before it took its ticket, so this CTA is the only reader left when it updates them.
             __threadfence();
             __syncthreads();
-            if constexpr (SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
-            else finalize_rows<ADAPT, FULL>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
+            else finalize_rows<R>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
             if (tid == 0 && anneal) anneal[0] += 1.0f;                        // annealed MPPI: the next iteration's row (every CTA read it)
         }
     }
@@ -739,21 +720,21 @@ constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
 
 // Shared-memory layout of the kernel with `nstage` ring stages, used by the host for the size and by the kernel for its pointers.
 // Offsets in floats from the base, except `bar` (bytes).  The last CTA reuses the ring for the fold (fold_and_finish), so the ring
-// region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.  With the C row (ROW_C)
+// region is at least fold_floats long; for every shape but T*nu + T <= 2 the ring stages alone are longer.  With the C row (RULE_FULL)
 // the fused K4 also keeps its covariance scratch there (full_fin_floats), which the ring stages of every accepted shape exceed.
 struct WsLayout {
     int g, gp, wk, cpart, misc;   // [NR4] lambda Sigma^-1 U | [T4] gamma^t | [8][32] weights | [nparts][P4] warp partials | [8]
     int us;                       // smooth: [NR4] U for the smoothness cost (no floats otherwise)
     int bar;                      // full[nstage], then empty[nstage] mbarriers
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
-    // kind: what the shard row carries after W (RowKind); nparts: warp partials stored, by default one per consumer warp
+    // row: the rule whose shard row the warp partials hold; nparts: warp partials stored, by default one per consumer warp
     // (min(nstage, WS_NCONS): the launch rounds the ring depth down to a multiple of the consumer count)
-    __host__ __device__ WsLayout(int T, int nu, int nstage, int kind = ROW_W, bool smooth = false, int nparts = -1, int modes = 1) {
-        const int NR = T * nu, P4 = (row_floats(T, nu, kind) + 3) & ~3;
+    __host__ __device__ WsLayout(int T, int nu, int nstage, Rule row, bool update_cov, bool smooth = false, int nparts = -1, int modes = 1) {
+        const int NR = T * nu, P4 = (shard_row_floats(row, T, nu, update_cov, 1, 0) + 3) & ~3;
         if (nparts < 0) nparts = nstage < WS_NCONS ? nstage : WS_NCONS;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
-        if (kind == ROW_C && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
+        if (row == RULE_FULL && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
         if (modes > 1 && g < modes_fin_floats(NR, modes, 1)) g = modes_fin_floats(NR, modes, 1);   // the fused K4 of n_modes > 1
         gp = g + ((NR + 3) & ~3);
         wk = gp + ((T + 3) & ~3);
@@ -769,7 +750,9 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// ADAPT (a distribution is registered): lambda comes from dist[0]; with update_cov the SIMPLE-mode Sigma^-1 is diag(1 / dist[1 + j])
+// The template is <RPL, rule, RISK>: rows of W per lane (T*nu <= 32 * RPL), the update rule (PLAIN, DIST, FULL, HORIZON, SMOOTH or
+// MODES; CEM has the elite kernel) and the risk flag (PLAIN, DIST and FULL only).  The body names what the rule implies:
+// ADAPT (DIST, FULL, HORIZON: a distribution is registered): lambda comes from dist[0]; with update_cov the SIMPLE-mode Sigma^-1 is diag(1 / dist[1 + j])
 // and phase C keeps a second running sum per row, M2[r] = sum_k w_k (x[r][k] - c[r])^2 with c = U (MEAN) or 0 (SIMPLE), rescaled
 // online like W; the shard row becomes (beta, eta, W[T*nu], M2[T*nu]).  The bytes read from HBM are the same.
 // FULL (update_cov with cov_full): the SIMPLE-mode Sigma^-1 is the full one of dist, and instead of M2 every consumer lane keeps the
@@ -789,13 +772,14 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // row m*gx + x, and the last CTA folds every mode into block m of the row [M][2 + T*nu] (fold_modes_and_finish).
 // anneal (annealed MPPI, nullable): the registered schedule of anneal_n iterations; SIMPLE mode scales g_r by r[t] = 1 / s[t]^2 of the
 // iteration's row after the lambda product (a schedule of ones changes no bit), and the fused K4 advances the counter.
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false, bool MODES = false>   // rows of W per lane: T*nu <= 32 * RPL
+template <int RPL, Rule R, bool RISK>
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                        float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
                        const float* __restrict__ hz_g, float* __restrict__ smooth, float* __restrict__ anneal, int anneal_n) {
+    constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON, SMOOTH = R == RULE_SMOOTH, MODES = R == RULE_MODES;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -803,14 +787,14 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
     const bool simple = SMOOTH || p.mode == MPPIB_MODE_SIMPLE;
-    const bool m2 = ADAPT && !FULL && !HZN && p.update_cov;
+    const bool m2 = R == RULE_DIST && p.update_cov;
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
-    const int P = 2 + (m2 ? 2 : 1) * NR + npairs;
+    const int P = shard_row_floats(k3_row_rule(R), T, nu, m2, 1, 0);
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
     const bool smooth_term = SMOOTH && p.smooth_weight != 0.f;
-    const WsLayout L(T, nu, nstage, FULL ? ROW_C : m2 ? ROW_M2 : ROW_W, smooth_term, -1, MODES ? p.n_modes : 1);
+    const WsLayout L(T, nu, nstage, k3_row_rule(R), m2, smooth_term, -1, MODES ? p.n_modes : 1);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -1057,56 +1041,36 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     __syncthreads();
     if (!s_last_ws) return;
     __threadfence();
-    if constexpr (MODES) {
-        fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
-        return;
-    }
-    fold_and_finish<ADAPT, FULL, SMOOTH>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda, dist,
-                                         smooth, anneal);
+    // the horizon K3 folds as DIST's does; it gets no fin_U and no peers, the SYRK finishes its row
+    if constexpr (MODES) fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
+    else fold_and_finish<HZN ? RULE_DIST : R>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda,
+                                              dist, smooth, anneal);
 }
 
-// K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; ADAPT: the
-// distribution update of finalize_rows (FULL: of the full covariance, HZN: of the covariance over the horizon); SMOOTH: smooth_rows;
-// MODES: modes_rows (n_modes > 1, dist = the mode state).  anneal (annealed MPPI, nullable): the counter of the registered schedule is
-// advanced by one after the update.
-template <bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool MODES = false>
+// K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; DIST / FULL /
+// HORIZON: the distribution update of finalize_rows (FULL: of the full covariance, HORIZON: of the covariance over the horizon); SMOOTH:
+// smooth_rows; MODES: modes_rows (n_modes > 1, dist = the mode state).  anneal (annealed MPPI, nullable): the counter of the registered
+// schedule is advanced by one after the update.
+template <Rule R>
 __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
                 float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth,
                 float* __restrict__ anneal) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
-    const int T = p.T, NR = T * nu;
-    int P = MODES ? p.n_modes * (2 + NR) : HZN ? hz_row_floats(NR) : FULL ? row_floats(T, nu, ROW_C) : 2 + ((ADAPT && p.update_cov) ? 2 : 1) * NR;   // row stride of the partials
     const float* partials = partials_in;
+    int P = shard_row_floats(R, p, nu);                                       // row stride of the partials
     uint32_t seq = 0;
-    if (partials_in == nullptr) {
-        // rows come from this rank's peer window: wait until every rank's row of exchange `seq` has landed
-        char* win = reinterpret_cast<char*>(peers.win[peers.rank]);
-        seq = *reinterpret_cast<const volatile uint32_t*>(win) + 1u;
-        if ((int)threadIdx.x < G) {
-            const uint32_t* flag = reinterpret_cast<const uint32_t*>(win + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + threadIdx.x;
-            unsigned long long t0, now; uint32_t got;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-            while (true) {
-                asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(got) : "l"(flag) : "memory");
-                if (got == seq) break;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-                if (now - t0 > peers.timeout_ns) {
-                    printf("mppib_finalize: rank %d waited %.1f s for rank %d (exchange %u, flag %u): peer lost\n", peers.rank, (double)peers.timeout_ns * 1e-9, (int)threadIdx.x, seq, got);
-                    __trap();
-                }
-                __nanosleep(64);
-            }
-        }
-        __syncthreads();
-        partials = reinterpret_cast<const float*>(win + MPPIB_WIN_DATA_OFF) + (size_t)(seq & 1u) * G * peers.pcap;
-        P = peers.pcap;
+    if (partials_in == nullptr) {                                             // rows come from this rank's peer window
+        const PeerRows w = peer_acquire(peers, G);
+        partials = w.rows;
+        P = w.stride;
+        seq = w.seq;
     }
-    if constexpr (MODES) modes_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
-    else if constexpr (SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
-    else finalize_rows<ADAPT, FULL, HZN>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
-    if (threadIdx.x == 0 && partials_in == nullptr) *reinterpret_cast<volatile uint32_t*>(peers.win[peers.rank]) = seq;   // exchange `seq` consumed
+    if constexpr (R == RULE_MODES) modes_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
+    else if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
+    else finalize_rows<R>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
+    if (threadIdx.x == 0 && partials_in == nullptr) peer_consume(peers, seq);
     if (threadIdx.x == 0 && anneal) anneal[0] += 1.0f;
 }
 
@@ -1127,7 +1091,7 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
                   const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action, float* __restrict__ fin_stats,
                   float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_sig) {
     extern __shared__ __align__(16) float hsm[];
-    const int n = p.T * nu, K = p.K, P = hz_row_floats(n);
+    const int n = p.T * nu, K = p.K, P = shard_row_floats(RULE_HORIZON, p, nu);
     const int tid = threadIdx.x;
     const int nb = (n + HZ_TILE - 1) / HZ_TILE, ntiles = nb * (nb + 1) / 2;
     const int tile = (int)blockIdx.x / ksplit, split = (int)blockIdx.x % ksplit;
@@ -1220,23 +1184,14 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
     if (peers.world > 1) {
         // the complete row goes into the window of every rank, then one release-store of the arrival flag per peer (as in
         // fold_and_finish)
-        const uint32_t seq = *reinterpret_cast<const volatile uint32_t*>(peers.win[peers.rank]) + 1u;
-        const size_t row_off = MPPIB_WIN_DATA_OFF / sizeof(float) + ((size_t)(seq & 1u) * peers.world + peers.rank) * peers.pcap;
-        for (int e = tid; e < P; e += blockDim.x) {
-            const float v = __ldcg(&partial[e]);
-            for (int g = 0; g < peers.world; ++g) reinterpret_cast<float*>(peers.win[g])[row_off + e] = v;
-        }
-        __threadfence_system();
-        __syncthreads();
-        if (tid < peers.world) {
-            uint32_t* flag = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers.win[tid]) + MPPIB_WIN_FLAGS_OFF) + (seq & 1u) * MPPIB_MAX_PEERS + peers.rank;
-            asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
-        }
+        const PeerRow row = peer_row(peers);
+        for (int e = tid; e < P; e += blockDim.x) peer_store(peers, row, e, __ldcg(&partial[e]));
+        peer_release(peers, row);
     }
     if (fin_U != nullptr) {
         // single-GPU plans: every CTA read U and lambda before it took its ticket, so this CTA is the only reader left
         __syncthreads();
-        finalize_rows<true, false, true>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, hsm, dist, hz_sig);
+        finalize_rows<RULE_HORIZON>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, hsm, dist, hz_sig);
     }
 }
 
@@ -1304,42 +1259,33 @@ int make_map(CUtensorMap* tm, const float* base, int rows, int K, int box_rows, 
     return 0;
 }
 
-// K3 writes into the windows only when every peer is mapped (otherwise: single-GPU behaviour, world = 0)
-static PeerArgs reduce_peers(const MppibContext* c) {
-    PeerArgs a = peer_args(c);
-    for (int g = 0; g < a.world; ++g) if (!a.win[g]) { a.world = 0; break; }
-    if (a.world < 2) a.world = 0;
-    return a;
-}
-
-// The ring depth: the deepest ring (<= 8 stages) that fits next to seven warp partials, the depths every shape was tuned at.  Where
-// that leaves fewer than two stages (the second-moment row at T = 256, T*nu = 512), two stages fit next to their two consumers'.
-static int reduce_ws_stages(int T, int nu, int kind, bool smooth = false) {
+// The ring depth: the deepest ring (<= 8 stages) that fits next to seven warp partials of the rule's row, the depths every shape was
+// tuned at.  Where that leaves fewer than two stages (the second-moment row at T = 256, T*nu = 512), two stages fit next to their two
+// consumers'.
+static int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth = false) {
     int ns = 8;
-    while (ns > 1 && WsLayout(T, nu, ns, kind, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
-    if (ns < 2 && WsLayout(T, nu, 2, kind, smooth).bytes <= 224 * 1024) ns = 2;
+    while (ns > 1 && WsLayout(p.T, nu, ns, row, p.update_cov, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
+    if (ns < 2 && WsLayout(p.T, nu, 2, row, p.update_cov, smooth).bytes <= 224 * 1024) ns = 2;
     return ns;
 }
 
-template <int RPL, bool ADAPT, bool FULL = false, bool HZN = false, bool SMOOTH = false, bool RISK = false, bool MODES = false>
+// smooth, anneal: the state of mode smooth and the annealing schedule, for the rules that read them (nullptr otherwise)
+template <int RPL, Rule R, bool RISK>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
-                       float* fin_stats, cudaStream_t s) {
+                       float* fin_stats, float* smooth, float* anneal, cudaStream_t s) {
     const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
-    const int kind = FULL ? ROW_C : (ADAPT && c->params.update_cov) ? ROW_M2 : ROW_W;
-    const bool smooth_term = SMOOTH && c->params.smooth_weight != 0.f;    // the `us` region of the kernel's layout
-    const int nstage_max = reduce_ws_stages(T, nu, kind, smooth_term);
+    // The horizon K3 sizes its ring for the M2 row of update_cov, which it does not write: its kernel addresses the W layout
+    // (DESIGN.md, "The horizon K3's ring is sized for a row it does not write").
+    const Rule row = R == RULE_HORIZON ? RULE_DIST : k3_row_rule(R);
+    const bool smooth_term = R == RULE_SMOOTH && c->params.smooth_weight != 0.f;   // the `us` region of the kernel's layout
+    const int nstage_max = reduce_ws_stages(c->params, nu, row, smooth_term);
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
-    const int modes = MODES ? c->params.n_modes : 1;
-    const size_t smem = WsLayout(T, nu, nstage, kind, smooth_term, -1, modes).bytes;
-    static size_t smem_attr[64] = {0};
-    size_t& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK, MODES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
-    }
+    const int modes = R == RULE_MODES ? c->params.n_modes : 1;
+    const size_t smem = WsLayout(T, nu, nstage, row, c->params.update_cov, smooth_term, -1, modes).bytes;
+    if (int rc = ensure_smem<mppib_reduce_ws_kernel<RPL, R, RISK>>(c->device, smem)) return rc;
     int xbox_rows = NR < 256 ? NR : 256;
     while (NR % xbox_rows != 0) --xbox_rows;
     // tensor maps are rebuilt only when a buffer, the shape or the device changes (the eager / stepwise path calls this per plan)
@@ -1353,7 +1299,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     const int ntiles = (K + WS_W - 1) / WS_W;
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
     if (grid > MAX_GRID) grid = MAX_GRID;
-    if (MODES) {
+    if (R == RULE_MODES) {
         // gx CTAs per mode, about one per SM over all modes, no more than the tiles of the largest mode's local range
         int tmax = 0;
         for (int m = 0; m < modes; ++m) {
@@ -1367,14 +1313,25 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     }
     MPPIB_REQUIRE(grid <= c->reduce_max_ctas, "mppib_reduce: scratch too small");
     PeerArgs peers = reduce_peers(c);
-    if (HZN) peers.world = 0;                                                 // the row is complete only after the SYRK, which stores it
-    mppib_reduce_ws_kernel<RPL, ADAPT, FULL, HZN, SMOOTH, RISK, MODES><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U,
-                                                                            c->reduce_scratch, c->reduce_ticket, partial, peers, fin_U, fin_action,
-                                                                            fin_stats, fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g,
-                                                                            SMOOTH ? c->smooth : nullptr, MODES || HZN || SMOOTH ? nullptr : c->anneal,
-                                                                            c->anneal_n);
+    if (R == RULE_HORIZON) peers.world = 0;                                   // the row is complete only after the SYRK, which stores it
+    mppib_reduce_ws_kernel<RPL, R, RISK><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch,
+                                                                             c->reduce_ticket, partial, peers, fin_U, fin_action, fin_stats,
+                                                                             fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g, smooth, anneal,
+                                                                             c->anneal_n);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+// the RPL ladder: T*nu <= 32 * RPL rows of W per lane (the horizon rule's n = T*nu <= 256 stops at 8)
+template <Rule R, bool RISK>
+int launch_reduce_rule(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
+                       float* fin_stats, float* smooth, float* anneal, cudaStream_t s) {
+    const int NR = c->params.T * c->model.nu;
+    if (NR <= 32 * 4) return launch_reduce_ws_t<4, R, RISK>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, smooth, anneal, s);
+    if constexpr (R != RULE_HORIZON) {
+        if (NR > 32 * 8) return launch_reduce_ws_t<16, R, RISK>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, smooth, anneal, s);
+    }
+    return launch_reduce_ws_t<8, R, RISK>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, smooth, anneal, s);
 }
 
 // ksplit x chunk length of the SYRK: about one CTA per SM over the lower-triangle tiles, chunks a multiple of HZ_KB samples
@@ -1398,12 +1355,7 @@ int launch_syrk(MppibContext* c, const float* x, const float* U, float* partial,
     MPPIB_REQUIRE((size_t)ntiles * ksplit * HZ_TILE * HZ_TILE <= (size_t)c->hz_scr_floats, "mppib_reduce: SYRK scratch too small");
     int smem = (int)sizeof(float) * 2 * HZ_KB * HZ_TILE;
     if (fin_U != nullptr && hz_fin_smem(n, 1) > smem) smem = hz_fin_smem(n, 1);
-    static int smem_attr[64] = {0};
-    int& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr = smem;
-    }
+    if (int rc = ensure_smem<mppib_syrk_kernel>(c->device, smem)) return rc;
     mppib_syrk_kernel<<<ntiles * ksplit, 256, smem, s>>>(c->params, c->model.nu, ksplit, kchunk, x, U, c->hz_S, partial, c->hz_scr, c->hz_ticket,
                                                          reduce_peers(c), fin_U, fin_action, fin_stats, fin_U ? c->action_mirror : nullptr, c->dist,
                                                          c->hz_sig);
@@ -1442,126 +1394,114 @@ int alloc_horizon(MppibContext* c) {
 
 int launch_reduce(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                   float* fin_stats, cudaStream_t s) {
+    const Rule rule = update_rule(c);
+    if (rule == RULE_CEM) return launch_elite(c, cost, x, partial, fin_U, fin_action, fin_stats, s);   // none of K3's limits apply
     const int T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(c->params.K >= 4 && c->params.K % 4 == 0, "mppib_reduce: K=%d must be a positive multiple of 4 (16-byte rows for TMA / 128-bit loads)", c->params.K);
     MPPIB_REQUIRE(T * nu <= 32 * 16, "mppib_reduce: T*nu = %d exceeds %d", T * nu, 32 * 16);
     MPPIB_REQUIRE(T <= 256, "mppib_reduce: T = %d exceeds the 256-row TMA box", T);
-    MPPIB_REQUIRE(reduce_ws_stages(T, nu, ROW_W) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
-    MPPIB_REQUIRE(!adaptive_cov(c) || adaptive_full(c) || reduce_ws_stages(T, nu, ROW_M2) >= 2,
+    MPPIB_REQUIRE(reduce_ws_stages(c->params, nu, RULE_PLAIN) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
+    MPPIB_REQUIRE(!adaptive_cov(c) || adaptive_full(c) || reduce_ws_stages(c->params, nu, RULE_DIST) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the second-moment row of update_cov", T, nu);
-    MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(T, nu, ROW_C) >= 2,
+    MPPIB_REQUIRE(!adaptive_full(c) || reduce_ws_stages(c->params, nu, RULE_FULL) >= 2,
                   "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the covariance row of cov_full", T, nu);
     const int NR = T * nu;
-    if (modes_on(c)) {
-        MPPIB_REQUIRE(c->dist != nullptr, "mppib_reduce: n_modes > 1 needs its mode state registered with mppib_set_distribution");
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16, false, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    }
-    if (smooth_mode(c)) {
-        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_reduce: mode smooth needs its state registered with mppib_set_smooth_state");
-        MPPIB_REQUIRE(reduce_ws_stages(T, nu, ROW_W, true) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages in mode smooth", T, nu);
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    }
-    if (risk_mode(c)) {
+    const bool risk = risk_mode(c);
+    if (risk) {
         const int R = c->params.n_worlds;
         MPPIB_REQUIRE(c->params.K % R == 0 && c->params.k_offset % (uint32_t)R == 0, "mppib_reduce: n_worlds = %d needs K = %d and k_offset = %u to be multiples of it",
                       R, c->params.K, c->params.k_offset);
-        MPPIB_REQUIRE(!adaptive_horizon(c), "mppib_reduce: n_worlds > 1 excludes cov_horizon");
-        if (adaptive_full(c)) {
-            if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-            if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-            return launch_reduce_ws_t<16, true, true, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        }
-        if (c->dist) {
-            if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-            if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-            return launch_reduce_ws_t<16, true, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        }
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16, false, false, false, false, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+        MPPIB_REQUIRE(rule != RULE_HORIZON, "mppib_reduce: n_worlds > 1 excludes cov_horizon");
     }
-    if (adaptive_horizon(c)) {
+    // the annealing schedule is read by the K3 of PLAIN, DIST and FULL, the smooth state by SMOOTH's
+    switch (rule) {
+    case RULE_MODES:
+        MPPIB_REQUIRE(c->dist != nullptr, "mppib_reduce: n_modes > 1 needs its mode state registered with mppib_set_distribution");
+        return launch_reduce_rule<RULE_MODES, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, nullptr, s);
+    case RULE_SMOOTH:
+        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_reduce: mode smooth needs its state registered with mppib_set_smooth_state");
+        MPPIB_REQUIRE(reduce_ws_stages(c->params, nu, RULE_SMOOTH, true) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages in mode smooth", T, nu);
+        return launch_reduce_rule<RULE_SMOOTH, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, c->smooth, nullptr, s);
+    case RULE_HORIZON: {
         MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N, "mppib_reduce: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, NR);
         MPPIB_REQUIRE(c->hz_S != nullptr && c->hz_K == c->params.K && c->hz_n == NR, "mppib_reduce: cov_horizon buffers are not sized for K = %d, n = %d",
                       c->params.K, NR);
-        const int rc = NR <= 32 * 4 ? launch_reduce_ws_t<4, true, false, true>(c, cost, x, U, partial, nullptr, nullptr, nullptr, s)
-                                    : launch_reduce_ws_t<8, true, false, true>(c, cost, x, U, partial, nullptr, nullptr, nullptr, s);
+        const int rc = launch_reduce_rule<RULE_HORIZON, false>(c, cost, x, U, partial, nullptr, nullptr, nullptr, nullptr, nullptr, s);
         if (rc) return rc;
         return launch_syrk(c, x, U, partial, fin_U, fin_action, fin_stats, s);
     }
-    if (adaptive_full(c)) {
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16, true, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
+    case RULE_FULL:
+        return risk ? launch_reduce_rule<RULE_FULL, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s)
+                    : launch_reduce_rule<RULE_FULL, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s);
+    case RULE_DIST:
+        return risk ? launch_reduce_rule<RULE_DIST, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s)
+                    : launch_reduce_rule<RULE_DIST, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s);
+    default:   // RULE_PLAIN
+        return risk ? launch_reduce_rule<RULE_PLAIN, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s)
+                    : launch_reduce_rule<RULE_PLAIN, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s);
     }
-    if (c->dist) {
-        if (NR <= 32 * 4) return launch_reduce_ws_t<4, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        if (NR <= 32 * 8) return launch_reduce_ws_t<8, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-        return launch_reduce_ws_t<16, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    }
-    if (NR <= 32 * 4) return launch_reduce_ws_t<4, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    if (NR <= 32 * 8) return launch_reduce_ws_t<8, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
-    return launch_reduce_ws_t<16, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, s);
 }
 
-int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
-    const int NR = c->params.T * c->model.nu;
-    if (modes_on(c)) {
-        MPPIB_REQUIRE(c->dist != nullptr, "mppib_finalize: n_modes > 1 needs its mode state registered with mppib_set_distribution");
-        const int smem = (int)sizeof(float) * modes_fin_floats(NR, c->params.n_modes, G);
-        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: n_modes = %d with T*nu = %d and G = %d needs %d bytes of shared memory", c->params.n_modes, NR, G, smem);
-        static int smem_attr[64] = {0};
-        int& attr = smem_attr[c->device & 63];
-        if (smem > attr) {
-            MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_finalize_kernel<false, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            attr = smem;
-        }
-        mppib_finalize_kernel<false, false, false, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                                   c->action_mirror, c->dist, nullptr, nullptr, nullptr);
-    } else if (smooth_mode(c)) {
-        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_finalize: mode smooth needs its state registered with mppib_set_smooth_state");
-        mppib_finalize_kernel<false, false, false, true><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats,
-                                                                                                peer_args(c), c->action_mirror, nullptr, nullptr, c->smooth, nullptr);
-    } else if (adaptive_horizon(c)) {
-        MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N && c->hz_sig != nullptr && c->hz_n == NR, "mppib_finalize: cov_horizon buffers are not sized for n = %d", NR);
-        const int smem = hz_fin_smem(NR, G);
-        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: cov_horizon with n = %d and G = %d needs %d bytes of shared memory", NR, G, smem);
-        static int smem_attr[64] = {0};
-        int& attr = smem_attr[c->device & 63];
-        if (smem > attr) {
-            MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_finalize_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            attr = smem;
-        }
-        mppib_finalize_kernel<true, false, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror,
-                                                                      c->dist, c->hz_sig, nullptr, nullptr);
-    } else if (adaptive_full(c)) {
-        const size_t smem = (NR + G + full_fin_floats(c->params.T, c->model.nu)) * sizeof(float);
-        mppib_finalize_kernel<true, true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                               nullptr, nullptr, c->anneal);
-    } else if (c->dist) {
-        const size_t smem = (NR + G + (adaptive_cov(c) ? NR : 0)) * sizeof(float);
-        mppib_finalize_kernel<true><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, c->dist,
-                                                         nullptr, nullptr, c->anneal);
-    } else {
-        mppib_finalize_kernel<false><<<1, 256, (NR + G) * sizeof(float), s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c),
-                                                                              c->action_mirror, nullptr, nullptr, nullptr, c->anneal);
-    }
+// one K4 launch; dist, hz_sig, smooth, anneal: the buffers the rule reads (nullptr otherwise)
+template <Rule R>
+static int launch_finalize_t(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, size_t smem, float* dist,
+                             float* hz_sig, float* smooth, float* anneal, cudaStream_t s) {
+    mppib_finalize_kernel<R><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, dist, hz_sig,
+                                                  smooth, anneal);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
+int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
+    const int NR = c->params.T * c->model.nu;
+    const size_t un = (NR + G) * sizeof(float);                               // U and the G scales, the shared floats of every rule
+    switch (update_rule(c)) {
+    case RULE_CEM:
+        return launch_cem_finalize(c, partials, G, U, action_out, stats, s);
+    case RULE_MODES: {
+        MPPIB_REQUIRE(c->dist != nullptr, "mppib_finalize: n_modes > 1 needs its mode state registered with mppib_set_distribution");
+        const int smem = (int)sizeof(float) * modes_fin_floats(NR, c->params.n_modes, G);
+        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: n_modes = %d with T*nu = %d and G = %d needs %d bytes of shared memory", c->params.n_modes, NR, G, smem);
+        if (int rc = ensure_smem<mppib_finalize_kernel<RULE_MODES>>(c->device, smem)) return rc;
+        return launch_finalize_t<RULE_MODES>(c, partials, G, U, action_out, stats, smem, c->dist, nullptr, nullptr, nullptr, s);
+    }
+    case RULE_SMOOTH:
+        MPPIB_REQUIRE(c->smooth != nullptr, "mppib_finalize: mode smooth needs its state registered with mppib_set_smooth_state");
+        return launch_finalize_t<RULE_SMOOTH>(c, partials, G, U, action_out, stats, un, nullptr, nullptr, c->smooth, nullptr, s);
+    case RULE_HORIZON: {
+        MPPIB_REQUIRE(NR <= MPPIB_HZ_MAX_N && c->hz_sig != nullptr && c->hz_n == NR, "mppib_finalize: cov_horizon buffers are not sized for n = %d", NR);
+        const int smem = hz_fin_smem(NR, G);
+        MPPIB_REQUIRE(smem <= 227 * 1024, "mppib_finalize: cov_horizon with n = %d and G = %d needs %d bytes of shared memory", NR, G, smem);
+        if (int rc = ensure_smem<mppib_finalize_kernel<RULE_HORIZON>>(c->device, smem)) return rc;
+        return launch_finalize_t<RULE_HORIZON>(c, partials, G, U, action_out, stats, smem, c->dist, c->hz_sig, nullptr, nullptr, s);
+    }
+    case RULE_FULL:
+        return launch_finalize_t<RULE_FULL>(c, partials, G, U, action_out, stats, un + full_fin_floats(c->params.T, c->model.nu) * sizeof(float), c->dist,
+                                            nullptr, nullptr, c->anneal, s);
+    case RULE_DIST:
+        return launch_finalize_t<RULE_DIST>(c, partials, G, U, action_out, stats, un + (adaptive_cov(c) ? NR : 0) * sizeof(float), c->dist, nullptr,
+                                            nullptr, c->anneal, s);
+    default:   // RULE_PLAIN
+        return launch_finalize_t<RULE_PLAIN>(c, partials, G, U, action_out, stats, un, nullptr, nullptr, nullptr, c->anneal, s);
+    }
+}
+
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) {
     const int NR = c->params.T * c->model.nu;
-    if (modes_on(c)) {
+    float* hz_g = nullptr;                                                    // lambda Sigma_H^-1 U for K3's control cost
+    switch (update_rule(c)) {
+    case RULE_CEM:
+        return launch_cem_shift(c, U, plan_ctr, s);
+    case RULE_MODES:
         mppib_shift_modes_kernel<<<1, 256, c->params.n_modes * NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr);
         MPPIB_CHECK_CUDA(cudaGetLastError());
         return 0;
+    case RULE_HORIZON:
+        if (c->params.mode == MPPIB_MODE_SIMPLE) hz_g = c->hz_g;
+        break;
+    default:
+        break;
     }
-    float* hz_g = adaptive_horizon(c) && c->params.mode == MPPIB_MODE_SIMPLE ? c->hz_g : nullptr;
     mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g, c->anneal);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;

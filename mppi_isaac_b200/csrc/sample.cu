@@ -232,12 +232,7 @@ int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
                             const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T, nu = c->model.nu;
     const int smem = (int)sizeof(float) * T * nu * CL_S;
-    static int smem_attr[64] = {0};
-    int& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_colored_kernel<DIAG, FULL, CEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr = smem;
-    }
+    if (int rc = ensure_smem<mppib_sample_colored_kernel<DIAG, FULL, CEM>>(c->device, smem)) return rc;
     mppib_sample_colored_kernel<DIAG, FULL, CEM><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
                                                                                           plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
                                                                                           DIAG || FULL || CEM ? c->dist : nullptr,
@@ -470,12 +465,7 @@ int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, c
     const int K = c->params.K, n = c->params.T * c->model.nu;
     MPPIB_REQUIRE(n <= MPPIB_HZ_MAX_N, "K1: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, n);
     const int smem = horizon_smem_bytes(n);
-    static int smem_attr[64] = {0};
-    int& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_horizon_kernel<LIB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr = smem;
-    }
+    if (int rc = ensure_smem<mppib_sample_horizon_kernel<LIB>>(c->device, smem)) return rc;
     mppib_sample_horizon_kernel<LIB><<<(K + HZ_S - 1) / HZ_S, 128, smem, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
                                                                               plan_ctr, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
     MPPIB_CHECK_CUDA(cudaGetLastError());
@@ -590,12 +580,7 @@ int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, cons
     MPPIB_REQUIRE(c->anneal == nullptr, "mppib_sample_smooth: annealed MPPI excludes mode smooth");
     MPPIB_REQUIRE(T * nu <= SM_MAX_N, "mppib_sample_smooth: needs T*nu <= %d, got %d", SM_MAX_N, T * nu);
     const int smem = (int)sizeof(float) * T * nu * SM_S;
-    static int smem_attr[64] = {0};
-    int& attr = smem_attr[c->device & 63];
-    if (smem > attr) {
-        MPPIB_CHECK_CUDA(cudaFuncSetAttribute(mppib_sample_smooth_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr = smem;
-    }
+    if (int rc = ensure_smem<mppib_sample_smooth_kernel>(c->device, smem)) return rc;
     mppib_sample_smooth_kernel<<<(K + SM_S - 1) / SM_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
                                                                       k_offset, k_total, U, actions, noise, c->smooth);
     MPPIB_CHECK_CUDA(cudaGetLastError());

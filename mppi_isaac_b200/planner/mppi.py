@@ -26,6 +26,7 @@ import os
 
 import torch
 
+from ..backend import shard_row_floats
 from ..model.blob import ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule
 
 
@@ -311,16 +312,7 @@ class MPPIPlanner:
         self.actions = torch.zeros((T, nu, K), **f32)       # [T][nu][K]
         self.noise = torch.zeros((T, nu, K), **f32)
         self.cost = torch.zeros((T, K), **f32)
-        P = 2 + T * nu * (2 if self.update_cov else 1)      # (beta, eta, W[T*nu]) + M2[T*nu] with update_cov
-        if self.cov_full:
-            P = 2 + T * nu + nu * (nu + 1) // 2               # (beta, eta, W[T*nu]) + C[lower triangle] with cov_type full
-        if self.cov_horizon:
-            P = 2 + T * nu + T * nu * (T * nu + 1) // 2       # (beta, eta, W[n]) + C[lower triangle of n x n] with cov_type horizon
-        if self.cem:
-            E = int(self.backend.params.n_elites)
-            P = (2 * E + E * T * nu + 3) & ~3                 # (S, index)[E] + actions[E][T*nu] of mppi_mode cem, padded to 4
-        if M > 1:
-            P = M * (2 + T * nu)                              # (beta_m, eta_m, W_m[T*nu]) of every mode
+        P = shard_row_floats(self.backend.params, nu)
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
         self._action = torch.zeros((nu,), **f32)
