@@ -262,6 +262,30 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
                      uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row,
                      float* actions, float* noise, void* stream);
 
+/* Which K1 entry samples which mode.  The draw follows the plan's update rule: mode cem, then mode smooth, then, with a registered
+ * distribution and update_cov, cov_horizon, cov_full or the diagonal; update_lambda alone, n_modes > 1 and annealing keep the fixed Sigma.
+ * A refused pair returns an error before anything is launched.
+ *
+ *   handle state                    mppib_sample  _colored  _smooth  mppib_noise_library   mppib_sample_library
+ *   fixed Sigma                     yes           yes       -        yes (coloured by L0)  yes
+ *   update_cov, diagonal            yes           yes       -        yes (white)           yes
+ *   update_cov, cov_full            yes           yes       -        yes (white)           yes
+ *   update_cov, cov_horizon         yes           - (a)     -        yes (white)           yes
+ *   mode cem                        -             yes (b)   -        -                     -
+ *   mode smooth                     -             -         yes (c)  -                     -
+ *   n_modes > 1                     yes (d)       yes (d)   -        yes                   yes (d)
+ *   n_worlds > 1                    yes (e)       yes (e)   -        yes (e)               yes (e)
+ *   annealing schedule registered   yes (f)       yes (f)   -        -                     -
+ *
+ * (a) even with no distribution registered: cov_horizon models the time correlation itself
+ * (b) with the CEM state registered (mppib_set_distribution)
+ * (c) with the smooth state registered (mppib_set_smooth_state); the parameter block already excludes n_worlds > 1 and n_modes > 1
+ * (d) k_total = n_modes * mode_samples
+ * (e) K, k_offset and k_total multiples of n_worlds
+ * (f) registered for the handle's T; the library entries refuse a schedule whatever its T
+ * Every entry also needs its pointers, k_offset + K <= k_total and its size limits: colored T <= 256 and T*nu <= 512, smooth
+ * T*nu <= 512, the noise library 1 <= n_knots <= 32, cov_horizon T*nu <= 256.                                              */
+
 /* K1 (colored variant, `sampling_method: colored`): the white draws z[t][i] of mppib_sample (same counters and transform) are
  * first correlated over the horizon, w[t][i] = sum_{t' <= t} Lt[t][t'] z[t'][i], with Lt[T][T] (caller-owned device memory,
  * row-major, lower) the Cholesky factor of the power-law temporal covariance, then coloured over the controls, clamped and
@@ -399,7 +423,7 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
  *   state    [2 + E + NR + E*NR]  (carry offset, elites valid, S_elite[E], sigma[T][nu], elites[E][T][nu]); offset and flag are 0.0 / 1.0
  * One plan is mppib_shift, then I iterations of K1 -> K2 -> cost -> mppib_reduce (+ mppib_finalize); nothing on the host changes
  * between iterations but plan_idx, so the whole plan is one CUDA graph.
- *   K1     mppib_sample_colored only (white noise: Lt = I): a = clamp(U + sigma (.) w); global rows K_total - 3 - e, e < n_keep, copy
+ *   K1     mppib_sample_colored (white noise: Lt = I): a = clamp(U + sigma (.) w); global rows K_total - 3 - e, e < n_keep, copy
  *          clamp(elites[e][t + off]) with off = the carry offset (the row's own draw where t + off = T) once the elites are valid.
  *   K3     mppib_reduce / mppib_reduce_finalize with x = actions: S_k = sum_t gamma^t cost[t][k] in t order (+0 for -0), key =
  *          (S_k, global index) lexicographically, non-finite S never an elite.  The shard row holds the shard's E smallest keys in
@@ -411,7 +435,7 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
  *          the carry offset to 0; with fewer it leaves U, sigma, the elites and the offset as they are.  Then Savitzky-Golay, clamp,
  *          first action and mirror as in the other modes; stats = (S of the best elite, S of the E-th).
  *   shift  U as in the other modes, sigma <- sigma0 for every t, carry offset <- 1, *plan_ctr += 1.
- * mppib_sample and mppib_sample_library refuse this mode.                                                                   */
+ * The other K1 entries refuse this mode (the K1 table at mppib_sample).                                                     */
 
 /* Smooth MPPI (mode MPPIB_MODE_SMOOTH, `mppi_mode: smooth`, after Kim, Kwon, Yoon, RA-L 2022).  U[T][nu] is the mean of the control
  * DERIVATIVE v; the rolled-out and executed actions are its integral from the last executed action, so with derivative bounds the
@@ -429,8 +453,8 @@ int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream);
  *          a = a_prev: A_t = clamp(fmaf(U'_t, dt, a), u_min, u_max), U'_t := (A_t - a)/dt where that clamp bound, a = A_t; U <- U',
  *          A stored, action_out and the mirror <- A_0, a_prev <- A_0; stats = (beta, eta).  filter_u is refused in this mode.
  *   shift  U as in the other modes (the appended u_init is a derivative: 0 holds the last action), *plan_ctr += 1; A is not shifted.
- * mppib_sample, mppib_sample_colored and the noise-library entry points refuse this mode; reduce and finalize refuse it while no
- * state is registered.  A distribution registered with mppib_set_distribution is ignored in this mode.                      */
+ * The other K1 entries refuse this mode (the K1 table at mppib_sample); reduce and finalize refuse it while no state is
+ * registered.  A distribution registered with mppib_set_distribution is ignored in this mode.                               */
 int32_t mppib_set_smooth_state(MppibHandle h, float* state);
 
 /* Risk-aware MPPI (n_worlds = R > 1, risk_tail = m; modes SIMPLE and MEAN, fixed, diagonal or full Sigma; not cov_horizon).  The K
@@ -453,7 +477,7 @@ int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  * (caller-owned, initialised by the caller; only K4 writes it):
  *   state    [1 + M + T*nu]  (active mode as a float, F[M], U_exec[T][nu])
  *   K1     mppib_sample, mppib_sample_colored and mppib_sample_library draw sample kg around U + m(kg)*T*nu with the counters of the
- *          global index: the columns of mode m equal today's K1 with U := U_m, bit for bit; k_total must be M * Kc
+ *          global index: the columns of mode m equal today's K1 with U := U_m, bit for bit (entries: the K1 table at mppib_sample)
  *   K3     one launch, CTAs (x, m): the shard row is M blocks of SIMPLE's / MEAN's row, [M][2 + T*nu], block m = (beta_m, eta_m, W_m)
  *          over the shard's samples of mode m only (g_m = lambda Sigma^-1 U_m in SIMPLE mode); a mode without a sample on the shard
  *          writes (+inf, 0, 0); a 32-sample tile straddling two modes is read by both modes' CTAs, each masking the other's lanes
@@ -484,8 +508,8 @@ int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  *   shift  as today, then counter := 0
  * With s = 1 every added operation multiplies by 1.0f: a registered schedule of ones with N = 1 reproduces the plain plan bit for bit.
  * Registration refuses N outside 1 .. MPPIB_MAX_ANNEAL and the excluded modes; the library records T there and refuses every launch once
- * mppib_set_params has changed T (or switched to an excluded mode) without a new registration.  mppib_sample_library, mppib_noise_library,
- * mppib_sample_smooth and the cem path refuse a registered schedule.  NULL switches it off: every launch is then today's.             */
+ * mppib_set_params has changed T (or switched to an excluded mode) without a new registration.  The K1 table at mppib_sample lists the
+ * entries that refuse a registered schedule.  NULL switches it off: every launch is then today's.                                    */
 int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations);
 
 #ifdef __cplusplus

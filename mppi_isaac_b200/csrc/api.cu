@@ -266,42 +266,35 @@ int32_t mppib_obs_size(MppibHandle h) { return h ? h->obs_rows : -1; }
 
 int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total, const float* U,
                      const float* prior_row, float* actions, float* noise, void* stream) {
-    MPPIB_REQUIRE(h && U && actions, "mppib_sample: null argument");
-    if (int rc = check_anneal(h, "mppib_sample")) return rc;
-    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
+    if (int rc = k1_admit(h, K1_SAMPLE, U && actions, k_offset, k_total)) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_sample(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, actions, noise, (cudaStream_t)stream);
 }
 
 int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                              const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, void* stream) {
-    MPPIB_REQUIRE(h && U && Lt && actions, "mppib_sample_colored: null argument");
-    if (int rc = check_anneal(h, "mppib_sample_colored")) return rc;
-    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_colored: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
+    if (int rc = k1_admit(h, K1_COLORED, U && Lt && actions, k_offset, k_total)) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_sample_colored(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, (cudaStream_t)stream);
 }
 
 int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                             const float* U, float* actions, float* noise, void* stream) {
-    MPPIB_REQUIRE(h && U && actions, "mppib_sample_smooth: null argument");
-    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_smooth: shard [%u,+%d) exceeds k_total %u", k_offset, h->params.K, k_total);
+    if (int rc = k1_admit(h, K1_SMOOTH, U && actions, k_offset, k_total)) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_sample_smooth(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, actions, noise, (cudaStream_t)stream);
 }
 
 int32_t mppib_noise_library(MppibHandle h, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int32_t n_knots,
                             float* Z, void* stream) {
-    MPPIB_REQUIRE(h && halton_tab && B && Z, "mppib_noise_library: null argument");
-    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_noise_library: shard exceeds k_total");
+    if (int rc = k1_admit(h, K1_NOISE_LIBRARY, halton_tab && B && Z, k_offset, k_total, n_knots)) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_noise_library(h, k_offset, k_total, halton_tab, B, n_knots, Z, (cudaStream_t)stream);
 }
 
 int32_t mppib_sample_library(MppibHandle h, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,
                              float* actions, float* noise, void* stream) {
-    MPPIB_REQUIRE(h && U && Z && actions, "mppib_sample_library: null argument");
-    MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)h->params.K <= (uint64_t)k_total, "mppib_sample_library: shard exceeds k_total");
+    if (int rc = k1_admit(h, K1_SAMPLE_LIBRARY, U && Z && actions, k_offset, k_total)) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_sample_library(h, k_offset, k_total, U, prior_row, Z, actions, noise, (cudaStream_t)stream);
 }

@@ -122,6 +122,19 @@ static inline Rule update_rule(const MppibContext* c) {
     if (c->dist) return RULE_DIST;
     return RULE_PLAIN;
 }
+// The draw K1 makes for the rule: the colour of the white draws (FIXED L0, DIAG / FULL / HORIZON the live adaptive ones, CEM the
+// per-step sigma) or SMOOTH's integrated derivative.  update_lambda alone keeps the fixed Sigma.
+enum Draw { DRAW_FIXED, DRAW_DIAG, DRAW_FULL, DRAW_HORIZON, DRAW_CEM, DRAW_SMOOTH };
+static inline Draw draw_rule(const MppibContext* c) {
+    switch (update_rule(c)) {
+    case RULE_CEM: return DRAW_CEM;
+    case RULE_SMOOTH: return DRAW_SMOOTH;
+    case RULE_HORIZON: return DRAW_HORIZON;
+    case RULE_FULL: return DRAW_FULL;
+    case RULE_DIST: return c->params.update_cov ? DRAW_DIAG : DRAW_FIXED;
+    default: return DRAW_FIXED;
+    }
+}
 // the rule the flags select once a distribution is registered: buffers are sized by it, so that registering a distribution never
 // needs a reallocation
 static inline Rule configured_rule(const MppibParams& p) {
@@ -242,6 +255,12 @@ int ensure_smem(int device, size_t bytes) {
     }
     return 0;
 }
+
+// The K1 entries of the C ABI.  k1_admit (sample.cu) holds which draw each entry samples and which it refuses: the null arguments
+// (args = the entry's pointers are all non-null), the shard range, the annealing schedule, the mode routing, the n_worlds and n_modes
+// shards and the size limits.  Returns 0 or the error of the first refusal; nothing is launched.
+enum K1Entry { K1_SAMPLE, K1_COLORED, K1_SMOOTH, K1_NOISE_LIBRARY, K1_SAMPLE_LIBRARY };
+int k1_admit(const MppibContext* c, K1Entry e, bool args, uint32_t k_offset, uint32_t k_total, int n_knots = 1);
 
 // kernel launchers (defined in the .cu files)
 int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,

@@ -32,28 +32,63 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
     z0 = r * c; z1 = r * s;
 }
 
-// The control-space colour, clamp and store of one (t, k) of every Philox K1: noise_j = sum_{i <= j} L0[j][i] z_i with the fixed
-// Sigma's Cholesky factor, summed from i = 0 upwards; DIAG (adaptive MPPI with update_cov): sqrt(cov_j) z_j with cov = dist[1..nu],
-// the live diagonal covariance; FULL (update_cov with cov_full): the live lower Cholesky factor L = dist[1 + nu*nu ..] in the same
-// order.  a = clamp(U + noise) with the null / prior rows, noise := a - U.  Annealed MPPI (srow = the s row of the iteration, fixed Sigma
-// only): noise_j := s[t] noise_j, one rounded multiplication, so a schedule of ones changes no bit.
-template <bool DIAG, bool FULL>
-__device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int t, int k, bool is_null,
-                                                   bool is_prior, const float* __restrict__ U, const float* __restrict__ prior_row,
-                                                   float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist,
-                                                   const float* __restrict__ srow = nullptr) {
-    const int K = p.K;
+// The Philox key of a plan: (seed_lo, seed_hi ^ plan_lo), with plan_hi the last counter word; plan = plan_idx + *plan_ctr (nullable),
+// so that a captured graph draws fresh noise on every replay.
+struct PhiloxKey { uint32_t k0, k1, plan_hi; };
+__device__ __forceinline__ PhiloxKey philox_key(uint32_t key0, uint32_t seed_hi, uint64_t plan_idx, const uint32_t* __restrict__ plan_ctr) {
+    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
+    return {key0, seed_hi ^ (uint32_t)plan, (uint32_t)(plan >> 32)};
+}
+// the white draws z[0..4) of controls 4*blk .. 4*blk + 3 of control sample kc at step t
+__device__ __forceinline__ void philox_gauss4(const PhiloxKey& key, uint32_t kc, int t, int blk, float* z) {
+    const uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, key.plan_hi), key.k0, key.k1);
+    box_muller(r.x, r.y, z[0], z[1]);
+    box_muller(r.z, r.w, z[2], z[3]);
+}
+
+// The special rows of global sample kg, tested on its control sample (n_worlds keying): the last control sample of the k_total is the
+// null action when enabled, the one before it takes prior_row when one is given.
+struct SpecialRows { bool null, prior; };
+__device__ __forceinline__ SpecialRows special_rows(const MppibParams& p, uint32_t kg, uint32_t k_total, bool has_prior) {
+    const uint32_t kc = sample_control(kg, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
+    return {p.sample_null_action && kc == kc_total - 1, has_prior && kc == kc_total - 2};
+}
+
+// The tail of every K1 but smooth at (t, j) of sample k: a = U + noise (0 on the null row) clamped to [u_min, u_max], prior_row on the
+// prior row, stored with noise := a - u.
+__device__ __forceinline__ void clamp_store(const MppibParams& p, int nu, int t, int j, int k, float a, float u, SpecialRows rows,
+                                            const float* __restrict__ prior_row, float* __restrict__ actions, float* __restrict__ noise) {
+    if (rows.null) a = 0.f;
+    a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+    if (rows.prior) a = prior_row[t * nu + j];
+    const size_t idx = ((size_t)t * nu + j) * p.K + k;
+    actions[idx] = a;
+    if (noise) noise[idx] = a - u;
+}
+
+// The control-space colour of one (t, k) in front of clamp_store.  FIXED: noise_j = sum_{i <= j} L0[j][i] z_i with the fixed Sigma's
+// Cholesky factor, summed from i = 0 upwards; DIAG (adaptive MPPI with update_cov): sqrt(cov_j) z_j with cov = dist[1..nu], the live
+// diagonal covariance; FULL (update_cov with cov_full): the live lower Cholesky factor L = dist[1 + nu*nu ..] in the same order.  LIB: z
+// is a column of the noise library, which mppib_noise_library has coloured by L0 already (FIXED) or left white (DIAG / FULL).
+// Annealed MPPI (srow = the s row of the iteration, FIXED only): noise_j := s[t] noise_j, one rounded multiplication, so a schedule of
+// ones changes no bit.
+template <Draw D, bool LIB = false>
+__device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int t, int k, SpecialRows rows,
+                                                   const float* __restrict__ U, const float* __restrict__ prior_row, float* __restrict__ actions,
+                                                   float* __restrict__ noise, const float* __restrict__ dist, const float* __restrict__ srow) {
 #pragma unroll
     for (int j = 0; j < MPPIB_MAX_NU; ++j) {
         if (j >= nu) break;
         float n = 0.f;
-        if (DIAG) {
+        if constexpr (D == DRAW_DIAG) {
             n = sqrtf(dist[1 + j]) * z[j];
-        } else if (FULL) {
+        } else if constexpr (D == DRAW_FULL) {
             const float* Ld = dist + 1 + nu * nu;
 #pragma unroll
             for (int i = 0; i < MPPIB_MAX_NU; ++i)
                 if (i <= j) n += Ld[j * nu + i] * z[i];
+        } else if constexpr (LIB) {
+            n = z[j];
         } else {
 #pragma unroll
             for (int i = 0; i < MPPIB_MAX_NU; ++i)
@@ -61,80 +96,67 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
             if (srow) n = __fmul_rn(srow[t], n);
         }
         const float u = U[t * nu + j];
-        float a = u + n;
-        if (is_null) a = 0.f;
-        a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-        if (is_prior) a = prior_row[t * nu + j];
-        const size_t idx = ((size_t)t * nu + j) * K + k;
-        actions[idx] = a;
-        if (noise) noise[idx] = a - u;
+        clamp_store(p, nu, t, j, k, u + n, u, rows, prior_row, actions, noise);
     }
 }
 
-// DIAG / FULL: the adaptive colours of colour_clamp_store.  One thread per (t, k), Philox counter (global sample, t, block); with
-// n_worlds = R > 1 the control sample kg / R replaces the global sample in the counter and in the null / prior tests.  With n_modes > 1
-// the sample is drawn around its mode's sequence (sample_mode), the counter stays the global sample; n_modes > 1 excludes update_cov,
-// so only the fixed-Sigma instantiations (not DIAG / FULL) carry the mode offset.  anneal (annealed MPPI, fixed Sigma only; nullable): the
+// One thread per (t, k) for the per-step colours D = FIXED, DIAG, FULL.  The white draws are the Philox draws of counter (global
+// sample, t, block) -- with n_worlds = R > 1 the control sample kg / R replaces the global sample -- or, LIB, column k of the noise
+// library Z.  With n_modes > 1 the sample is drawn around its mode's sequence (sample_mode), the counter stays the global sample;
+// n_modes > 1 excludes update_cov, so only FIXED carries the mode offset.  anneal (annealed MPPI, FIXED only; nullable): the
 // registered schedule of anneal_n iterations, whose s row scales the noise.
-template <bool DIAG, bool FULL = false>
+template <Draw D, bool LIB>
 __global__ void __launch_bounds__(128)
 mppib_sample_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
-              const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U, const float* __restrict__ prior_row,
-              float* __restrict__ actions, float* __restrict__ noise, const float* __restrict__ dist, const float* __restrict__ anneal, int anneal_n) {
+                    const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
+                    const float* __restrict__ prior_row, const float* __restrict__ Z, float* __restrict__ actions, float* __restrict__ noise,
+                    const float* __restrict__ dist, const float* __restrict__ anneal, int anneal_n) {
     const int K = p.K;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     const int t = blockIdx.y;
     if (k >= K) return;
-    const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds), kc_last = sample_control(k_total - 1, p.n_worlds);
-    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
-    const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
+    const uint32_t kg = k_offset + (uint32_t)k;
     float z[MPPIB_MAX_NU];
+    if constexpr (LIB) {
 #pragma unroll
-    for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk) {
-        if (blk * 4 < nu) {
-            uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
-            box_muller(r.x, r.y, z[4 * blk], z[4 * blk + 1]);
-            box_muller(r.z, r.w, z[4 * blk + 2], z[4 * blk + 3]);
-        }
+        for (int i = 0; i < MPPIB_MAX_NU; ++i) z[i] = i < nu ? Z[((size_t)t * nu + i) * K + k] : 0.f;
+    } else {
+        const PhiloxKey key = philox_key(key0, seed_hi, plan_idx, plan_ctr);
+        const uint32_t kc = sample_control(kg, p.n_worlds);
+#pragma unroll
+        for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk)
+            if (blk * 4 < nu) philox_gauss4(key, kc, t, blk, z + 4 * blk);
     }
-    const bool is_null = p.sample_null_action && kc == kc_last;
-    const bool is_prior = prior_row != nullptr && kc + 1 == kc_last;
     const float* Um = U;
-    if constexpr (!DIAG && !FULL) Um += (size_t)sample_mode(k_offset + (uint32_t)k, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
-    const float* srow = (!DIAG && !FULL && anneal) ? anneal_row(anneal, anneal_n, p.T, false) : nullptr;
-    colour_clamp_store<DIAG, FULL>(p, nu, z, t, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
+    if constexpr (D == DRAW_FIXED) Um += (size_t)sample_mode(kg, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
+    const float* srow = (D == DRAW_FIXED && anneal) ? anneal_row(anneal, anneal_n, p.T, false) : nullptr;
+    colour_clamp_store<D, LIB>(p, nu, z, t, k, special_rows(p, kg, k_total, prior_row != nullptr), Um, prior_row, actions, noise, dist, srow);
 }
 
 // The white Philox draws of a tile of S samples [k0, k0 + S) to shared memory, zs[(t*nu + i) * S + sample]: the draws of the
 // fixed-Sigma kernel (counter (control sample of n_worlds = R, t, block)), spread over the CTA.
 template <int S>
-__device__ __forceinline__ void stage_white_tile(float* zs, int T, int nu, int k0, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
-                                                 const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, int R) {
-    const uint64_t plan = plan_idx + (plan_ctr ? (uint64_t)*plan_ctr : 0ull);
-    const uint32_t key1 = seed_hi ^ (uint32_t)plan, plan_hi = (uint32_t)(plan >> 32);
+__device__ __forceinline__ void stage_white_tile(float* zs, int T, int nu, int k0, const PhiloxKey& key, uint32_t k_offset, int R) {
     const int nblk = (nu + 3) / 4;
     for (int idx = threadIdx.x; idx < S * T * nblk; idx += blockDim.x) {
         const int sl = idx % S, rest = idx / S, blk = rest % nblk, t = rest / nblk;
-        const uint32_t kc = sample_control(k_offset + (uint32_t)(k0 + sl), R);
-        const uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, plan_hi), key0, key1);
         float z[4];
-        box_muller(r.x, r.y, z[0], z[1]);
-        box_muller(r.z, r.w, z[2], z[3]);
+        philox_gauss4(key, sample_control(k_offset + (uint32_t)(k0 + sl), R), t, blk, z);
 #pragma unroll
         for (int e = 0; e < 4; ++e)
             if (4 * blk + e < nu) zs[(t * nu + 4 * blk + e) * S + sl] = z[e];
     }
 }
 
-// CEM (mppi_mode: cem): the colour, clamp and store of one (t, k) with the per-step diagonal sigma[t][j] of the CEM state
-// (include/mppib.h): a = clamp(U + sigma (.) w), the product rounded on its own as colour_clamp_store rounds L0[j][j] z_j, so a diagonal
-// Sigma with sigma = sigma0 draws what colour_clamp_store draws, bit for bit.  Once the state holds elites, global rows
-// k_total - 3 - e (e < n_keep) copy clamp(elites[e][t + off]), off = the state's carry offset; a row whose t + off = T keeps its draw.
+// CEM (mppi_mode: cem): the colour of one (t, k) in front of clamp_store with the per-step diagonal sigma[t][j] of the CEM state
+// (include/mppib.h): a = U + sigma (.) w, the product rounded on its own as the FIXED colour rounds L0[j][j] z_j, so a diagonal Sigma
+// with sigma = sigma0 draws what FIXED draws, bit for bit.  Once the state holds elites, global rows k_total - 3 - e (e < n_keep) take
+// elites[e][t + off] instead, off = the state's carry offset; a row whose t + off = T keeps its draw.
 __device__ __forceinline__ void cem_clamp_store(const MppibParams& p, int nu, const float (&w)[MPPIB_MAX_NU], int t, int k, uint32_t kg,
-                                                uint32_t k_total, bool is_null, bool is_prior, const float* __restrict__ U,
+                                                uint32_t k_total, SpecialRows rows, const float* __restrict__ U,
                                                 const float* __restrict__ prior_row, float* __restrict__ actions, float* __restrict__ noise,
                                                 const float* __restrict__ state) {
-    const int K = p.K, NR = p.T * nu;
+    const int NR = p.T * nu;
     const float* sig = state + 2 + p.n_elites;
     const float* el = sig + NR;
     const uint32_t e = k_total - 3u - kg;                                     // carried row e when kg = k_total - 3 - e
@@ -144,20 +166,15 @@ __device__ __forceinline__ void cem_clamp_store(const MppibParams& p, int nu, co
     for (int j = 0; j < MPPIB_MAX_NU; ++j) {
         if (j >= nu) break;
         const float u = U[t * nu + j];
-        float a = carried ? el[(size_t)e * NR + ts * nu + j] : u + __fmul_rn(sig[t * nu + j], w[j]);
-        if (is_null) a = 0.f;
-        a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-        if (is_prior) a = prior_row[t * nu + j];
-        const size_t idx = ((size_t)t * nu + j) * K + k;
-        actions[idx] = a;
-        if (noise) noise[idx] = a - u;
+        const float a = carried ? el[(size_t)e * NR + ts * nu + j] : u + __fmul_rn(sig[t * nu + j], w[j]);
+        clamp_store(p, nu, t, j, k, a, u, rows, prior_row, actions, noise);
     }
 }
 
 // COLORED (sampling_method: colored): time-correlated noise w[t][i] = sum_{t' <= t} L_b[t][t'] z[t'][i] over the white draws of
-// the fixed-Sigma kernel, with L_b = Lt[T][T] the lower Cholesky factor of the power-law temporal covariance, then the control-space
-// colour, clamp and store of colour_clamp_store (fixed L0, or DIAG / FULL the live adaptive ones).  A CTA of 128 threads owns a tile
-// of CL_S = 32 samples, lane = sample: the tile's white draws go to shared memory, then warp w takes the row pairs (t, T-1-t),
+// the fixed-Sigma kernel, with L_b = Lt[T][T] the lower Cholesky factor of the power-law temporal covariance, then the colour step
+// of D: colour_clamp_store (FIXED L0, or DIAG / FULL the live adaptive ones) or cem_clamp_store (CEM).  A CTA of 128 threads owns a
+// tile of CL_S = 32 samples, lane = sample: the tile's white draws go to shared memory, then warp w takes the row pairs (t, T-1-t),
 // t = w, w + 4, ..., so that every warp sums about the same number of terms and every shared-memory load of z feeds two rows.  The
 // rows of L_b are read with warp-uniform loads (one L1 line per row segment, shared by all CTAs).  Both sums run in a fixed order
 // (t' and i from 0 upwards), so a sample's noise depends only on its global index; with L_b = I the temporal sum adds only exact
@@ -166,10 +183,10 @@ constexpr int CL_S = 32;            // samples per CTA
 constexpr int CL_MAX_T = 256;
 constexpr int CL_MAX_N = 512;       // T*nu: the tile's draws take CL_MAX_N * CL_S * 4 = 64 KB of shared memory
 
-// The fixed-Sigma instantiation asks for 8 CTAs per SM: with the annealing scale it takes 64 registers (78 unbounded, 63 without the
+// The FIXED instantiation asks for 8 CTAs per SM: with the annealing scale it takes 64 registers (78 unbounded, 63 without the
 // scale) and spills nothing; 0 leaves the other instantiations as the compiler allocates them.
-template <bool DIAG, bool FULL, bool CEM = false>
-__global__ void __launch_bounds__(128, (DIAG || FULL || CEM) ? 0 : 8)
+template <Draw D>
+__global__ void __launch_bounds__(128, D == DRAW_FIXED ? 8 : 0)
 mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
                             const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
                             const float* __restrict__ prior_row, const float* __restrict__ Lt, float* __restrict__ actions,
@@ -178,15 +195,13 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
     const int K = p.K, T = p.T;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int k0 = blockIdx.x * CL_S, k = k0 + lane;
-    stage_white_tile<CL_S>(cs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, p.n_worlds);
-    __syncthreads();
     const uint32_t kg = k_offset + (uint32_t)k;
-    const uint32_t kc = sample_control(kg, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
-    const bool is_null = p.sample_null_action && kc == kc_total - 1;
-    const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
+    const SpecialRows rows = special_rows(p, kg, k_total, prior_row != nullptr);
+    stage_white_tile<CL_S>(cs, T, nu, k0, philox_key(key0, seed_hi, plan_idx, plan_ctr), k_offset, p.n_worlds);
+    __syncthreads();
     const float* Um = U;
-    if constexpr (!DIAG && !FULL && !CEM) Um += (size_t)sample_mode(kg, p) * (T * nu);   // n_modes > 1 (fixed Sigma only)
-    const float* srow = (!DIAG && !FULL && !CEM && anneal) ? anneal_row(anneal, anneal_n, T, false) : nullptr;   // annealed MPPI
+    if constexpr (D == DRAW_FIXED) Um += (size_t)sample_mode(kg, p) * (T * nu);   // n_modes > 1 (fixed Sigma only)
+    const float* srow = (D == DRAW_FIXED && anneal) ? anneal_row(anneal, anneal_n, T, false) : nullptr;   // annealed MPPI
     const float* zl = cs + lane;
     for (int tl = warp; tl < (T + 1) / 2; tl += 4) {
         const int th = T - 1 - tl;                                            // th >= tl; th == tl for the middle row of an odd T
@@ -217,26 +232,26 @@ mppib_sample_colored_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             }
         }
         if (k >= K) continue;
-        if constexpr (CEM) {
-            cem_clamp_store(p, nu, wl, tl, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
-            if (th != tl) cem_clamp_store(p, nu, wh, th, k, kg, k_total, is_null, is_prior, U, prior_row, actions, noise, dist);
+        if constexpr (D == DRAW_CEM) {
+            cem_clamp_store(p, nu, wl, tl, k, kg, k_total, rows, U, prior_row, actions, noise, dist);
+            if (th != tl) cem_clamp_store(p, nu, wh, th, k, kg, k_total, rows, U, prior_row, actions, noise, dist);
         } else {
-            colour_clamp_store<DIAG, FULL>(p, nu, wl, tl, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
-            if (th != tl) colour_clamp_store<DIAG, FULL>(p, nu, wh, th, k, is_null, is_prior, Um, prior_row, actions, noise, dist, srow);
+            colour_clamp_store<D>(p, nu, wl, tl, k, rows, Um, prior_row, actions, noise, dist, srow);
+            if (th != tl) colour_clamp_store<D>(p, nu, wh, th, k, rows, Um, prior_row, actions, noise, dist, srow);
         }
     }
 }
 
-template <bool DIAG, bool FULL, bool CEM = false>
+template <Draw D>
 int launch_sample_colored_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                             const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, T = c->params.T, nu = c->model.nu;
     const int smem = (int)sizeof(float) * T * nu * CL_S;
-    if (int rc = ensure_smem<mppib_sample_colored_kernel<DIAG, FULL, CEM>>(c->device, smem)) return rc;
-    mppib_sample_colored_kernel<DIAG, FULL, CEM><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
-                                                                                          plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise,
-                                                                                          DIAG || FULL || CEM ? c->dist : nullptr,
-                                                                                          DIAG || FULL || CEM ? nullptr : c->anneal, c->anneal_n);
+    if (int rc = ensure_smem<mppib_sample_colored_kernel<D>>(c->device, smem)) return rc;
+    mppib_sample_colored_kernel<D><<<(K + CL_S - 1) / CL_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
+                                                                            k_offset, k_total, U, prior_row, Lt, actions, noise,
+                                                                            D == DRAW_FIXED ? nullptr : c->dist,
+                                                                            D == DRAW_FIXED ? c->anneal : nullptr, c->anneal_n);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -258,10 +273,10 @@ mppib_sample_smooth_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     const int K = p.K, T = p.T;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int k0 = blockIdx.x * SM_S, k = k0 + lane;
-    stage_white_tile<SM_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, 1);
+    stage_white_tile<SM_S>(zs, T, nu, k0, philox_key(key0, seed_hi, plan_idx, plan_ctr), k_offset, 1);
     __syncthreads();
     if (k >= K) return;
-    const bool is_null = p.sample_null_action && k_offset + (uint32_t)k == k_total - 1;
+    const bool is_null = special_rows(p, k_offset + (uint32_t)k, k_total, false).null;
     const float dt = p.dt;
     const float* zl = zs + lane;
     for (int j = warp; j < nu; j += 4) {
@@ -299,8 +314,8 @@ __device__ __forceinline__ float halton(uint32_t index, uint32_t base, uint32_t 
 
 constexpr int MAX_KNOTS = 32;
 
-// one thread per sample k: Gaussian knots (n_knots x nu) -> coloured -> spline-interpolated to T points.  WHITE (adaptive MPPI with
-// update_cov): identity colour, the library sampler scales by the live sqrt(cov) (or colours by the live L, cov_full) on every plan.
+// one thread per sample k: Gaussian knots (n_knots x nu) -> coloured -> spline-interpolated to T points.  WHITE (draws DIAG, FULL
+// and HORIZON of adaptive MPPI with update_cov): identity colour, the library sampler colours by the live distribution on every plan.
 template <bool WHITE>
 __global__ void __launch_bounds__(128)
 mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total,
@@ -309,7 +324,7 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= K) return;
     const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds);
-    const bool null_row = p.sample_null_action && kc == sample_control(k_total, p.n_worlds) - 1;
+    const bool null_row = special_rows(p, k_offset + (uint32_t)k, k_total, false).null;
     const int nd = n_knots * nu;
     for (int j = 0; j < nu; ++j) {
         // coloured knots of control dimension j:  c[n] = sum_i L[j][i] z[n][i]
@@ -332,62 +347,13 @@ mppib_noise_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     }
 }
 
-// DIAG (adaptive MPPI with update_cov): Z is the white library, scaled by the live sqrt(cov_j) = sqrt(dist[1 + j]).
-// FULL (update_cov with cov_full): Z is the white library, coloured by the live L = dist[1 + nu*nu ..]: a = clamp(U + L Z[t][:, k]).
-template <bool DIAG, bool FULL = false>
-__global__ void __launch_bounds__(128)
-mppib_sample_library_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
-                            const float* __restrict__ prior_row, const float* __restrict__ Z, float* __restrict__ actions,
-                            float* __restrict__ noise, const float* __restrict__ dist) {
-    const int K = p.K;
-    const int k = blockIdx.x * blockDim.x + threadIdx.x, t = blockIdx.y;
-    if (k >= K) return;
-    const uint32_t kc = sample_control(k_offset + (uint32_t)k, p.n_worlds), kc_total = sample_control(k_total, p.n_worlds);
-    const bool is_null = p.sample_null_action && kc == kc_total - 1;
-    const bool is_prior = prior_row != nullptr && kc == kc_total - 2;
-    if constexpr (!DIAG && !FULL) U += (size_t)sample_mode(k_offset + (uint32_t)k, p) * (p.T * nu);   // n_modes > 1 (fixed Sigma only)
-    if constexpr (FULL) {
-        const float* Ld = dist + 1 + nu * nu;
-        float zc[MPPIB_MAX_NU];
-#pragma unroll
-        for (int i = 0; i < MPPIB_MAX_NU; ++i) zc[i] = i < nu ? Z[((size_t)t * nu + i) * K + k] : 0.f;
-#pragma unroll
-        for (int j = 0; j < MPPIB_MAX_NU; ++j) {
-            if (j >= nu) break;
-            float n = 0.f;
-#pragma unroll
-            for (int i = 0; i < MPPIB_MAX_NU; ++i)
-                if (i <= j) n += Ld[j * nu + i] * zc[i];
-            const size_t idx = ((size_t)t * nu + j) * K + k;
-            const float u = U[t * nu + j];
-            float a = u + n;
-            if (is_null) a = 0.f;
-            a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-            if (is_prior) a = prior_row[t * nu + j];
-            actions[idx] = a;
-            if (noise) noise[idx] = a - u;
-        }
-    } else {
-        for (int j = 0; j < nu; ++j) {
-            const size_t idx = ((size_t)t * nu + j) * K + k;
-            const float u = U[t * nu + j];
-            float a = u + (DIAG ? sqrtf(dist[1 + j]) * Z[idx] : Z[idx]);
-            if (is_null) a = 0.f;
-            a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-            if (is_prior) a = prior_row[t * nu + j];
-            actions[idx] = a;
-            if (noise) noise[idx] = a - u;
-        }
-    }
-}
-
 // HORIZON (update_cov with cov_horizon, n = T*nu <= 256): noise = L_H z over the whole n-vector of a sample, with L_H =
 // dist[1 + n*n ..] the live lower Cholesky factor of Sigma_H, rows and columns ordered (t, j) like U.  A CTA of 128 threads owns a
 // tile of HZ_S = 64 samples: the white draws of the tile go to shared memory first -- the Philox draws of the fixed-Sigma kernel
 // (counter (global sample, t, block)) or, LIB, the white library Z -- then L_H is staged 32 rows at a time, transposed, and every
 // warp multiplies 8 of those rows with the tile: lane = samples lane and lane + 32, an 8 x 2 register block, two broadcast LDS.128
 // of L_H and two LDS of z per 16 FFMA.  The sum over columns runs from 0 upwards (the zeros above the diagonal add nothing), so a
-// sample's noise depends only on its global index.  Clamping and the null / prior rows are those of the other K1 variants.
+// sample's noise depends only on its global index.  Then clamp_store, as in the other K1 variants.
 constexpr int HZ_S = 64;        // samples per CTA
 constexpr int HZ_LP = 36;       // padded row of the transposed L_H panel (16-byte aligned, 4-way store conflicts at most)
 
@@ -411,7 +377,7 @@ mppib_sample_horizon_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             zs[idx] = k < K ? Z[(size_t)r * K + k] : 0.f;
         }
     } else {
-        stage_white_tile<HZ_S>(zs, T, nu, k0, key0, seed_hi, plan_idx, plan_ctr, k_offset, 1);
+        stage_white_tile<HZ_S>(zs, T, nu, k0, philox_key(key0, seed_hi, plan_idx, plan_ctr), k_offset, 1);
     }
     const float* Ld = dist + 1 + (size_t)n * n;
     for (int r0 = 0; r0 < n; r0 += 32) {
@@ -446,14 +412,8 @@ mppib_sample_horizon_kernel(const __grid_constant__ MppibParams p, int nu, uint3
             for (int h = 0; h < 2; ++h) {
                 const int k = k0 + lane + 32 * h;
                 if (k >= K) continue;
-                const uint32_t kg = k_offset + (uint32_t)k;
-                float a = u + (h ? acc1[i] : acc0[i]);
-                if (p.sample_null_action && kg == k_total - 1) a = 0.f;
-                a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
-                if (prior_row != nullptr && kg == k_total - 2) a = prior_row[t * nu + j];
-                const size_t idx = (size_t)r * K + k;
-                actions[idx] = a;
-                if (noise) noise[idx] = a - u;
+                clamp_store(p, nu, t, j, k, u + (h ? acc1[i] : acc0[i]), u, special_rows(p, k_offset + (uint32_t)k, k_total, prior_row != nullptr),
+                            prior_row, actions, noise);
             }
         }
     }
@@ -463,11 +423,37 @@ template <bool LIB>
 int launch_sample_horizon_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                             const float* U, const float* prior_row, const float* Z, float* actions, float* noise, cudaStream_t s) {
     const int K = c->params.K, n = c->params.T * c->model.nu;
-    MPPIB_REQUIRE(n <= MPPIB_HZ_MAX_N, "K1: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, n);
     const int smem = horizon_smem_bytes(n);
     if (int rc = ensure_smem<mppib_sample_horizon_kernel<LIB>>(c->device, smem)) return rc;
     mppib_sample_horizon_kernel<LIB><<<(K + HZ_S - 1) / HZ_S, 128, smem, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx,
                                                                               plan_ctr, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// mppib_sample (LIB = false: the Philox draws) and mppib_sample_library (LIB: the draws are the library Z) for the handle's draw;
+// k1_admit has refused CEM and SMOOTH.
+template <bool LIB>
+int launch_sample_t(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                    const float* U, const float* prior_row, const float* Z, float* actions, float* noise, cudaStream_t s) {
+    const int nu = c->model.nu;
+    const uint32_t key0 = (uint32_t)seed, seed_hi = (uint32_t)(seed >> 32);
+    const dim3 grid((c->params.K + 127) / 128, c->params.T);
+    switch (draw_rule(c)) {
+    case DRAW_HORIZON:
+        return launch_sample_horizon_t<LIB>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Z, actions, noise, s);
+    case DRAW_FULL:
+        mppib_sample_kernel<DRAW_FULL, LIB><<<grid, 128, 0, s>>>(c->params, nu, key0, seed_hi, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Z,
+                                                                 actions, noise, c->dist, nullptr, 0);
+        break;
+    case DRAW_DIAG:
+        mppib_sample_kernel<DRAW_DIAG, LIB><<<grid, 128, 0, s>>>(c->params, nu, key0, seed_hi, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Z,
+                                                                 actions, noise, c->dist, nullptr, 0);
+        break;
+    default:
+        mppib_sample_kernel<DRAW_FIXED, LIB><<<grid, 128, 0, s>>>(c->params, nu, key0, seed_hi, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Z,
+                                                                  actions, noise, nullptr, c->anneal, c->anneal_n);
+    }
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -492,16 +478,61 @@ int check_modes_total(const MppibContext* c, const char* who, uint32_t k_total) 
 
 }  // namespace
 
+// Which K1 entry samples which draw (the table of include/mppib.h), checked on the host before any launch:
+//   mppib_sample          FIXED, DIAG, FULL, HORIZON
+//   mppib_sample_colored  FIXED, DIAG, FULL, CEM (with its state); not cov_horizon, even with no distribution registered
+//   mppib_sample_smooth   SMOOTH (with its state); validate excludes n_worlds > 1 and n_modes > 1 from it
+//   mppib_noise_library   FIXED, DIAG, FULL, HORIZON: the library is white exactly for DIAG, FULL and HORIZON
+//   mppib_sample_library  FIXED, DIAG, FULL, HORIZON
+// A registered annealing schedule goes through check_anneal in the two Philox entries; the library entries refuse one whatever its T.
+// args: the entry's required pointers are all non-null.
+int k1_admit(const MppibContext* c, K1Entry e, bool args, uint32_t k_offset, uint32_t k_total, int n_knots) {
+    static const char* const names[] = {"mppib_sample", "mppib_sample_colored", "mppib_sample_smooth", "mppib_noise_library", "mppib_sample_library"};
+    const char* who = names[e];
+    const bool lib = e == K1_NOISE_LIBRARY || e == K1_SAMPLE_LIBRARY;
+    MPPIB_REQUIRE(c && args, "%s: null argument", who);
+    if (e == K1_SAMPLE || e == K1_COLORED)
+        if (int rc = check_anneal(c, who)) return rc;
+    const bool in_range = (uint64_t)k_offset + (uint64_t)c->params.K <= (uint64_t)k_total;
+    if (lib) MPPIB_REQUIRE(in_range, "%s: shard exceeds k_total", who);
+    else MPPIB_REQUIRE(in_range, "%s: shard [%u,+%d) exceeds k_total %u", who, k_offset, c->params.K, k_total);
+    const int T = c->params.T, nu = c->model.nu;
+    const Draw d = draw_rule(c);
+    if (e == K1_SMOOTH) {
+        MPPIB_REQUIRE(d == DRAW_SMOOTH, "%s: needs mode smooth (MPPIB_MODE_SMOOTH), the handle has mode %d", who, c->params.mode);
+        MPPIB_REQUIRE(c->smooth != nullptr, "%s: no smooth state registered (mppib_set_smooth_state)", who);
+        MPPIB_REQUIRE(c->anneal == nullptr, "%s: annealed MPPI excludes mode smooth", who);
+        MPPIB_REQUIRE(T * nu <= SM_MAX_N, "%s: needs T*nu <= %d, got %d", who, SM_MAX_N, T * nu);
+        return 0;
+    }
+    MPPIB_REQUIRE(d != DRAW_CEM || e == K1_COLORED, "%s: mode cem samples through mppib_sample_colored%s", who,
+                  e == K1_SAMPLE ? " (white noise: Lt = I)" : "");
+    MPPIB_REQUIRE(d != DRAW_SMOOTH, "%s: mode smooth samples through mppib_sample_smooth", who);
+    if (lib)
+        MPPIB_REQUIRE(c->anneal == nullptr, "%s: annealed MPPI excludes the noise library (every iteration would reuse the same directions); "
+                      "register no schedule (mppib_set_anneal(h, NULL, 0))", who);
+    if (int rc = check_risk_shard(c, who, k_offset, k_total)) return rc;
+    if (e == K1_NOISE_LIBRARY) {
+        MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "%s: n_knots = %d out of range [1, %d]", who, n_knots, MAX_KNOTS);
+        return 0;
+    }
+    if (int rc = check_modes_total(c, who, k_total)) return rc;
+    if (e == K1_COLORED) {
+        MPPIB_REQUIRE(!c->params.cov_horizon, "%s: cov_horizon already models the time correlation; colored noise excludes it", who);
+        MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "%s: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", who, CL_MAX_T, CL_MAX_N, T,
+                      T * nu);
+        MPPIB_REQUIRE(d != DRAW_CEM || c->dist != nullptr, "%s: mppi_mode cem needs its state registered with mppib_set_distribution", who);
+        return 0;
+    }
+    MPPIB_REQUIRE(d != DRAW_HORIZON || T * nu <= MPPIB_HZ_MAX_N, "K1: cov_horizon needs n = T*nu <= %d, got %d", MPPIB_HZ_MAX_N, T * nu);
+    return 0;
+}
+
 int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const int32_t* halton_tab, const float* B, int n_knots,
                          float* Z, cudaStream_t s) {
-    MPPIB_REQUIRE(!cem_mode(c), "mppib_noise_library: mode cem samples through mppib_sample_colored");
-    MPPIB_REQUIRE(!smooth_mode(c), "mppib_noise_library: mode smooth samples through mppib_sample_smooth");
-    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_noise_library: annealed MPPI excludes the noise library (every iteration would reuse the same directions); "
-                  "register no schedule (mppib_set_anneal(h, NULL, 0))");
-    if (int rc = check_risk_shard(c, "mppib_noise_library", k_offset, k_total)) return rc;
-    MPPIB_REQUIRE(n_knots >= 1 && n_knots <= MAX_KNOTS, "mppib_noise_library: n_knots = %d out of range [1, %d]", n_knots, MAX_KNOTS);
     const int K = c->params.K;
-    if (adaptive_cov(c))
+    const Draw d = draw_rule(c);
+    if (d == DRAW_DIAG || d == DRAW_FULL || d == DRAW_HORIZON)
         mppib_noise_library_kernel<true><<<(K + 127) / 128, 128, 0, s>>>(c->params, c->model.nu, k_offset, k_total, halton_tab, B, n_knots, Z);
     else
         mppib_noise_library_kernel<false><<<(K + 127) / 128, 128, 0, s>>>(c->params, c->model.nu, k_offset, k_total, halton_tab, B, n_knots, Z);
@@ -511,75 +542,28 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
 
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,
                           float* actions, float* noise, cudaStream_t s) {
-    MPPIB_REQUIRE(!cem_mode(c), "mppib_sample_library: mode cem samples through mppib_sample_colored");
-    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_library: mode smooth samples through mppib_sample_smooth");
-    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_sample_library: annealed MPPI excludes the noise library (every iteration would reuse the same directions); "
-                  "register no schedule (mppib_set_anneal(h, NULL, 0))");
-    if (int rc = check_risk_shard(c, "mppib_sample_library", k_offset, k_total)) return rc;
-    if (int rc = check_modes_total(c, "mppib_sample_library", k_total)) return rc;
-    const int K = c->params.K, T = c->params.T;
-    dim3 block(128), grid((K + 127) / 128, T);
-    if (adaptive_horizon(c))
-        return launch_sample_horizon_t<true>(c, 0, 0, nullptr, k_offset, k_total, U, prior_row, Z, actions, noise, s);
-    if (adaptive_full(c))
-        mppib_sample_library_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
-    else if (adaptive_cov(c))
-        mppib_sample_library_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, c->dist);
-    else
-        mppib_sample_library_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, k_offset, k_total, U, prior_row, Z, actions, noise, nullptr);
-    MPPIB_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return launch_sample_t<true>(c, 0, 0, nullptr, k_offset, k_total, U, prior_row, Z, actions, noise, s);
 }
 
 int launch_sample(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                   const float* U, const float* prior_row, float* actions, float* noise, cudaStream_t s) {
-    MPPIB_REQUIRE(!cem_mode(c), "mppib_sample: mode cem samples through mppib_sample_colored (white noise: Lt = I)");
-    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample: mode smooth samples through mppib_sample_smooth");
-    if (int rc = check_risk_shard(c, "mppib_sample", k_offset, k_total)) return rc;
-    if (int rc = check_modes_total(c, "mppib_sample", k_total)) return rc;
-    const int K = c->params.K, T = c->params.T;
-    dim3 block(128), grid((K + 127) / 128, T);
-    if (adaptive_horizon(c))
-        return launch_sample_horizon_t<false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, nullptr, actions, noise, s);
-    if (adaptive_full(c))
-        mppib_sample_kernel<false, true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset,
-                                                                k_total, U, prior_row, actions, noise, c->dist, nullptr, 0);
-    else if (adaptive_cov(c))
-        mppib_sample_kernel<true><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
-                                                         prior_row, actions, noise, c->dist, nullptr, 0);
-    else
-        mppib_sample_kernel<false><<<grid, block, 0, s>>>(c->params, c->model.nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr, k_offset, k_total, U,
-                                                          prior_row, actions, noise, nullptr, c->anneal, c->anneal_n);
-    MPPIB_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return launch_sample_t<false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, nullptr, actions, noise, s);
 }
 
 int launch_sample_colored(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                           const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, cudaStream_t s) {
-    const int T = c->params.T, nu = c->model.nu;
-    MPPIB_REQUIRE(!smooth_mode(c), "mppib_sample_colored: mode smooth samples through mppib_sample_smooth");
-    if (int rc = check_risk_shard(c, "mppib_sample_colored", k_offset, k_total)) return rc;
-    if (int rc = check_modes_total(c, "mppib_sample_colored", k_total)) return rc;
-    MPPIB_REQUIRE(!c->params.cov_horizon, "mppib_sample_colored: cov_horizon already models the time correlation; colored noise excludes it");
-    MPPIB_REQUIRE(T <= CL_MAX_T && T * nu <= CL_MAX_N, "mppib_sample_colored: needs T <= %d and T*nu <= %d, got T = %d, T*nu = %d", CL_MAX_T,
-                  CL_MAX_N, T, T * nu);
-    if (cem_mode(c)) {
-        MPPIB_REQUIRE(c->dist != nullptr, "mppib_sample_colored: mppi_mode cem needs its state registered with mppib_set_distribution");
-        return launch_sample_colored_t<false, false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    switch (draw_rule(c)) {
+    case DRAW_CEM: return launch_sample_colored_t<DRAW_CEM>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    case DRAW_FULL: return launch_sample_colored_t<DRAW_FULL>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    case DRAW_DIAG: return launch_sample_colored_t<DRAW_DIAG>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
+    default: return launch_sample_colored_t<DRAW_FIXED>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
     }
-    if (adaptive_full(c)) return launch_sample_colored_t<false, true>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
-    if (adaptive_cov(c)) return launch_sample_colored_t<true, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
-    return launch_sample_colored_t<false, false>(c, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, Lt, actions, noise, s);
 }
 
 int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                          const float* U, float* actions, float* noise, cudaStream_t s) {
-    const int K = c->params.K, T = c->params.T, nu = c->model.nu;
-    MPPIB_REQUIRE(smooth_mode(c), "mppib_sample_smooth: needs mode smooth (MPPIB_MODE_SMOOTH), the handle has mode %d", c->params.mode);
-    MPPIB_REQUIRE(c->smooth != nullptr, "mppib_sample_smooth: no smooth state registered (mppib_set_smooth_state)");
-    MPPIB_REQUIRE(c->anneal == nullptr, "mppib_sample_smooth: annealed MPPI excludes mode smooth");
-    MPPIB_REQUIRE(T * nu <= SM_MAX_N, "mppib_sample_smooth: needs T*nu <= %d, got %d", SM_MAX_N, T * nu);
-    const int smem = (int)sizeof(float) * T * nu * SM_S;
+    const int K = c->params.K, nu = c->model.nu;
+    const int smem = (int)sizeof(float) * c->params.T * nu * SM_S;
     if (int rc = ensure_smem<mppib_sample_smooth_kernel>(c->device, smem)) return rc;
     mppib_sample_smooth_kernel<<<(K + SM_S - 1) / SM_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
                                                                       k_offset, k_total, U, actions, noise, c->smooth);
