@@ -13,7 +13,8 @@ and, for the adaptive row kinds, the live distribution:
 ``ws_layout`` restates the shared-memory plan of the warp-specialised K3 (``WsLayout`` and the ring-depth rule of
 ``launch_reduce_ws_t`` in ``csrc/reduce.cu``), so a case id can name the instantiation and the consumer-warp count that run.  For
 ``H`` the host sizes the ring with the M2 layout while the kernel addresses the (smaller) W layout, and the restatement follows the
-host.  ``syrk_split`` restates the split of the SYRK over lower-triangle 64 x 64 tiles and K-chunks.
+host.  With ``modes`` = M > 1 it follows the MODES launch, whose ring region also holds the fused K4 (``modes_fin_floats``), and
+``modes_grid`` restates that launch's (gx, M) grid.  ``syrk_split`` restates the split of the SYRK over lower-triangle 64 x 64 tiles and K-chunks.
 
 The K3 gate (``k3_gate``) bounds the float32 error of the kernel per case instead of using a constant tolerance:
   dS_k <= eps * [(n/4 + 6 + 2 ln2 |log2 gamma| T) * sum_t |gamma^t c_tk| + (n/4 + nu + 6) * sum_r |x_rk| |lambda Sigma^-1|_r |U|]
@@ -37,6 +38,7 @@ KINDS = ("W", "M2", "C")
 
 # ---------------------------------------------------------------------------------------------------------------- K3 layout
 WS_W, WS_NCONS, MAX_GRID, SMEM_CAP = 32, 7, 512, 224 * 1024
+SMEM_OPTIN, MAX_NU = 227 * 1024, 16    # the H100's opt-in shared memory per CTA; MPPIB_MAX_NU
 
 
 def row_floats(T, nu, kind):
@@ -44,14 +46,23 @@ def row_floats(T, nu, kind):
     return 2 + NR + (NR if kind == "M2" else nu * (nu + 1) // 2 if kind == "C" else NR * (NR + 1) // 2 if kind == "H" else 0)
 
 
-def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False):
-    """Bytes of ``WsLayout``: nparts warp partials (default one per consumer, min(nstage, 7)); smooth adds the [NR4] U region."""
+def modes_fin_floats(NR, M, G):
+    """Shared floats ``modes_rows`` (the K4 of n_modes = M > 1) needs with G shard rows: d, Sigma^-1 U / the coupled U and U [M*NR]
+    each, Sigma^-1 [16 x 16], the G scales of every mode, (beta, eta, F, sum_j k_ij) [M], D and k [M][M], 4 floats."""
+    return 3 * M * NR + MAX_NU * MAX_NU + M * G + 4 * M + 2 * M * M + 4
+
+
+def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False, modes=1):
+    """Bytes of ``WsLayout``: nparts warp partials (default one per consumer, min(nstage, 7)); smooth adds the [NR4] U region; with
+    modes = M > 1 the ring region holds at least modes_fin_floats(NR, M, 1), where the fused K4 runs ``modes_rows``."""
     NR = T * nu
     P4 = (row_floats(T, nu, kind) + 3) & ~3
     ring, fold = nstage * (NR + T) * WS_W, MAX_GRID + 4 * P4
     g = max(ring, fold)
     if kind == "C":
         g = max(g, NR + 1 + 2 * NR + nu * (nu + 1) // 2 + 3 * nu * nu)
+    if modes > 1:
+        g = max(g, modes_fin_floats(NR, modes, 1))
     gp = g + ((NR + 3) & ~3)
     wk = gp + ((T + 3) & ~3)
     misc = wk + 8 * WS_W + (min(nstage, WS_NCONS) if nparts is None else nparts) * P4
@@ -70,9 +81,10 @@ def ws_stages(T, nu, kind, smooth=False):
     return ns
 
 
-def ws_layout(T, nu, kind, smooth=False):
+def ws_layout(T, nu, kind, smooth=False, modes=1):
     """(rows of W per lane, consumer warps, ring stages, rows per x TMA box) of the K3 launch, or None if the shape is refused.
-    `smooth`: the layout of mode smooth (row W, plus the U region of the smoothness cost)."""
+    `smooth`: the layout of mode smooth (row W, plus the U region of the smoothness cost).  `modes` = M > 1: the MODES launch (row W
+    per mode): the ring depth is chosen without the modes_rows floor, and the launch, floor included, must fit the opt-in limit."""
     NR = T * nu
     if kind == "H":
         if NR > HZ_MAX_N:
@@ -82,10 +94,31 @@ def ws_layout(T, nu, kind, smooth=False):
         return None
     ns = ws_stages(T, nu, kind, smooth)
     ncons = min(ns, WS_NCONS)
+    nstage = ncons * (ns // ncons)
+    if modes > 1 and _ws_bytes(T, nu, nstage, kind, None, smooth, modes) > SMEM_OPTIN:
+        return None
     xbox = min(NR, 256)
     while NR % xbox:
         xbox -= 1
-    return (4 if NR <= 128 else 8 if NR <= 256 else 16), ncons, ncons * (ns // ncons), xbox
+    return (4 if NR <= 128 else 8 if NR <= 256 else 16), ncons, nstage, xbox
+
+
+def mode_range(K, k_offset, Kc, m):
+    """[lo, hi) local samples of mode m in the shard [k_offset, k_offset + K) (lo >= hi: none), as the MODES K3 CTA restates it."""
+    return max(0, m * Kc - k_offset), min(K, (m + 1) * Kc - k_offset)
+
+
+def mode_tiles(K, k_offset, Kc, m):
+    """32-sample tiles the MODES K3 walks for mode m: from the tile of its first local sample to that of its last (0 without one)."""
+    lo, hi = mode_range(K, k_offset, Kc, m)
+    return (hi + WS_W - 1) // WS_W - lo // WS_W if hi > lo else 0
+
+
+def modes_grid(K, k_offset, Kc, M, sms=NUM_SMS):
+    """gx of the MODES K3 grid (gx, M) (``launch_reduce_ws_t``): about one CTA per SM over all modes, no more than the tiles of the
+    largest mode's local range, at least 1."""
+    tmax = max(mode_tiles(K, k_offset, Kc, m) for m in range(M))
+    return max(1, min(tmax, sms // M))
 
 
 def wrap_K(T, nu, kind, sms=NUM_SMS, smooth=False):
