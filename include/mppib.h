@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 21
+#define MPPIB_ABI_VERSION 22
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -97,6 +97,7 @@ extern "C" {
 #define MPPIB_MAX_WORLDS 32   /* risk-aware MPPI: largest n_worlds (a group of worlds never straddles a 32-sample tile) */
 #define MPPIB_MAX_MODES 16    /* multi-modal MPPI: largest n_modes */
 #define MPPIB_MAX_ANNEAL 16   /* annealed MPPI: largest number of MPPI iterations per plan */
+#define MPPIB_MAX_SPLINE_DEGREE 3   /* spline MPPI: largest spline_degree */
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -235,6 +236,9 @@ typedef struct MppibParams {
     int32_t n_modes;           /* M in 1 .. MPPIB_MAX_MODES nominal sequences planned side by side                                   */
     float   mode_margin;       /* >= 0: the executed mode is kept while its free energy is within this margin of the lowest          */
     int32_t mode_samples;      /* Kc = K_total / M >= 32: global sample kg belongs to mode kg / Kc (the shard alone cannot tell K_total) */
+    /* spline MPPI (see "Spline MPPI" below); control_knots = 0 (and a zero-initialised block) keeps today's planner                   */
+    int32_t control_knots;     /* P: U, the samples K3 weights and the shard row hold P knots per control instead of T steps            */
+    int32_t spline_degree;     /* d in 1 .. MPPIB_MAX_SPLINE_DEGREE, read only when control_knots > 0; P in d + 1 .. T, P*nu <= 512   */
 } MppibParams;
 
 typedef struct MppibContext* MppibHandle;
@@ -276,6 +280,7 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
  *   n_modes > 1                     yes (d)       yes (d)   -        yes                   yes (d)
  *   n_worlds > 1                    yes (e)       yes (e)   -        yes (e)               yes (e)
  *   annealing schedule registered   yes (f)       yes (f)   -        -                     -
+ *   control_knots > 0               -             -         -        -                     -          (mppib_sample_spline: yes (g))
  *
  * (a) even with no distribution registered: cov_horizon models the time correlation itself
  * (b) with the CEM state registered (mppib_set_distribution)
@@ -283,6 +288,8 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
  * (d) k_total = n_modes * mode_samples
  * (e) K, k_offset and k_total multiples of n_worlds
  * (f) registered for the handle's T; the library entries refuse a schedule whatever its T
+ * (g) with a spline table registered for the handle's (T, control_knots, spline_degree) (mppib_set_spline); the parameter block already
+ *     excludes every draw but the fixed Sigma
  * Every entry also needs its pointers, k_offset + K <= k_total and its size limits: colored T <= 256 and T*nu <= 512, smooth
  * T*nu <= 512, the noise library 1 <= n_knots <= 32, cov_horizon T*nu <= 256.                                              */
 
@@ -511,6 +518,28 @@ int32_t mppib_sample_smooth(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  * mppib_set_params has changed T (or switched to an excluded mode) without a new registration.  The K1 table at mppib_sample lists the
  * entries that refuse a registered schedule.  NULL switches it off: every launch is then today's.                                    */
 int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations);
+
+/* Spline MPPI (control_knots = P > 0, spline_degree = d; modes SIMPLE and MEAN with the fixed Sigma; no filter_u, update_cov /
+ * update_lambda, cem, smooth, n_modes > 1, n_worlds > 1 or annealing).  The planned control sequence is a clamped uniform B-spline of
+ * degree d on [0, T-1] with P control knots theta[P][nu]: the action at step t is a_t = sum_p B[t][p] theta_p.  U is theta[P][nu], and
+ * the vector K3 weights, K4 updates and the shard row carries is P*nu long (partial [2 + P*nu]); the cost rows stay T.  The table is a
+ * device buffer registered with mppib_set_spline (caller-owned, filled by the caller; S = d + 3 floats per row):
+ *   table    [(T + P)*S + T*nu]  rows[T + P][S], then U_exec[T][nu].  Row r = (first index, count, weights[count]) of the non-zero
+ *            weights in ascending index order: rows 0 .. T-1 interpolate (B[t]), rows T .. T+P-1 shift (theta'_p = sum_q N_q(xi_p + 1)
+ *            theta_q at the Greville abscissa xi_p, count 0 = u_init).  Indices and counts are stored as floats.
+ *   K1     mppib_sample_spline: for knot p of sample k the white draws of mppib_sample with p in the t slot of the counter,
+ *          theta~ = clamp(theta_p + L0 z) (null row: clamp(0)), xk[P][nu][K] = theta~ - theta_p (SIMPLE) or theta~ (MEAN);
+ *          actions[T][nu][K] = clamp(sum_q w_q theta~_{first+q}, u_min, u_max) (the first term a product, the rest fmaf in index
+ *          order; the clamp only absorbs the rounding of the float32 weights, whose exact values are convex)
+ *   K3     mppib_reduce / mppib_reduce_finalize with x = xk: today's K3 over the P*nu rows (g = lambda Sigma^-1 theta per knot)
+ *   K4     today's update of theta (split and fused tail); action_out = theta_0 = a_0 (B[0] = e_0); U_exec = B theta by the same sums
+ *   shift  theta <- the shift rows applied to theta; *plan_ctr += 1
+ * With d = 1 and P = T, B = I and every row holds one weight 1.0: the plan equals today's bit for bit.  Registration records (T, P, d);
+ * K1, K3, K4 and the shift refuse a handle with P > 0 while no table or one registered for another (T, P, d) is set, or while a
+ * distribution is registered.  NULL switches it off.                                                                              */
+int32_t mppib_set_spline(MppibHandle h, float* table, int32_t P, int32_t d);
+int32_t mppib_sample_spline(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset,
+                            uint32_t k_total, const float* U, float* actions, float* xk, void* stream);
 
 #ifdef __cplusplus
 }

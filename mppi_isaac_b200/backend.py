@@ -25,6 +25,7 @@ SYMBOLS = [
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
     "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth", "mppib_set_anneal",
+    "mppib_set_spline", "mppib_sample_spline",
 ]
 
 
@@ -78,9 +79,9 @@ def shard_row_floats(params, nu):
     """Floats of one shard row that K3 (or the elite kernel of mppi_mode cem) writes under `params` with `nu` inputs once a
     distribution is registered, as the library sizes its buffers (shard_row_floats in csrc/common.cuh): 2 + T*nu, + T*nu with
     update_cov, + nu(nu+1)/2 with cov_full, + n(n+1)/2 with cov_horizon (n = T*nu); n_modes * (2 + T*nu) with n_modes > 1;
-    cem_row_floats with mppi_mode cem."""
+    cem_row_floats with mppi_mode cem.  With control_knots = P > 0 the control vector is P*nu long (ctrl_rows in csrc/common.cuh)."""
     T, nu = int(params.T), int(nu)
-    n = T * nu
+    n = (int(params.control_knots) or T) * nu
     if params.mode == MODE_CEM:
         return cem_row_floats(T, nu, params.n_elites)
     if params.n_modes > 1:
@@ -100,6 +101,11 @@ def smooth_state_floats(T, nu):
 def anneal_state_floats(T, n_iterations):
     """Floats of the schedule of annealed MPPI: (counter, s[N][T], r[N][T])."""
     return 1 + 2 * int(n_iterations) * int(T)
+
+
+def spline_table_floats(T, P, d, nu):
+    """Floats of the spline table of spline MPPI: rows[T + P][d + 3], then U_exec[T][nu]."""
+    return (int(T) + int(P)) * (int(d) + 3) + int(T) * int(nu)
 
 
 def cem_row_floats(T, nu, E):
@@ -137,6 +143,7 @@ class CudaBackend:
         self._dist_keepalive = None
         self._smooth_keepalive = None
         self._anneal_keepalive = None     # (state, N)
+        self._spline_keepalive = None     # the registered spline table
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -160,6 +167,12 @@ class CudaBackend:
             state, n = self._anneal_keepalive            # rebuilt for another horizon or mode registers its own)
             if not (state.numel() == anneal_state_floats(params.T, n) and self.lib.mppib_set_anneal(self.handle, _ptr(state), C.c_int32(n)) == 0):
                 self._anneal_keepalive = None
+        if self._spline_keepalive is not None:           # ... and its spline table, while the block still has the (P, d) it was built for
+            table, P, d = self._spline_keepalive
+            if not (int(params.control_knots) == P and int(params.spline_degree) == d
+                    and table.numel() == spline_table_floats(params.T, P, d, model.nu)
+                    and self.lib.mppib_set_spline(self.handle, _ptr(table), C.c_int32(P), C.c_int32(d)) == 0):
+                self._spline_keepalive = None
 
     def destroy(self):
         if self.handle:
@@ -325,6 +338,29 @@ class CudaBackend:
                                    f"{state.dtype} {state.numel()}")
         self._check(self.lib.mppib_set_anneal(self.handle, _ptr(state), C.c_int32(0 if state is None else int(n_iterations))), "mppib_set_anneal")
         self._anneal_keepalive = None if state is None else (state, int(n_iterations))
+
+    def set_spline(self, table):
+        """Spline MPPI: register the device tensor (rows[T + P][d + 3], U_exec[T][nu]) of ``blob.spline_table`` for the parameter
+        block's (T, control_knots, spline_degree); K1 and the shift read it, K4 writes U_exec (None switches it off)."""
+        P, d = int(self.params.control_knots), int(self.params.spline_degree)
+        if table is not None:
+            need = spline_table_floats(self.params.T, P, d, self.model.nu)
+            if table.numel() != need or table.dtype != torch.float32 or not table.is_contiguous():
+                raise RuntimeError(f"mppib_set_spline: (rows[T + P][d + 3], U_exec[T][nu]) = {need} contiguous float32 values, got "
+                                   f"{table.dtype} {table.numel()}")
+        self._check(self.lib.mppib_set_spline(self.handle, _ptr(table), C.c_int32(P), C.c_int32(d)), "mppib_set_spline")
+        self._spline_keepalive = None if table is None else (table, P, d)
+
+    def sample_spline(self, seed, plan_idx, k_offset, k_total, U, actions, xk, plan_ctr=None):
+        """K1 of spline MPPI: knots theta~ = clamp(U + L0 z) per sample, xk[P][nu][K] = theta~ - U (SIMPLE) or theta~ (MEAN), and
+        actions[T][nu][K] interpolated by the registered table."""
+        P, T, nu, K = int(self.params.control_knots), int(self.params.T), int(self.model.nu), int(self.params.K)
+        for name, t, n in (("actions", actions, T * nu * K), ("xk", xk, P * nu * K)):
+            if t is None or t.numel() != n:
+                raise RuntimeError(f"mppib_sample_spline: {name} must hold {n} floats")
+        self.launches += 1
+        self._check(self.lib.mppib_sample_spline(self.handle, C.c_uint64(seed), C.c_uint64(plan_idx), _ptr(plan_ctr), C.c_uint32(k_offset),
+                                                 C.c_uint32(k_total), _ptr(U), _ptr(actions), _ptr(xk), self._stream()), "mppib_sample_spline")
 
     def reduce(self, cost, x, U, partial):
         self._check_row(partial, "mppib_reduce")

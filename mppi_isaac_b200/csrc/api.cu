@@ -87,6 +87,17 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->n_worlds <= 1, "n_modes > 1 excludes n_worlds > 1");
         MPPIB_REQUIRE(p->T * m->nu <= 512, "n_modes > 1 needs T*nu <= 512, got %d", p->T * m->nu);
     }
+    MPPIB_REQUIRE(p->control_knots >= 0, "control_knots = %d must be >= 0", p->control_knots);
+    if (p->control_knots > 0) {
+        const int P = p->control_knots, d = p->spline_degree;
+        MPPIB_REQUIRE(d >= 1 && d <= MPPIB_MAX_SPLINE_DEGREE, "spline_degree = %d out of range [1, %d]", d, MPPIB_MAX_SPLINE_DEGREE);
+        MPPIB_REQUIRE(P >= d + 1 && P <= p->T, "control_knots = %d out of range [spline_degree + 1 = %d, T = %d]", P, d + 1, p->T);
+        MPPIB_REQUIRE(P * m->nu <= 512 && p->T <= 256, "control_knots needs P*nu <= 512 and T <= 256, got P*nu = %d, T = %d", P * m->nu, p->T);
+        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "control_knots > 0 excludes mode cem and mode smooth");
+        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "control_knots > 0 excludes update_cov and update_lambda");
+        MPPIB_REQUIRE(p->n_modes <= 1 && p->n_worlds <= 1, "control_knots > 0 excludes n_modes > 1 and n_worlds > 1");
+        MPPIB_REQUIRE(!p->filter_u, "control_knots > 0 excludes filter_u: the spline is smooth already, switch filter_u off");
+    }
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -122,6 +133,7 @@ static int anneal_excludes(const MppibParams& p, const char* who) {
     MPPIB_REQUIRE(p.mode == MPPIB_MODE_SIMPLE || p.mode == MPPIB_MODE_MEAN, "%s: annealed MPPI excludes mode cem (it has its own sigma) and mode smooth", who);
     MPPIB_REQUIRE(!p.update_cov && !p.update_lambda, "%s: annealed MPPI excludes update_cov and update_lambda", who);
     MPPIB_REQUIRE(p.n_modes <= 1, "%s: annealed MPPI excludes n_modes > 1 (the Stein coupling's Sigma^-1 metric would need the schedule)", who);
+    MPPIB_REQUIRE(p.control_knots == 0, "%s: annealed MPPI excludes control_knots > 0", who);
     return 0;
 }
 
@@ -130,6 +142,18 @@ int check_anneal(const MppibContext* c, const char* who) {
     MPPIB_REQUIRE(c->params.T == c->anneal_T, "%s: the annealing schedule was registered for T = %d, the parameter block has T = %d; register a schedule "
                   "for the new horizon (mppib_set_anneal)", who, c->anneal_T, c->params.T);
     return anneal_excludes(c->params, who);
+}
+
+int check_spline(const MppibContext* c, const char* who) {
+    const MppibParams& p = c->params;
+    if (p.control_knots == 0) return 0;
+    MPPIB_REQUIRE(c->spline != nullptr, "%s: control_knots = %d needs its spline table registered (mppib_set_spline)", who, p.control_knots);
+    MPPIB_REQUIRE(c->spline_T == p.T && c->spline_P == p.control_knots && c->spline_d == p.spline_degree && c->spline_nu == c->model.nu,
+                  "%s: the spline table was registered for (T, P, d, nu) = (%d, %d, %d, %d), the handle has (%d, %d, %d, %d); register a table "
+                  "for the new block (mppib_set_spline)", who, c->spline_T, c->spline_P, c->spline_d, c->spline_nu, p.T, p.control_knots,
+                  p.spline_degree, c->model.nu);
+    MPPIB_REQUIRE(update_rule(c) == RULE_PLAIN, "%s: control_knots > 0 runs plain MPPI; register no distribution", who);
+    return 0;
 }
 
 extern "C" {
@@ -271,6 +295,13 @@ int32_t mppib_sample(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint
     return launch_sample(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, prior_row, actions, noise, (cudaStream_t)stream);
 }
 
+int32_t mppib_sample_spline(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                            const float* U, float* actions, float* xk, void* stream) {
+    if (int rc = k1_admit(h, K1_SPLINE, U && actions && xk, k_offset, k_total)) return rc;
+    MPPIB_ON_DEVICE(h);
+    return launch_sample_spline(h, seed, plan_idx, plan_ctr, k_offset, k_total, U, actions, xk, (cudaStream_t)stream);
+}
+
 int32_t mppib_sample_colored(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
                              const float* U, const float* prior_row, const float* Lt, float* actions, float* noise, void* stream) {
     if (int rc = k1_admit(h, K1_COLORED, U && Lt && actions, k_offset, k_total)) return rc;
@@ -311,6 +342,7 @@ int32_t mppib_rollout(MppibHandle h, const float* state0, const float* root0, fl
 int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const float* U, float* partial, void* stream) {
     MPPIB_REQUIRE(h && cost && x && U && partial, "mppib_reduce: null argument");
     if (int rc = check_anneal(h, "mppib_reduce")) return rc;
+    if (int rc = check_spline(h, "mppib_reduce")) return rc;
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
@@ -319,6 +351,7 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
 int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, float* U, float* partial, float* action_out, float* stats, void* stream) {
     MPPIB_REQUIRE(h && cost && x && U && partial && action_out, "mppib_reduce_finalize: null argument");
     if (int rc = check_anneal(h, "mppib_reduce_finalize")) return rc;
+    if (int rc = check_spline(h, "mppib_reduce_finalize")) return rc;
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, U, action_out, stats, (cudaStream_t)stream);
@@ -327,6 +360,7 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
 int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U, float* action_out, float* stats, void* stream) {
     MPPIB_REQUIRE(h && U && action_out && G >= 1, "mppib_finalize: bad argument");
     if (int rc = check_anneal(h, "mppib_finalize")) return rc;
+    if (int rc = check_spline(h, "mppib_finalize")) return rc;
     if (!partials) {
         MPPIB_REQUIRE(h->peer_world >= 2 && G == h->peer_world, "mppib_finalize: partials == NULL needs an open peer window and G == world (G=%d, world=%d)", G, h->peer_world);
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
@@ -387,9 +421,23 @@ int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations) {
     return 0;
 }
 
+int32_t mppib_set_spline(MppibHandle h, float* table, int32_t P, int32_t d) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    if (table == nullptr) {
+        h->spline = nullptr; h->spline_T = h->spline_P = h->spline_d = h->spline_nu = 0;
+        return 0;
+    }
+    MPPIB_REQUIRE(P > 0 && P == h->params.control_knots && d == h->params.spline_degree,
+                  "mppib_set_spline: (P, d) = (%d, %d) does not match the parameter block's (control_knots, spline_degree) = (%d, %d)", P, d,
+                  h->params.control_knots, h->params.spline_degree);
+    h->spline = table; h->spline_T = h->params.T; h->spline_P = P; h->spline_d = d; h->spline_nu = h->model.nu;
+    return 0;
+}
+
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream) {
     MPPIB_REQUIRE(h && U, "mppib_shift: null argument");
     if (int rc = check_anneal(h, "mppib_shift")) return rc;
+    if (int rc = check_spline(h, "mppib_shift")) return rc;
     MPPIB_ON_DEVICE(h);
     return launch_shift(h, U, plan_ctr, (cudaStream_t)stream);
 }

@@ -50,6 +50,8 @@ struct MppibContext {
     float* smooth;                             // MODE_SMOOTH: device (a_prev[nu], A[T][nu]), read by K1, updated by K4 (nullable)
     float* anneal;                             // annealed MPPI: device (counter, s[N][T], r[N][T]), read by K1 / K3, counter set by K4 / shift (nullable)
     int anneal_n, anneal_T;                    // N iterations and the horizon T the schedule was registered for
+    float* spline;                             // spline MPPI: device (rows[T + P][d + 3], U_exec[T][nu]), read by K1 / K4 / shift, U_exec written by K4 (nullable)
+    int spline_T, spline_P, spline_d, spline_nu;   // the (T, P, d, nu) the table was registered for
     // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
     float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
     float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
@@ -80,10 +82,28 @@ struct DeviceGuard {
     DeviceGuard _guard((h)->device);                                                        \
     MPPIB_CHECK_CUDA(_guard.err)
 
+// Spline MPPI (control_knots = P > 0): the control vector U that K1 samples around, K3 weights and K4 updates is the knot vector
+// theta[P][nu], while the cost rows stay T.  Its rows: P, or T with the feature off.  Every length of that vector comes from here.
+__host__ __device__ __forceinline__ int ctrl_rows(const MppibParams& p) { return p.control_knots > 0 ? p.control_knots : p.T; }
+// The spline table (include/mppib.h "Spline MPPI"): rows[T + P] of (first, count, weights[d + 1]), then U_exec[T][nu]
+__host__ __device__ __forceinline__ int spline_row_floats(int d) { return d + 3; }
+static inline long long spline_table_floats(int T, int P, int d, int nu) { return (long long)(T + P) * spline_row_floats(d) + (long long)T * nu; }
+// sum_q w_q v[(first + q) * stride] over a table row's non-zero weights in index order: the first term a product, the rest fmaf
+__device__ __forceinline__ float spline_apply(const float* __restrict__ row, const float* v, int stride) {
+    const int first = (int)row[0], n = (int)row[1];
+    float a = row[2] * v[first * stride];
+    for (int q = 1; q < n; ++q) a = fmaf(row[2 + q], v[(first + q) * stride], a);
+    return a;
+}
+// the launch-time refusals of spline MPPI (api.cu): the registered table must match (T, P, d, nu), and the plan must be plain MPPI
+int check_spline(const MppibContext* c, const char* who);
+// the table the kernels read: none while the parameter block has control_knots = 0, whatever was registered before
+static inline float* live_spline(const MppibContext* c) { return c->params.control_knots > 0 ? c->spline : nullptr; }
+
 // The update rule a plan runs: which K3 (or elite kernel), K4 and shift, and what their shard row carries.  Risk-aware MPPI is not a
 // rule but a K3 flag (risk_mode) that combines with PLAIN, DIST and FULL.
 enum Rule { RULE_PLAIN, RULE_DIST, RULE_FULL, RULE_HORIZON, RULE_SMOOTH, RULE_MODES, RULE_CEM };
-// Floats of one shard row:
+// Floats of one shard row (T: the control rows, ctrl_rows() of the parameter block):
 //   PLAIN, SMOOTH  (beta, eta, W[T*nu])
 //   DIST           (beta, eta, W[T*nu]), + M2[T*nu] with update_cov
 //   FULL           (beta, eta, W[T*nu], C[nu(nu+1)/2])
@@ -103,7 +123,7 @@ __host__ __device__ inline int shard_row_floats(Rule r, int T, int nu, bool upda
     }
 }
 __host__ __device__ inline int shard_row_floats(Rule r, const MppibParams& p, int nu) {
-    return shard_row_floats(r, p.T, nu, p.update_cov, p.n_modes, p.n_elites);
+    return shard_row_floats(r, ctrl_rows(p), nu, p.update_cov, p.n_modes, p.n_elites);
 }
 static inline bool risk_mode(const MppibContext* c) { return c->params.n_worlds > 1; }
 static inline bool modes_on(const MppibContext* c) { return c->params.n_modes > 1; }
@@ -259,7 +279,7 @@ int ensure_smem(int device, size_t bytes) {
 // The K1 entries of the C ABI.  k1_admit (sample.cu) holds which draw each entry samples and which it refuses: the null arguments
 // (args = the entry's pointers are all non-null), the shard range, the annealing schedule, the mode routing, the n_worlds and n_modes
 // shards and the size limits.  Returns 0 or the error of the first refusal; nothing is launched.
-enum K1Entry { K1_SAMPLE, K1_COLORED, K1_SMOOTH, K1_NOISE_LIBRARY, K1_SAMPLE_LIBRARY };
+enum K1Entry { K1_SAMPLE, K1_COLORED, K1_SMOOTH, K1_NOISE_LIBRARY, K1_SAMPLE_LIBRARY, K1_SPLINE };
 int k1_admit(const MppibContext* c, K1Entry e, bool args, uint32_t k_offset, uint32_t k_total, int n_knots = 1);
 
 // kernel launchers (defined in the .cu files)
@@ -273,6 +293,8 @@ int launch_noise_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, c
                          float* Z, cudaStream_t s);
 int launch_sample_library(MppibContext* c, uint32_t k_offset, uint32_t k_total, const float* U, const float* prior_row, const float* Z,
                           float* actions, float* noise, cudaStream_t s);
+int launch_sample_spline(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                         const float* U, float* actions, float* xk, cudaStream_t s);
 int launch_rollout(MppibContext* c, const float* state0, const float* root0, float* state, const float* actions, int t0, int nsteps,
                    float* obs, cudaStream_t s);
 int launch_reduce(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,

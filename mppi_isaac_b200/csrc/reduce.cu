@@ -215,7 +215,7 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
                                               float* __restrict__ dist, float* __restrict__ hz_sig = nullptr) {
     constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON;
-    const int T = p.T, NR = T * nu;
+    const int T = p.T, NR = (R == RULE_PLAIN ? ctrl_rows(p) : T) * nu;   // knots parameterise PLAIN only
     float* sg = un + NR;
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
@@ -365,6 +365,14 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
             dist[0] = fminf(fmaxf(l, 1e-3f * p.lambda_), 1e3f * p.lambda_);
         }
     }
+}
+
+// Spline MPPI: after finalize_rows, U_exec[T][nu] = B theta with the table's interpolation rows, theta = un (finalize_rows synchronised
+// after writing it; filter_u is refused with knots, so un holds the updated knots as U does).
+__device__ __forceinline__ void spline_exec(const MppibParams& p, int nu, const float* un, float* __restrict__ spline) {
+    const int T = p.T, S = spline_row_floats(p.spline_degree);
+    float* ue = spline + (size_t)(T + p.control_knots) * S;
+    for (int r = threadIdx.x; r < T * nu; r += blockDim.x) ue[r] = spline_apply(spline + (r / nu) * S, un + r % nu, nu);
 }
 
 // K4 of mode smooth (smooth = (a_prev[nu], A[T][nu])): combine G rows (beta_g, eta_g, W_g) of stride P as finalize_rows does, the SIMPLE
@@ -633,7 +641,8 @@ template <Rule R>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
-                                                float* __restrict__ dist, float* __restrict__ smooth = nullptr, float* __restrict__ anneal = nullptr) {
+                                                float* __restrict__ dist, float* __restrict__ smooth = nullptr, float* __restrict__ anneal = nullptr,
+                                                float* __restrict__ spline = nullptr) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = (int)gridDim.x;
     float* sc = tiles;                   // [MAX_GRID] scale of every CTA partial (the ring is idle now)
@@ -699,6 +708,7 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             __syncthreads();
             if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
             else finalize_rows<R>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            if constexpr (R == RULE_PLAIN) if (spline) spline_exec(p, nu, tiles, spline);
             if (tid == 0 && anneal) anneal[0] += 1.0f;                        // annealed MPPI: the next iteration's row (every CTA read it)
         }
     }
@@ -729,8 +739,9 @@ struct WsLayout {
     int bytes;                    // + 128 bytes of headroom: the ring depth of every shape stays what it was tuned at
     // row: the rule whose shard row the warp partials hold; nparts: warp partials stored, by default one per consumer warp
     // (min(nstage, WS_NCONS): the launch rounds the ring depth down to a multiple of the consumer count)
-    __host__ __device__ WsLayout(int T, int nu, int nstage, Rule row, bool update_cov, bool smooth = false, int nparts = -1, int modes = 1) {
-        const int NR = T * nu, P4 = (shard_row_floats(row, T, nu, update_cov, 1, 0) + 3) & ~3;
+    // T: the cost rows of a tile, Tc: the control rows (ctrl_rows())
+    __host__ __device__ WsLayout(int T, int Tc, int nu, int nstage, Rule row, bool update_cov, bool smooth = false, int nparts = -1, int modes = 1) {
+        const int NR = Tc * nu, P4 = (shard_row_floats(row, Tc, nu, update_cov, 1, 0) + 3) & ~3;
         if (nparts < 0) nparts = nstage < WS_NCONS ? nstage : WS_NCONS;
         const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
         g = ring > fold_floats ? ring : fold_floats;
@@ -778,10 +789,11 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                        int nu, int xbox_rows, int nstage, int ncons, const float* __restrict__ U, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                        float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
-                       const float* __restrict__ hz_g, float* __restrict__ smooth, float* __restrict__ anneal, int anneal_n) {
+                       const float* __restrict__ hz_g, float* __restrict__ smooth, float* __restrict__ anneal, int anneal_n,
+                       float* __restrict__ spline) {
     constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON, SMOOTH = R == RULE_SMOOTH, MODES = R == RULE_MODES;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    const int K = p.K, T = p.T, NR = T * nu;
+    const int K = p.K, T = p.T, Tc = R == RULE_PLAIN ? ctrl_rows(p) : T, NR = Tc * nu;   // knots parameterise PLAIN only
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if constexpr (MODES) U += (size_t)blockIdx.y * NR;                       // this CTA's mode
     const float lam = ADAPT ? dist[0] : p.lambda_;
@@ -789,12 +801,12 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const bool simple = SMOOTH || p.mode == MPPIB_MODE_SIMPLE;
     const bool m2 = R == RULE_DIST && p.update_cov;
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
-    const int P = shard_row_floats(k3_row_rule(R), T, nu, m2, 1, 0);
+    const int P = shard_row_floats(k3_row_rule(R), Tc, nu, m2, 1, 0);
 
     const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
     const bool smooth_term = SMOOTH && p.smooth_weight != 0.f;
-    const WsLayout L(T, nu, nstage, k3_row_rule(R), m2, smooth_term, -1, MODES ? p.n_modes : 1);
+    const WsLayout L(T, Tc, nu, nstage, k3_row_rule(R), m2, smooth_term, -1, MODES ? p.n_modes : 1);
     float* tiles = reinterpret_cast<float*>(smem_raw);                        // [nstage][(NR+T)*32]
     float* g = tiles + L.g;                                                   // [NR4] lambda * Sigma^-1 U (SIMPLE), zero padded; FULL MEAN: U
     float* gp = tiles + L.gp;                                                 // [T4]  gamma^t, zero padded
@@ -1044,7 +1056,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     // the horizon K3 folds as DIST's does; it gets no fin_U and no peers, the SYRK finishes its row
     if constexpr (MODES) fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
     else fold_and_finish<HZN ? RULE_DIST : R>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda,
-                                              dist, smooth, anneal);
+                                              dist, smooth, anneal, spline);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; DIST / FULL /
@@ -1056,7 +1068,7 @@ __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
                 float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth,
-                float* __restrict__ anneal) {
+                float* __restrict__ anneal, float* __restrict__ spline) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const float* partials = partials_in;
     int P = shard_row_floats(R, p, nu);                                       // row stride of the partials
@@ -1070,6 +1082,7 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
     if constexpr (R == RULE_MODES) modes_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
     else if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
     else finalize_rows<R>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
+    if constexpr (R == RULE_PLAIN) if (spline) spline_exec(p, nu, un, spline);
     if (threadIdx.x == 0 && partials_in == nullptr) peer_consume(peers, seq);
     if (threadIdx.x == 0 && anneal) anneal[0] += 1.0f;
 }
@@ -1198,11 +1211,20 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
 // hz_g (cov_horizon with a registered distribution, SIMPLE mode): g = lambda Sigma_H^-1 U of the shifted U, once per plan, for K3's
 // control cost (a row of Sigma_H^-1 per thread, summed in column order).  anneal (annealed MPPI, nullable): the plan starts at
 // iteration 0, so the counter of the registered schedule is reset.
+// spline (spline MPPI, nullable): the knots shift by the table's shift rows (count 0: u_init) instead of by one step.
 __global__ void mppib_shift_kernel(const __grid_constant__ MppibParams p, int nu, float* __restrict__ U, uint32_t* __restrict__ plan_ctr,
-                                   const float* __restrict__ dist, float* __restrict__ hz_g, float* __restrict__ anneal) {
+                                   const float* __restrict__ dist, float* __restrict__ hz_g, float* __restrict__ anneal,
+                                   const float* __restrict__ spline) {
     extern __shared__ float tmp[];
-    const int NR = p.T * nu;
-    for (int r = threadIdx.x; r < NR; r += blockDim.x) tmp[r] = r + nu < NR ? U[r + nu] : p.u_init[r % nu];
+    const int NR = ctrl_rows(p) * nu;
+    for (int r = threadIdx.x; r < NR; r += blockDim.x) {
+        if (spline) {
+            const float* row = spline + (size_t)(p.T + r / nu) * spline_row_floats(p.spline_degree);
+            tmp[r] = row[1] > 0.f ? spline_apply(row, U + r % nu, nu) : p.u_init[r % nu];
+        } else {
+            tmp[r] = r + nu < NR ? U[r + nu] : p.u_init[r % nu];
+        }
+    }
     __syncthreads();
     for (int r = threadIdx.x; r < NR; r += blockDim.x) U[r] = tmp[r];
     if (threadIdx.x == 0 && plan_ctr) *plan_ctr += 1u;
@@ -1264,8 +1286,8 @@ int make_map(CUtensorMap* tm, const float* base, int rows, int K, int box_rows, 
 // consumers'.
 static int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth = false) {
     int ns = 8;
-    while (ns > 1 && WsLayout(p.T, nu, ns, row, p.update_cov, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
-    if (ns < 2 && WsLayout(p.T, nu, 2, row, p.update_cov, smooth).bytes <= 224 * 1024) ns = 2;
+    while (ns > 1 && WsLayout(p.T, ctrl_rows(p), nu, ns, row, p.update_cov, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
+    if (ns < 2 && WsLayout(p.T, ctrl_rows(p), nu, 2, row, p.update_cov, smooth).bytes <= 224 * 1024) ns = 2;
     return ns;
 }
 
@@ -1273,7 +1295,7 @@ static int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth 
 template <int RPL, Rule R, bool RISK>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, float* smooth, float* anneal, cudaStream_t s) {
-    const int T = c->params.T, nu = c->model.nu, NR = T * nu, K = c->params.K;
+    const int T = c->params.T, Tc = ctrl_rows(c->params), nu = c->model.nu, NR = Tc * nu, K = c->params.K;
     // consumers = min(7, stages that fit); the ring depth is rounded down to a multiple of the consumer count so that a stage always
     // belongs to the same consumer (see the kernel)
     // The horizon K3 sizes its ring for the M2 row of update_cov, which it does not write: its kernel addresses the W layout
@@ -1284,17 +1306,17 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     const int ncons = nstage_max < WS_NCONS ? nstage_max : WS_NCONS;
     const int nstage = ncons * (nstage_max / ncons);
     const int modes = R == RULE_MODES ? c->params.n_modes : 1;
-    const size_t smem = WsLayout(T, nu, nstage, row, c->params.update_cov, smooth_term, -1, modes).bytes;
+    const size_t smem = WsLayout(T, Tc, nu, nstage, row, c->params.update_cov, smooth_term, -1, modes).bytes;
     if (int rc = ensure_smem<mppib_reduce_ws_kernel<RPL, R, RISK>>(c->device, smem)) return rc;
     int xbox_rows = NR < 256 ? NR : 256;
     while (NR % xbox_rows != 0) --xbox_rows;
     // tensor maps are rebuilt only when a buffer, the shape or the device changes (the eager / stepwise path calls this per plan)
-    struct MapCache { const void* x; const void* c; int K, T, nu, dev; CUtensorMap tm_x, tm_c; };
+    struct MapCache { const void* x; const void* c; int K, T, NR, dev; CUtensorMap tm_x, tm_c; };
     static thread_local MapCache mc = {nullptr, nullptr, 0, 0, 0, -1, {}, {}};
-    if (mc.x != x || mc.c != cost || mc.K != K || mc.T != T || mc.nu != nu || mc.dev != c->device) {
+    if (mc.x != x || mc.c != cost || mc.K != K || mc.T != T || mc.NR != NR || mc.dev != c->device) {
         if (int rc = make_map(&mc.tm_x, x, NR, K, xbox_rows, WS_W)) return rc;
         if (int rc = make_map(&mc.tm_c, cost, T, K, T, WS_W)) return rc;
-        mc.x = x; mc.c = cost; mc.K = K; mc.T = T; mc.nu = nu; mc.dev = c->device;
+        mc.x = x; mc.c = cost; mc.K = K; mc.T = T; mc.NR = NR; mc.dev = c->device;
     }
     const int ntiles = (K + WS_W - 1) / WS_W;
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
@@ -1317,7 +1339,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     mppib_reduce_ws_kernel<RPL, R, RISK><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch,
                                                                              c->reduce_ticket, partial, peers, fin_U, fin_action, fin_stats,
                                                                              fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g, smooth, anneal,
-                                                                             c->anneal_n);
+                                                                             c->anneal_n, R == RULE_PLAIN ? live_spline(c) : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1326,7 +1348,7 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
 template <Rule R, bool RISK>
 int launch_reduce_rule(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
                        float* fin_stats, float* smooth, float* anneal, cudaStream_t s) {
-    const int NR = c->params.T * c->model.nu;
+    const int NR = ctrl_rows(c->params) * c->model.nu;
     if (NR <= 32 * 4) return launch_reduce_ws_t<4, R, RISK>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, smooth, anneal, s);
     if constexpr (R != RULE_HORIZON) {
         if (NR > 32 * 8) return launch_reduce_ws_t<16, R, RISK>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, smooth, anneal, s);
@@ -1398,7 +1420,8 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
     if (rule == RULE_CEM) return launch_elite(c, cost, x, partial, fin_U, fin_action, fin_stats, s);   // none of K3's limits apply
     const int T = c->params.T, nu = c->model.nu;
     MPPIB_REQUIRE(c->params.K >= 4 && c->params.K % 4 == 0, "mppib_reduce: K=%d must be a positive multiple of 4 (16-byte rows for TMA / 128-bit loads)", c->params.K);
-    MPPIB_REQUIRE(T * nu <= 32 * 16, "mppib_reduce: T*nu = %d exceeds %d", T * nu, 32 * 16);
+    MPPIB_REQUIRE(ctrl_rows(c->params) * nu <= 32 * 16, "mppib_reduce: %s = %d exceeds %d", c->params.control_knots > 0 ? "P*nu" : "T*nu",
+                  ctrl_rows(c->params) * nu, 32 * 16);
     MPPIB_REQUIRE(T <= 256, "mppib_reduce: T = %d exceeds the 256-row TMA box", T);
     MPPIB_REQUIRE(reduce_ws_stages(c->params, nu, RULE_PLAIN) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages", T, nu);
     MPPIB_REQUIRE(!adaptive_cov(c) || adaptive_full(c) || reduce_ws_stages(c->params, nu, RULE_DIST) >= 2,
@@ -1447,13 +1470,13 @@ template <Rule R>
 static int launch_finalize_t(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, size_t smem, float* dist,
                              float* hz_sig, float* smooth, float* anneal, cudaStream_t s) {
     mppib_finalize_kernel<R><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, dist, hz_sig,
-                                                  smooth, anneal);
+                                                  smooth, anneal, R == RULE_PLAIN ? live_spline(c) : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
 int launch_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s) {
-    const int NR = c->params.T * c->model.nu;
+    const int NR = ctrl_rows(c->params) * c->model.nu;
     const size_t un = (NR + G) * sizeof(float);                               // U and the G scales, the shared floats of every rule
     switch (update_rule(c)) {
     case RULE_CEM:
@@ -1487,7 +1510,7 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
 }
 
 int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) {
-    const int NR = c->params.T * c->model.nu;
+    const int NR = ctrl_rows(c->params) * c->model.nu;
     float* hz_g = nullptr;                                                    // lambda Sigma_H^-1 U for K3's control cost
     switch (update_rule(c)) {
     case RULE_CEM:
@@ -1502,7 +1525,7 @@ int launch_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s) 
     default:
         break;
     }
-    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g, c->anneal);
+    mppib_shift_kernel<<<1, 256, NR * sizeof(float), s>>>(c->params, c->model.nu, U, plan_ctr, c->dist, hz_g, c->anneal, live_spline(c));
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

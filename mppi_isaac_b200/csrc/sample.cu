@@ -56,10 +56,14 @@ __device__ __forceinline__ SpecialRows special_rows(const MppibParams& p, uint32
 
 // The tail of every K1 but smooth at (t, j) of sample k: a = U + noise (0 on the null row) clamped to [u_min, u_max], prior_row on the
 // prior row, stored with noise := a - u.
+// The clamp of that tail: 0 on the null row, then [u_min, u_max] (spline MPPI applies it to the knots).
+__device__ __forceinline__ float clamp_action(const MppibParams& p, int j, float a, SpecialRows rows) {
+    if (rows.null) a = 0.f;
+    return fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+}
 __device__ __forceinline__ void clamp_store(const MppibParams& p, int nu, int t, int j, int k, float a, float u, SpecialRows rows,
                                             const float* __restrict__ prior_row, float* __restrict__ actions, float* __restrict__ noise) {
-    if (rows.null) a = 0.f;
-    a = fminf(fmaxf(a, p.u_min[j]), p.u_max[j]);
+    a = clamp_action(p, j, a, rows);
     if (rows.prior) a = prior_row[t * nu + j];
     const size_t idx = ((size_t)t * nu + j) * p.K + k;
     actions[idx] = a;
@@ -72,6 +76,15 @@ __device__ __forceinline__ void clamp_store(const MppibParams& p, int nu, int t,
 // is a column of the noise library, which mppib_noise_library has coloured by L0 already (FIXED) or left white (DIAG / FULL).
 // Annealed MPPI (srow = the s row of the iteration, FIXED only): noise_j := s[t] noise_j, one rounded multiplication, so a schedule of
 // ones changes no bit.
+// The FIXED colour of control j: sum_{i <= j} L0[j][i] z_i, summed from i = 0 upwards.
+__device__ __forceinline__ float fixed_colour(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int j) {
+    float n = 0.f;
+#pragma unroll
+    for (int i = 0; i < MPPIB_MAX_NU; ++i)
+        if (i <= j) n += p.sigma_chol[j * nu + i] * z[i];
+    return n;
+}
+
 template <Draw D, bool LIB = false>
 __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu, const float (&z)[MPPIB_MAX_NU], int t, int k, SpecialRows rows,
                                                    const float* __restrict__ U, const float* __restrict__ prior_row, float* __restrict__ actions,
@@ -90,9 +103,7 @@ __device__ __forceinline__ void colour_clamp_store(const MppibParams& p, int nu,
         } else if constexpr (LIB) {
             n = z[j];
         } else {
-#pragma unroll
-            for (int i = 0; i < MPPIB_MAX_NU; ++i)
-                if (i <= j) n += p.sigma_chol[j * nu + i] * z[i];
+            n = fixed_colour(p, nu, z, j);
             if (srow) n = __fmul_rn(srow[t], n);
         }
         const float u = U[t * nu + j];
@@ -299,6 +310,50 @@ mppib_sample_smooth_kernel(const __grid_constant__ MppibParams p, int nu, uint32
     }
 }
 
+// SPLINE (control_knots = P > 0, include/mppib.h "Spline MPPI"): K1 over the knots.  A CTA of 128 threads owns a tile of SP_S = 32
+// samples, lane = sample: warp w draws knots p = w, w + 4, ... with the Philox counters of mppib_sample (p in the t slot), colours them
+// with L0 (fixed_colour), clamps them (clamp_action, the null row included) into the tile's theta~ in shared memory and stores
+// xk = theta~ - theta (SIMPLE) or theta~ (MEAN); then warp w interpolates steps t = w, w + 4, ... with the table's row t (spline_apply)
+// and clamps the sum to [u_min, u_max].
+// With d = 1 and P = T every row is one weight 1.0, and actions / xk equal mppib_sample's actions / noise bit for bit.
+constexpr int SP_S = 32;            // samples per CTA
+constexpr int SP_MAX_N = 512;       // P*nu: the tile's knots take SP_MAX_N * SP_S * 4 = 64 KB of shared memory
+
+__global__ void __launch_bounds__(128)
+mppib_sample_spline_kernel(const __grid_constant__ MppibParams p, int nu, uint32_t key0, uint32_t seed_hi, uint64_t plan_idx,
+                           const uint32_t* __restrict__ plan_ctr, uint32_t k_offset, uint32_t k_total, const float* __restrict__ U,
+                           const float* __restrict__ spline, float* __restrict__ actions, float* __restrict__ xk) {
+    extern __shared__ __align__(16) float ths[];                             // [P*nu][SP_S] theta~ of the tile
+    const int K = p.K, T = p.T, P = p.control_knots, S = spline_row_floats(p.spline_degree);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int k = blockIdx.x * SP_S + lane;
+    const uint32_t kg = k_offset + (uint32_t)k;
+    const PhiloxKey key = philox_key(key0, seed_hi, plan_idx, plan_ctr);
+    const SpecialRows rows = special_rows(p, kg, k_total, false);
+    const bool mean = p.mode == MPPIB_MODE_MEAN;
+    for (int pk = warp; pk < P; pk += 4) {
+        float z[MPPIB_MAX_NU];
+#pragma unroll
+        for (int blk = 0; blk < MPPIB_MAX_NU / 4; ++blk)
+            if (blk * 4 < nu) philox_gauss4(key, kg, pk, blk, z + 4 * blk);
+#pragma unroll
+        for (int j = 0; j < MPPIB_MAX_NU; ++j) {
+            if (j >= nu) break;
+            const float th = U[pk * nu + j];
+            const float a = clamp_action(p, j, th + fixed_colour(p, nu, z, j), rows);
+            ths[(pk * nu + j) * SP_S + lane] = a;
+            if (k < K) xk[((size_t)pk * nu + j) * K + k] = mean ? a : a - th;
+        }
+    }
+    __syncthreads();
+    if (k >= K) return;
+    for (int t = warp; t < T; t += 4) {
+        const float* row = spline + t * S;
+        for (int j = 0; j < nu; ++j)   // the float32 weights sum to 1 only up to rounding: the clamp keeps a_t in the bounds
+            actions[((size_t)t * nu + j) * K + k] = fminf(fmaxf(spline_apply(row, ths + j * SP_S + lane, nu * SP_S), p.u_min[j]), p.u_max[j]);
+    }
+}
+
 // generalised Halton: radical inverse of `index` in base b with multiplicative digit scrambling (digit -> mult * digit mod b)
 __device__ __forceinline__ float halton(uint32_t index, uint32_t base, uint32_t mult) {
     const float inv_b = 1.0f / (float)base;
@@ -484,13 +539,25 @@ int check_modes_total(const MppibContext* c, const char* who, uint32_t k_total) 
 //   mppib_sample_smooth   SMOOTH (with its state); validate excludes n_worlds > 1 and n_modes > 1 from it
 //   mppib_noise_library   FIXED, DIAG, FULL, HORIZON: the library is white exactly for DIAG, FULL and HORIZON
 //   mppib_sample_library  FIXED, DIAG, FULL, HORIZON
+//   mppib_sample_spline   FIXED with control_knots > 0 and a matching spline table; every other entry refuses control_knots > 0
 // A registered annealing schedule goes through check_anneal in the two Philox entries; the library entries refuse one whatever its T.
 // args: the entry's required pointers are all non-null.
 int k1_admit(const MppibContext* c, K1Entry e, bool args, uint32_t k_offset, uint32_t k_total, int n_knots) {
-    static const char* const names[] = {"mppib_sample", "mppib_sample_colored", "mppib_sample_smooth", "mppib_noise_library", "mppib_sample_library"};
+    static const char* const names[] = {"mppib_sample", "mppib_sample_colored", "mppib_sample_smooth", "mppib_noise_library", "mppib_sample_library",
+                                        "mppib_sample_spline"};
     const char* who = names[e];
     const bool lib = e == K1_NOISE_LIBRARY || e == K1_SAMPLE_LIBRARY;
     MPPIB_REQUIRE(c && args, "%s: null argument", who);
+    if (e == K1_SPLINE) {
+        MPPIB_REQUIRE(c->params.control_knots > 0, "%s: needs control_knots > 0 (spline MPPI)", who);
+        if (int rc = check_spline(c, who)) return rc;
+        MPPIB_REQUIRE((uint64_t)k_offset + (uint64_t)c->params.K <= (uint64_t)k_total, "%s: shard [%u,+%d) exceeds k_total %u", who, k_offset,
+                      c->params.K, k_total);
+        MPPIB_REQUIRE(c->params.control_knots * c->model.nu <= SP_MAX_N, "%s: needs P*nu <= %d, got %d", who, SP_MAX_N,
+                      c->params.control_knots * c->model.nu);
+        return 0;
+    }
+    MPPIB_REQUIRE(c->params.control_knots == 0, "%s: control_knots > 0 samples through mppib_sample_spline", who);
     if (e == K1_SAMPLE || e == K1_COLORED)
         if (int rc = check_anneal(c, who)) return rc;
     const bool in_range = (uint64_t)k_offset + (uint64_t)c->params.K <= (uint64_t)k_total;
@@ -567,6 +634,17 @@ int launch_sample_smooth(MppibContext* c, uint64_t seed, uint64_t plan_idx, cons
     if (int rc = ensure_smem<mppib_sample_smooth_kernel>(c->device, smem)) return rc;
     mppib_sample_smooth_kernel<<<(K + SM_S - 1) / SM_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
                                                                       k_offset, k_total, U, actions, noise, c->smooth);
+    MPPIB_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_sample_spline(MppibContext* c, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset, uint32_t k_total,
+                         const float* U, float* actions, float* xk, cudaStream_t s) {
+    const int K = c->params.K, nu = c->model.nu;
+    const int smem = (int)sizeof(float) * c->params.control_knots * nu * SP_S;
+    if (int rc = ensure_smem<mppib_sample_spline_kernel>(c->device, smem)) return rc;
+    mppib_sample_spline_kernel<<<(K + SP_S - 1) / SP_S, 128, smem, s>>>(c->params, nu, (uint32_t)seed, (uint32_t)(seed >> 32), plan_idx, plan_ctr,
+                                                                      k_offset, k_total, U, live_spline(c), actions, xk);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 21
+ABI_VERSION = 22
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -34,6 +34,7 @@ MAX_WORLDS = 32                                 # risk-aware MPPI: largest n_wor
 MAX_MODES = 16                                  # multi-modal MPPI: largest n_modes
 MAX_ANNEAL = 16                                 # annealed MPPI: largest anneal_iterations
 ANNEAL_MIN_SCALE = 2.0 ** -20                   # annealed MPPI: smallest noise scale, so that r = 1 / s^2 stays finite in float32
+MAX_SPLINE_DEGREE = 3                           # spline MPPI: largest spline_degree
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -84,6 +85,7 @@ class MppibParams(C.Structure):
         ("du_min", f32 * MAX_NU), ("du_max", f32 * MAX_NU), ("smooth_weight", f32),
         ("n_worlds", i32), ("risk_tail", i32),
         ("n_modes", i32), ("mode_margin", f32), ("mode_samples", i32),
+        ("control_knots", i32), ("spline_degree", i32),
     ]
 
 
@@ -538,6 +540,99 @@ def _anneal_params(p: MppibParams, mppi_cfg) -> None:
         raise ValueError("annealed MPPI excludes n_modes > 1: the Stein coupling's Sigma^-1 metric would need the schedule")
 
 
+def spline_knot_vector(T: int, P: int, d: int):
+    """The clamped uniform knot vector of spline MPPI on [0, T-1] (float64): d+1 zeros, i (T-1) / (P-d) for i = 1 .. P-d-1, d+1 copies
+    of T-1.  The interior knots are integers divided once, so they are exact wherever the quotient is."""
+    inner = [i * (T - 1) / (P - d) for i in range(1, P - d)]
+    return np.array([0.0] * (d + 1) + inner + [float(T - 1)] * (d + 1), np.float64)
+
+
+def _bspline_row(u, P: int, d: int, x: float):
+    """(P,) float64 values N_{p,d}(x) of the B-splines of knot vector u by Cox-de Boor (0/0 = 0); at the right end x = u[-1] the last
+    basis function is 1."""
+    if x >= u[-1]:
+        row = np.zeros(P)
+        row[P - 1] = 1.0
+        return row
+    N = np.array([1.0 if u[i] <= x < u[i + 1] else 0.0 for i in range(len(u) - 1)])
+    for k in range(1, d + 1):
+        M = np.zeros(len(u) - 1 - k)
+        for i in range(len(M)):
+            a = (x - u[i]) / (u[i + k] - u[i]) * N[i] if u[i + k] > u[i] else 0.0
+            b = (u[i + k + 1] - x) / (u[i + k + 1] - u[i + 1]) * N[i + 1] if u[i + k + 1] > u[i + 1] else 0.0
+            M[i] = a + b
+        N = M
+    return N[:P]
+
+
+def spline_basis(T: int, P: int, d: int):
+    """(B, S, xi) in float64 of spline MPPI (DESIGN.md section 2, "Spline MPPI"): B[T][P] = N_{p,d}(t) at the steps, xi[P] the Greville
+    abscissae (u_{p+1} + ... + u_{p+d}) / d, and the shift map S[P][P] with row p = N(xi_p + 1) where xi_p + 1 <= T-1 and NaN otherwise
+    (that knot takes u_init)."""
+    u = spline_knot_vector(T, P, d)
+    B = np.stack([_bspline_row(u, P, d, float(t)) for t in range(T)])
+    xi = np.array([u[p + 1:p + d + 1].sum() / d for p in range(P)])
+    S = np.full((P, P), np.nan)
+    for p in range(P):
+        if xi[p] + 1.0 <= T - 1:
+            S[p] = _bspline_row(u, P, d, xi[p] + 1.0)
+    return B, S, xi
+
+
+def spline_table(T: int, P: int, d: int, nu: int, theta=None):
+    """The float32 spline table of include/mppib.h (mppib_set_spline): rows[T + P][d + 3] of (first, count, weights) over the non-zero
+    weights of B's rows, then of the shift rows (count 0: u_init), then U_exec[T][nu] = B theta (zeros without theta), from float64
+    rounded once."""
+    B, S, _ = spline_basis(T, P, d)
+    rows = np.zeros((T + P, d + 3), np.float64)
+    for r, w in enumerate(list(B) + list(S)):
+        if np.isnan(w).any():
+            continue
+        nz = np.nonzero(w)[0]
+        lo, hi = int(nz[0]), int(nz[-1])
+        rows[r, 0], rows[r, 1] = lo, hi - lo + 1
+        rows[r, 2:2 + hi - lo + 1] = w[lo:hi + 1]
+    ue = np.zeros((T, nu)) if theta is None else B @ np.asarray(theta, np.float64).reshape(P, nu)
+    return np.concatenate([rows.reshape(-1), ue.reshape(-1)]).astype(np.float32)
+
+
+def spline_initial_knots(T: int, P: int, d: int, U_init):
+    """(P, nu) float32 knots of a (T, nu) initial sequence: theta_p = U_init at xi_p by linear interpolation of its rows, in float64."""
+    _, _, xi = spline_basis(T, P, d)
+    U = np.asarray(U_init, np.float64).reshape(T, -1)
+    return np.stack([np.interp(xi, np.arange(T, dtype=np.float64), U[:, j]) for j in range(U.shape[1])], axis=1).astype(np.float32)
+
+
+def _spline_params(p: MppibParams, mppi_cfg, nu: int) -> None:
+    """The `control_knots` / `spline_degree` keys of spline MPPI (DESIGN.md section 2, "Spline MPPI") and what they exclude.  P = 0 leaves
+    both fields 0, so the block is today's byte for byte."""
+    P, d = int(getattr(mppi_cfg, "control_knots", 0)), int(getattr(mppi_cfg, "spline_degree", 1))
+    if P < 0:
+        raise ValueError(f"control_knots = {P} must be >= 0 (0: off)")
+    if P == 0:
+        return
+    if not 1 <= d <= MAX_SPLINE_DEGREE:
+        raise ValueError(f"spline_degree = {d} must be 1, 2 or 3")
+    if not d + 1 <= P <= p.T:
+        raise ValueError(f"control_knots = {P} must lie in spline_degree + 1 = {d + 1} .. horizon = {p.T}")
+    if P * nu > 512 or p.T > 256:
+        raise ValueError(f"control_knots needs control_knots * nu <= 512 and horizon <= 256; P*nu = {P * nu}, T = {p.T}")
+    method = str(getattr(mppi_cfg, "sampling_method", "halton"))
+    if method in ("halton", "colored"):
+        raise ValueError(f"control_knots > 0 samples its knots with sampling_method random, not {method}")
+    if p.mode == MODE_CEM or p.mode == MODE_SMOOTH:
+        raise ValueError("control_knots > 0 excludes mppi_mode cem and smooth")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("control_knots > 0 excludes update_cov and update_lambda")
+    if p.n_modes > 1 or p.n_worlds > 1:
+        raise ValueError("control_knots > 0 excludes n_modes > 1 and n_worlds > 1")
+    if anneal_on(mppi_cfg):
+        raise ValueError("control_knots > 0 excludes annealed MPPI")
+    if p.filter_u:
+        raise ValueError("control_knots > 0 excludes filter_u: the spline is smooth already, switch filter_u off")
+    p.control_knots, p.spline_degree = P, d
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -617,6 +712,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     _risk_params(p, mppi_cfg, int(K_local))
     _modes_params(p, mppi_cfg)
     _anneal_params(p, mppi_cfg)
+    _spline_params(p, mppi_cfg, nu)
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

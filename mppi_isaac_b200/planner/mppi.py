@@ -27,7 +27,8 @@ import os
 import torch
 
 from ..backend import shard_row_floats
-from ..model.blob import ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule
+from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule, spline_basis, spline_initial_knots,
+                          spline_table)
 
 
 class _NoRange:
@@ -226,7 +227,15 @@ class MPPIPlanner:
             sigma = np.asarray(cfg.noise_sigma, np.float64).reshape(self.nu, self.nu)
             if np.any(sigma != np.diag(np.diag(sigma))):
                 raise ValueError("update_cov adapts a diagonal covariance: noise_sigma must be diagonal")
+        # spline MPPI (DESIGN.md section 2, "Spline MPPI"): U is P knots per control of a degree-d B-spline over the horizon; K1 samples
+        # the knots and interpolates the actions, K3 / K4 run on the knots; make_params checks the keys against the mode
+        self.control_knots = int(getattr(cfg, "control_knots", 0))
+        self.spline_degree = int(getattr(cfg, "spline_degree", 1))
+        if self.control_knots > 0 and bool(getattr(cfg, "use_priors", False)) and prior is not None:
+            raise ValueError("control_knots > 0 does not take a prior: the prior row is an action sequence and cannot be written as knots")
         self.backend = sim.backend
+        if self.control_knots > 0 and not hasattr(self.backend, "set_spline"):
+            raise ValueError(f"control_knots > 0 needs a backend with set_spline ({type(self.backend).__name__} has none)")
         if self.adaptive and not hasattr(self.backend, "set_distribution"):
             raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
         if self.cem and not hasattr(self.backend, "set_distribution"):
@@ -300,10 +309,14 @@ class MPPIPlanner:
         dev, T, nu, K = self.device, self.T, self.nu, self.K
         f32 = dict(dtype=torch.float32, device=dev)
         M = self.n_modes
-        self.U = torch.zeros((T, nu), **f32) if M == 1 else torch.zeros((M, T, nu), **f32)
+        Pk, d = self.control_knots, self.spline_degree
+        Tc = Pk or T                                         # rows of U: the knots with control_knots > 0, the steps otherwise
+        self.U = torch.zeros((Tc, nu), **f32) if M == 1 else torch.zeros((M, T, nu), **f32)
         U0 = self.U if M == 1 else self.U[0]
         U_init = getattr(self.cfg, "U_init", None)
-        if U_init is not None:
+        if U_init is not None and Pk:
+            U0.copy_(torch.from_numpy(spline_initial_knots(T, Pk, d, U_init)))
+        elif U_init is not None:
             U0.copy_(torch.as_tensor(U_init, dtype=torch.float32).reshape(T, nu))
         else:
             U0 += torch.as_tensor(self.backend.params.u_init[:nu], dtype=torch.float32).to(dev)
@@ -311,6 +324,15 @@ class MPPIPlanner:
             self.U[1:].copy_(torch.from_numpy(mode_starts(self.backend.params, nu, U0.cpu().numpy(), M, self.seed)))
         self.actions = torch.zeros((T, nu, K), **f32)       # [T][nu][K]
         self.noise = torch.zeros((T, nu, K), **f32)
+        # spline MPPI: the knot samples xk[P][nu][K] K3 weights (theta~ - U in SIMPLE mode, theta~ in MEAN mode) and the table
+        # (rows, U_exec) K1 / K4 / the shift read; a planner rebuilt with control_knots = 0 registers none
+        self.xk, self.spline_table = None, None
+        if Pk:
+            self.xk = torch.zeros((Pk, nu, K), **f32)
+            self.spline_table = torch.from_numpy(spline_table(T, Pk, d, nu, U0.cpu().numpy())).to(dev)
+            self.backend.set_spline(self.spline_table)
+        elif hasattr(self.backend, "set_spline"):
+            self.backend.set_spline(None)
         self.cost = torch.zeros((T, K), **f32)
         P = shard_row_floats(self.backend.params, nu)
         self.partial = torch.zeros((P,), **f32)
@@ -399,10 +421,20 @@ class MPPIPlanner:
         self.Z = torch.zeros((T, nu, K), dtype=torch.float32, device=dev)
         self.backend.noise_library(self.k_offset, self.K_total, self._halton_tab, self._spline_B, n_knots, self.Z)
 
+    def refresh_mean_action(self):
+        """Spline MPPI: recompute U_exec = B U (float64, rounded once) after U was written from outside a plan (a warm start)."""
+        if self.spline_table is not None:
+            T, nu = self.T, self.nu
+            B, _, _ = spline_basis(T, self.control_knots, self.spline_degree)
+            ue = (B @ self.U.detach().cpu().double().numpy()).astype("float32")
+            self.mean_action.copy_(torch.from_numpy(ue))
+
     def _sample(self, iteration=0):
         be = self.backend
         # iteration i of a plan (cem, or annealed MPPI) keys Philox with plan_idx = i << 32: iteration 0 draws what a one-iteration plan draws
-        if self.cem:
+        if self.xk is not None:
+            be.sample_spline(self.seed, 0, self.k_offset, self.K_total, self.U, self.actions, self.xk, self.plan_ctr)
+        elif self.cem:
             be.sample_colored(self.seed, iteration << 32, self.k_offset, self.K_total, self.U, None, self._noise_Lt, self.actions, self.noise,
                               self.plan_ctr)
         elif self.smooth:
@@ -441,10 +473,23 @@ class MPPIPlanner:
     @property
     def mean_action(self):
         """(T, nu) device view of the nominal sequence U; with mppi_mode smooth that is the mean of the control DERIVATIVE (the
-        planned actions are ``action_sequence``); with n_modes > 1 the sequence of the executed mode after the last plan."""
+        planned actions are ``action_sequence``); with n_modes > 1 the sequence of the executed mode after the last plan; with
+        control_knots > 0 the interpolated sequence U_exec = B U that K4 writes."""
+        if self.spline_table is not None:
+            return self.spline_table[-self.T * self.nu:].view(self.T, self.nu)
         if self.mode_state is not None:
             return self.mode_state[1 + self.n_modes:].view(self.T, self.nu)
         return self.U
+
+    @property
+    def knots(self):
+        """(P, nu) device view of the control knots of spline MPPI (U itself; None with control_knots = 0)."""
+        return self.U if self.xk is not None else None
+
+    @property
+    def knot_samples(self):
+        """(P, nu, K) device buffer of the last plan's knot samples of spline MPPI (None with control_knots = 0)."""
+        return self.xk
 
     @property
     def modes(self):
@@ -558,6 +603,12 @@ class MPPIPlanner:
             torch.distributed.all_gather(rows, self.partial, group=self.pg)
         return self.partials, self.world
 
+    def _weighted(self):
+        """The samples K3 weights: the knot samples with control_knots > 0, else noise (SIMPLE, smooth) or actions (MEAN)."""
+        if self.xk is not None:
+            return self.xk
+        return self.noise if self.backend.params.mode in (MODE_SIMPLE, MODE_SMOOTH) else self.actions
+
     def _plan_batched(self):
         be = self.backend
         with _nvtx("mppi/shift"):
@@ -573,7 +624,7 @@ class MPPIPlanner:
             self.sim.rollout_all(self.actions)
         with _nvtx("mppi/objective cost"):
             cost = self._cost_batched()
-        x = self.noise if be.params.mode in (MODE_SIMPLE, MODE_SMOOTH) else self.actions
+        x = self._weighted()
         with _nvtx("mppi/K3 reduce + exchange + K4 update"):
             if self.world == 1 and hasattr(be, "reduce_finalize"):
                 be.reduce_finalize(cost, x, self.U, self.partial, self._action, self.stats)      # K3 + K4 in one launch
@@ -607,7 +658,7 @@ class MPPIPlanner:
         if self.use_priors and prior_local:
             row = self.K_total - 2 - self.k_offset
             self.noise[:, :, row] = self.actions[:, :, row] - self.U
-        x = self.noise if be.params.mode in (MODE_SIMPLE, MODE_SMOOTH) else self.actions
+        x = self._weighted()
         be.reduce(self.cost, x, self.U, self.partial)
         partials, G = self._exchange()
         be.finalize(partials, G, self.U, self._action, self.stats)

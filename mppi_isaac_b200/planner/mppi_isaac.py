@@ -84,6 +84,7 @@ class MPPIisaacPlanner(object):
             if old.mode_state is not None and self.mppi.mode_state is not None and old.mode_state.shape == self.mppi.mode_state.shape:
                 self.mppi.mode_state.copy_(old.mode_state)       # and, with n_modes > 1, the executed mode and its free energies
             # the annealing schedule is rebuilt from the config, not carried over: a keep_U rebuild starts from the configured decays
+            self.mppi.refresh_mean_action()              # spline MPPI: U_exec of the carried knots
 
     def _make_mppi(self):
         return MPPIPlanner(

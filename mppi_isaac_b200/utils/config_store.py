@@ -52,6 +52,8 @@ class MPPIConfig:
     anneal_iterations: int = 1           # annealed MPPI (DESIGN.md section 2): N MPPI iterations per plan, 1 .. 16
     anneal_iter_decay: float = 1.0       # annealed MPPI: c_i in (0, 1], the noise std factor per iteration
     anneal_horizon_decay: float = 1.0    # annealed MPPI: c_h in (0, 1], the noise std factor per step towards the start of the horizon
+    control_knots: int = 0               # spline MPPI (DESIGN.md section 2): P control knots per horizon, interpolated to every step; 0 = off
+    spline_degree: int = 1               # spline MPPI: B-spline degree d in 1 .. 3, P in d + 1 .. horizon
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0
