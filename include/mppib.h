@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 22
+#define MPPIB_ABI_VERSION 23
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -236,6 +236,11 @@ typedef struct MppibParams {
     int32_t n_modes;           /* M in 1 .. MPPIB_MAX_MODES nominal sequences planned side by side                                   */
     float   mode_margin;       /* >= 0: the executed mode is kept while its free energy is within this margin of the lowest          */
     int32_t mode_samples;      /* Kc = K_total / M >= 32: global sample kg belongs to mode kg / Kc (the shard alone cannot tell K_total) */
+    /* constrained MPPI (see "Constrained MPPI" below); constraint_mode = 0 (and a zero-initialised block) keeps today's planner        */
+    int32_t constraint_mode;   /* 1: feasibility-first weighting over the per-step violations registered with mppib_set_constraint      */
+    float   constraint_tol;    /* a sample is feasible when its total violation V_k <= tol; finite and >= 0                             */
+    float   constraint_lambda; /* lambda_c: the temperature of the violation fallback; finite and > 0                                    */
+    int32_t constraint_pad;    /* 0; keeps the spline fields below at the 8-byte alignment they had before the constraint fields       */
     /* spline MPPI (see "Spline MPPI" below); control_knots = 0 (and a zero-initialised block) keeps today's planner                   */
     int32_t control_knots;     /* P: U, the samples K3 weights and the shard row hold P knots per control instead of T steps            */
     int32_t spline_degree;     /* d in 1 .. MPPIB_MAX_SPLINE_DEGREE, read only when control_knots > 0; P in d + 1 .. T, P*nu <= 512   */
@@ -540,6 +545,28 @@ int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations);
 int32_t mppib_set_spline(MppibHandle h, float* table, int32_t P, int32_t d);
 int32_t mppib_sample_spline(MppibHandle h, uint64_t seed, uint64_t plan_idx, const uint32_t* plan_ctr, uint32_t k_offset,
                             uint32_t k_total, const float* U, float* actions, float* xk, void* stream);
+
+/* Constrained MPPI (constraint_mode = 1; modes SIMPLE and MEAN with the fixed Sigma, any K1 that feeds the plain rule -- Gaussian,
+ * colored, Halton library -- filter_u, the null / prior rows and any number of ranks; no update_cov / update_lambda, cem, smooth,
+ * n_modes > 1, n_worlds > 1, annealing or control_knots > 0).  The Objective returns a signed margin g[t][k] per step (<= 0 satisfied,
+ * > 0 the amount of violation) into a device buffer registered with mppib_set_constraint (caller-owned, written by the caller before
+ * every K3):
+ *   viol     [T][K]  g of the shard's samples, float32
+ *   cstate   [2]     (n_feasible as int32 bits, min V) of the last plan, written by K4
+ *   K3     per sample V_k = sum_t c[t][k] in t order in float32, c = g where g > 0, 0 where g <= 0 (NaN stays NaN); valid = today's
+ *          validity and V_k finite, feasible = valid and V_k <= constraint_tol.  A tile holding a feasible sample weights its feasible
+ *          samples by exp(-(S_k - b)/lambda) (S_k as today); one without weights its valid samples by exp(-(V_k - b)/lambda_c) (no
+ *          control cost, no gamma^t).  The states (n_feasible, b, eta, W) merge lexicographically: one with n_feasible > 0 beats one
+ *          with 0 (which then weighs 0), two of one kind merge by today's rescale with their temperature and add their counts
+ *          (feas_scale in csrc/common.cuh, the same function at every fold).  The shard row is
+ *   partial  [4 + T*nu]  (beta, eta, W[T*nu], n_feasible as int32 bits, min V over the shard's valid samples (+inf: none))
+ *   K4     mppib_finalize (or the fused tail) merges the G rows the same way, then today's update, Savitzky-Golay, clamp, action, mirror;
+ *          stats = (beta, eta) of the kind that won, cstate = (sum n_feasible, min V).  No valid sample anywhere: U unchanged.
+ *   shift  unchanged.
+ * With every g <= 0 each sample is feasible exactly when it is valid today, and every weight, sum and scale is today's: the plan equals
+ * today's bit for bit.  Registration records (T, K); reduce and finalize refuse a handle whose constraint_mode and registration disagree
+ * or whose T or K changed since, and one with a distribution or annealing schedule registered.  NULL switches it off.             */
+int32_t mppib_set_constraint(MppibHandle h, const float* viol, float* cstate);
 
 #ifdef __cplusplus
 }

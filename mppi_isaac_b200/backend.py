@@ -25,7 +25,7 @@ SYMBOLS = [
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
     "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth", "mppib_set_anneal",
-    "mppib_set_spline", "mppib_sample_spline",
+    "mppib_set_spline", "mppib_sample_spline", "mppib_set_constraint",
 ]
 
 
@@ -79,7 +79,8 @@ def shard_row_floats(params, nu):
     """Floats of one shard row that K3 (or the elite kernel of mppi_mode cem) writes under `params` with `nu` inputs once a
     distribution is registered, as the library sizes its buffers (shard_row_floats in csrc/common.cuh): 2 + T*nu, + T*nu with
     update_cov, + nu(nu+1)/2 with cov_full, + n(n+1)/2 with cov_horizon (n = T*nu); n_modes * (2 + T*nu) with n_modes > 1;
-    cem_row_floats with mppi_mode cem.  With control_knots = P > 0 the control vector is P*nu long (ctrl_rows in csrc/common.cuh)."""
+    cem_row_floats with mppi_mode cem; 4 + T*nu with constraint_mode (the row adds n_feasible and min V).  With control_knots = P > 0
+    the control vector is P*nu long (ctrl_rows in csrc/common.cuh)."""
     T, nu = int(params.T), int(nu)
     n = (int(params.control_knots) or T) * nu
     if params.mode == MODE_CEM:
@@ -90,7 +91,9 @@ def shard_row_floats(params, nu):
         return 2 + n + n * (n + 1) // 2
     if params.update_cov and params.cov_full:
         return 2 + n + nu * (nu + 1) // 2
-    return 2 + n * (2 if params.update_cov else 1)
+    if params.update_cov or params.update_lambda:
+        return 2 + n * (2 if params.update_cov else 1)
+    return 4 + n if params.constraint_mode else 2 + n
 
 
 def smooth_state_floats(T, nu):
@@ -144,6 +147,7 @@ class CudaBackend:
         self._smooth_keepalive = None
         self._anneal_keepalive = None     # (state, N)
         self._spline_keepalive = None     # the registered spline table
+        self._constraint_keepalive = None  # (viol, cstate) of constrained MPPI
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -173,6 +177,11 @@ class CudaBackend:
                     and table.numel() == spline_table_floats(params.T, P, d, model.nu)
                     and self.lib.mppib_set_spline(self.handle, _ptr(table), C.c_int32(P), C.c_int32(d)) == 0):
                 self._spline_keepalive = None
+        if self._constraint_keepalive is not None:       # ... and its violation buffer, while the block still plans with it for the same (T, K)
+            viol, cstate = self._constraint_keepalive
+            if not (params.constraint_mode and viol.numel() == int(params.T) * int(params.K)
+                    and self.lib.mppib_set_constraint(self.handle, _ptr(viol), _ptr(cstate)) == 0):
+                self._constraint_keepalive = None
 
     def destroy(self):
         if self.handle:
@@ -350,6 +359,18 @@ class CudaBackend:
                                    f"{table.dtype} {table.numel()}")
         self._check(self.lib.mppib_set_spline(self.handle, _ptr(table), C.c_int32(P), C.c_int32(d)), "mppib_set_spline")
         self._spline_keepalive = None if table is None else (table, P, d)
+
+    def set_constraint(self, viol, cstate=None):
+        """Constrained MPPI: register the (T, K) float32 device tensor of per-step constraint margins K3 reads and the (2,) float32
+        device tensor (n_feasible as int32 bits, min V) K4 writes (None switches it off).  The library records (T, K)."""
+        if viol is not None:
+            T, K = int(self.params.T), int(self.params.K)
+            if viol.numel() != T * K or viol.dtype != torch.float32 or not viol.is_contiguous():
+                raise RuntimeError(f"mppib_set_constraint: viol must be a contiguous float32 (T, K) = ({T}, {K}) tensor, got {viol.dtype} {tuple(viol.shape)}")
+            if cstate is None or cstate.numel() != 2 or cstate.dtype != torch.float32:
+                raise RuntimeError("mppib_set_constraint: cstate must be a float32 tensor of 2 values")
+        self._check(self.lib.mppib_set_constraint(self.handle, _ptr(viol), _ptr(None if viol is None else cstate)), "mppib_set_constraint")
+        self._constraint_keepalive = None if viol is None else (viol, cstate)
 
     def sample_spline(self, seed, plan_idx, k_offset, k_total, U, actions, xk, plan_ctr=None):
         """K1 of spline MPPI: knots theta~ = clamp(U + L0 z) per sample, xk[P][nu][K] = theta~ - U (SIMPLE) or theta~ (MEAN), and

@@ -98,6 +98,15 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->n_modes <= 1 && p->n_worlds <= 1, "control_knots > 0 excludes n_modes > 1 and n_worlds > 1");
         MPPIB_REQUIRE(!p->filter_u, "control_knots > 0 excludes filter_u: the spline is smooth already, switch filter_u off");
     }
+    MPPIB_REQUIRE(p->constraint_mode == 0 || p->constraint_mode == 1, "constraint_mode = %d must be 0 or 1", p->constraint_mode);
+    if (p->constraint_mode) {
+        MPPIB_REQUIRE(isfinite(p->constraint_tol) && p->constraint_tol >= 0.f, "constraint_tol = %g must be finite and >= 0", p->constraint_tol);
+        MPPIB_REQUIRE(isfinite(p->constraint_lambda) && p->constraint_lambda > 0.f, "constraint_lambda = %g must be finite and > 0", p->constraint_lambda);
+        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "constraint_mode excludes mode cem and mode smooth");
+        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "constraint_mode excludes update_cov and update_lambda");
+        MPPIB_REQUIRE(p->n_modes <= 1 && p->n_worlds <= 1, "constraint_mode excludes n_modes > 1 and n_worlds > 1");
+        MPPIB_REQUIRE(p->control_knots == 0, "constraint_mode excludes control_knots > 0");
+    }
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -153,6 +162,19 @@ int check_spline(const MppibContext* c, const char* who) {
                   "for the new block (mppib_set_spline)", who, c->spline_T, c->spline_P, c->spline_d, c->spline_nu, p.T, p.control_knots,
                   p.spline_degree, c->model.nu);
     MPPIB_REQUIRE(update_rule(c) == RULE_PLAIN, "%s: control_knots > 0 runs plain MPPI; register no distribution", who);
+    return 0;
+}
+
+int check_constraint(const MppibContext* c, const char* who) {
+    const MppibParams& p = c->params;
+    if (!p.constraint_mode) {
+        MPPIB_REQUIRE(c->viol == nullptr, "%s: a constraint buffer is registered but constraint_mode is 0; register none (mppib_set_constraint(h, NULL, NULL))", who);
+        return 0;
+    }
+    MPPIB_REQUIRE(c->viol != nullptr, "%s: constraint_mode needs its violation buffer registered (mppib_set_constraint)", who);
+    MPPIB_REQUIRE(c->viol_T == p.T && c->viol_K == p.K, "%s: the violation buffer was registered for (T, K) = (%d, %d), the handle has (%d, %d); register a "
+                  "buffer for the new block (mppib_set_constraint)", who, c->viol_T, c->viol_K, p.T, p.K);
+    MPPIB_REQUIRE(c->dist == nullptr && c->anneal == nullptr, "%s: constraint_mode runs plain MPPI; register no distribution and no annealing schedule", who);
     return 0;
 }
 
@@ -343,6 +365,7 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
     MPPIB_REQUIRE(h && cost && x && U && partial, "mppib_reduce: null argument");
     if (int rc = check_anneal(h, "mppib_reduce")) return rc;
     if (int rc = check_spline(h, "mppib_reduce")) return rc;
+    if (int rc = check_constraint(h, "mppib_reduce")) return rc;
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
@@ -352,6 +375,7 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
     MPPIB_REQUIRE(h && cost && x && U && partial && action_out, "mppib_reduce_finalize: null argument");
     if (int rc = check_anneal(h, "mppib_reduce_finalize")) return rc;
     if (int rc = check_spline(h, "mppib_reduce_finalize")) return rc;
+    if (int rc = check_constraint(h, "mppib_reduce_finalize")) return rc;
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, U, action_out, stats, (cudaStream_t)stream);
@@ -361,6 +385,7 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
     MPPIB_REQUIRE(h && U && action_out && G >= 1, "mppib_finalize: bad argument");
     if (int rc = check_anneal(h, "mppib_finalize")) return rc;
     if (int rc = check_spline(h, "mppib_finalize")) return rc;
+    if (int rc = check_constraint(h, "mppib_finalize")) return rc;
     if (!partials) {
         MPPIB_REQUIRE(h->peer_world >= 2 && G == h->peer_world, "mppib_finalize: partials == NULL needs an open peer window and G == world (G=%d, world=%d)", G, h->peer_world);
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
@@ -431,6 +456,19 @@ int32_t mppib_set_spline(MppibHandle h, float* table, int32_t P, int32_t d) {
                   "mppib_set_spline: (P, d) = (%d, %d) does not match the parameter block's (control_knots, spline_degree) = (%d, %d)", P, d,
                   h->params.control_knots, h->params.spline_degree);
     h->spline = table; h->spline_T = h->params.T; h->spline_P = P; h->spline_d = d; h->spline_nu = h->model.nu;
+    return 0;
+}
+
+int32_t mppib_set_constraint(MppibHandle h, const float* viol, float* cstate) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    if (viol == nullptr) {
+        h->viol = nullptr; h->cstate = nullptr; h->viol_T = h->viol_K = 0;
+        return 0;
+    }
+    MPPIB_REQUIRE(cstate != nullptr, "mppib_set_constraint: the constraint state (n_feasible, min V) is needed with a violation buffer");
+    MPPIB_REQUIRE(h->params.constraint_mode, "mppib_set_constraint: the parameter block has constraint_mode = 0");
+    MPPIB_REQUIRE(((uintptr_t)viol & 15) == 0, "mppib_set_constraint: viol must be 16-byte aligned");
+    h->viol = viol; h->cstate = cstate; h->viol_T = h->params.T; h->viol_K = h->params.K;
     return 0;
 }
 

@@ -52,6 +52,9 @@ struct MppibContext {
     int anneal_n, anneal_T;                    // N iterations and the horizon T the schedule was registered for
     float* spline;                             // spline MPPI: device (rows[T + P][d + 3], U_exec[T][nu]), read by K1 / K4 / shift, U_exec written by K4 (nullable)
     int spline_T, spline_P, spline_d, spline_nu;   // the (T, P, d, nu) the table was registered for
+    const float* viol;                         // constrained MPPI: device g[T][K] K3 reads (nullable)
+    float* cstate;                             // constrained MPPI: device (n_feasible as int bits, min V), written by K4
+    int viol_T, viol_K;                        // the (T, K) the buffer was registered for
     // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
     float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
     float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
@@ -102,7 +105,7 @@ static inline float* live_spline(const MppibContext* c) { return c->params.contr
 
 // The update rule a plan runs: which K3 (or elite kernel), K4 and shift, and what their shard row carries.  Risk-aware MPPI is not a
 // rule but a K3 flag (risk_mode) that combines with PLAIN, DIST and FULL.
-enum Rule { RULE_PLAIN, RULE_DIST, RULE_FULL, RULE_HORIZON, RULE_SMOOTH, RULE_MODES, RULE_CEM };
+enum Rule { RULE_PLAIN, RULE_DIST, RULE_FULL, RULE_HORIZON, RULE_SMOOTH, RULE_MODES, RULE_CEM, RULE_FEASIBLE };
 // Floats of one shard row (T: the control rows, ctrl_rows() of the parameter block):
 //   PLAIN, SMOOTH  (beta, eta, W[T*nu])
 //   DIST           (beta, eta, W[T*nu]), + M2[T*nu] with update_cov
@@ -110,6 +113,7 @@ enum Rule { RULE_PLAIN, RULE_DIST, RULE_FULL, RULE_HORIZON, RULE_SMOOTH, RULE_MO
 //   HORIZON        (beta, eta, W[n], C[n(n+1)/2]), n = T*nu
 //   MODES          (beta, eta, W[T*nu]) of every mode
 //   CEM            (S, index bits)[E] + actions[E][T*nu], padded to 4 floats, E = n_elites
+//   FEASIBLE       (beta, eta, W[T*nu], n_feasible as int bits, min V)
 // The kernels pass the parts they already hold (T, update_cov, ...); the host passes the parameter block.
 __host__ __device__ inline int shard_row_floats(Rule r, int T, int nu, bool update_cov, int n_modes, int E) {
     const int NR = T * nu;
@@ -119,6 +123,7 @@ __host__ __device__ inline int shard_row_floats(Rule r, int T, int nu, bool upda
     case RULE_HORIZON: return 2 + NR + NR * (NR + 1) / 2;
     case RULE_MODES: return n_modes * (2 + NR);
     case RULE_CEM: return (2 * E + E * T * nu + 3) & ~3;
+    case RULE_FEASIBLE: return 4 + NR;
     default: return 2 + NR;
     }
 }
@@ -140,6 +145,7 @@ static inline Rule update_rule(const MppibContext* c) {
     if (adaptive_horizon(c)) return RULE_HORIZON;
     if (adaptive_full(c)) return RULE_FULL;
     if (c->dist) return RULE_DIST;
+    if (c->viol && c->params.constraint_mode) return RULE_FEASIBLE;
     return RULE_PLAIN;
 }
 // The draw K1 makes for the rule: the colour of the white draws (FIXED L0, DIAG / FULL / HORIZON the live adaptive ones, CEM the
@@ -164,6 +170,7 @@ static inline Rule configured_rule(const MppibParams& p) {
     if (p.update_cov && p.cov_horizon) return RULE_HORIZON;
     if (p.update_cov && p.cov_full) return RULE_FULL;
     if (p.update_cov || p.update_lambda) return RULE_DIST;
+    if (p.constraint_mode) return RULE_FEASIBLE;
     return RULE_PLAIN;
 }
 static inline int partial_row_capacity(const MppibParams& p, int nu) { return shard_row_floats(configured_rule(p), p, nu); }
@@ -182,6 +189,20 @@ __device__ __forceinline__ const float* anneal_row(const float* __restrict__ a, 
 }
 // the launch-time refusals of a registered schedule (api.cu)
 int check_anneal(const MppibContext* c, const char* who);
+// Constrained MPPI (include/mppib.h "Constrained MPPI"): the feasibility-first merge of two or more states (n_feasible, b, eta, W).  The
+// merged state has n_all = the sum of the counts and b_all = feas_min over the states; a state's eta and W enter it times feas_scale.
+// A state with a feasible sample beats one without, which then weighs 0; states of one kind merge by today's online-softmax rescale
+// with their temperature (lambda for the feasible kind, lambda_c for the violation kind).  One accumulator suffices: once any state
+// holds a feasible sample the violation kind can never win again, so its sums are dropped.  Empty states (b = +inf) weigh 0.
+__device__ __forceinline__ float feas_min(int nf, float b, int n_all, float b_acc) { return (nf > 0) == (n_all > 0) ? fminf(b_acc, b) : b_acc; }
+__device__ __forceinline__ float feas_scale(int nf, float b, int n_all, float b_all, float inv_lambda, float inv_lambda_c) {
+    if ((nf > 0) != (n_all > 0) || b == INFINITY) return 0.f;
+    return expf(-(b - b_all) * (n_all > 0 ? inv_lambda : inv_lambda_c));
+}
+// the per-step violation a margin g contributes: g where g > 0, 0 where g <= 0; NaN stays NaN, so the sample becomes invalid
+__device__ __forceinline__ float feas_violation(float g) { return g <= 0.f ? 0.f : g; }
+// the launch-time refusals of constrained MPPI (api.cu): the mode and the registration must agree, for the registered (T, K)
+int check_constraint(const MppibContext* c, const char* who);
 #define MPPIB_HZ_MAX_N 256                    // cov_horizon: largest n = T*nu (the packed n x n triangle K4 factors in shared memory)
 #define HZ_TILE 64                             // SYRK output tile
 #define HZ_MAX_TILES 10                        // lower-triangle tiles of a 256 x 256 C

@@ -210,11 +210,13 @@ __device__ __noinline__ void horizon_update(const MppibParams& p, int nu, const 
 // Sigma^-1 as they were.  The diagonal equals the diagonal rule above without its clamp at 0.
 // HZN (update_cov with cov_horizon): the rows carry C_g[n(n+1)/2] over the whole sequence; m1 and d are kept as n-vectors and
 // horizon_update does the rest.
+// FEAS (constraint_mode): the rows carry (n_feasible bits, min V) after W_g; they merge by feas_min / feas_scale instead of the minimum
+// and today's scales, then the update is today's; thread 0 writes cstate = (sum n_feasible, min V) (nullable).
 template <Rule R>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
-                                              float* __restrict__ dist, float* __restrict__ hz_sig = nullptr) {
-    constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON;
+                                              float* __restrict__ dist, float* __restrict__ hz_sig = nullptr, float* __restrict__ cstate = nullptr) {
+    constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON, FEAS = R == RULE_FEASIBLE;
     const int T = p.T, NR = (R == RULE_PLAIN ? ctrl_rows(p) : T) * nu;   // knots parameterise PLAIN only
     float* sg = un + NR;
     const float lam = ADAPT ? dist[0] : p.lambda_;
@@ -229,10 +231,23 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
     float* Lm = sn + nu * nu;
     float* Mi = Lm + nu * nu;
     float b = INFINITY;
-    for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
-    for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
-        const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
-        sg[gidx] = eg > 0.f ? expf(-(__ldcg(&partials[(size_t)gidx * P]) - b) * inv_lambda) : 0.f;
+    if constexpr (FEAS) {
+        auto nf_of = [&](int gidx) { return __float_as_int(__ldcg(&partials[(size_t)gidx * P + 2 + NR])); };
+        int n_all = 0;
+        float vmin = INFINITY;
+        for (int gidx = 0; gidx < G; ++gidx) { n_all += nf_of(gidx); vmin = fminf(vmin, __ldcg(&partials[(size_t)gidx * P + 3 + NR])); }
+        for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = feas_min(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b);
+        for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
+            const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
+            sg[gidx] = eg > 0.f ? feas_scale(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b, inv_lambda, 1.0f / p.constraint_lambda) : 0.f;
+        }
+        if (threadIdx.x == 0 && cstate) { cstate[0] = __int_as_float(n_all); cstate[1] = vmin; }
+    } else {
+        for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
+        for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
+            const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
+            sg[gidx] = eg > 0.f ? expf(-(__ldcg(&partials[(size_t)gidx * P]) - b) * inv_lambda) : 0.f;
+        }
     }
     __syncthreads();
     float e = 0.f;
@@ -636,13 +651,15 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
 
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
-// at least, `misc` = 8 floats.
+// at least, `misc` = 8 floats.  FEASIBLE: the CTA scales come from feas_min / feas_scale over (n_feasible, beta) of every CTA, and the
+// row's last two entries are the summed count and the minimum of min V.
 template <Rule R>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                                                 float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* tiles, float* misc, float inv_lambda,
                                                 float* __restrict__ dist, float* __restrict__ smooth = nullptr, float* __restrict__ anneal = nullptr,
-                                                float* __restrict__ spline = nullptr) {
+                                                float* __restrict__ spline = nullptr, float* __restrict__ cstate = nullptr) {
+    constexpr bool FEAS = R == RULE_FEASIBLE;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = (int)gridDim.x;
     float* sc = tiles;                   // [MAX_GRID] scale of every CTA partial (the ring is idle now)
@@ -650,14 +667,41 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
     {
         float b = (tid < G) ? __ldcg(scratch + (size_t)tid * ((((P + 3) >> 2) << 2))) : INFINITY;
         const float b2 = (tid + NT < G) ? __ldcg(scratch + (size_t)(tid + NT) * ((((P + 3) >> 2) << 2))) : INFINITY;   // CTAs 256..511
-        float bm = warp_min(fminf(b, b2));
-        if (lane == 0) misc[warp] = bm;
-        __syncthreads();
         float bb = INFINITY;
+        int n_all = 0;
+        float vmin = INFINITY;
+        if constexpr (FEAS) {
+            const size_t PP = ((P + 3) >> 2) << 2;
+            const int n1 = tid < G ? __float_as_int(__ldcg(scratch + (size_t)tid * PP + P - 2)) : 0;
+            const int n2 = tid + NT < G ? __float_as_int(__ldcg(scratch + (size_t)(tid + NT) * PP + P - 2)) : 0;
+            const float v1 = tid < G ? __ldcg(scratch + (size_t)tid * PP + P - 1) : INFINITY;
+            const float v2 = tid + NT < G ? __ldcg(scratch + (size_t)(tid + NT) * PP + P - 1) : INFINITY;
+            int ns = n1 + n2;
 #pragma unroll
-        for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
-        if (tid < G) sc[tid] = (b == INFINITY) ? 0.f : expf(-(b - bb) * inv_lambda);
-        if (tid + NT < G) sc[tid + NT] = (b2 == INFINITY) ? 0.f : expf(-(b2 - bb) * inv_lambda);
+            for (int o = 16; o > 0; o >>= 1) ns += __shfl_xor_sync(0xffffffffu, ns, o);
+            const float vm = warp_min(fminf(v1, v2));
+            if (lane == 0) { misc[warp] = __int_as_float(ns); tiles[warp] = vm; }
+            __syncthreads();
+#pragma unroll
+            for (int w8 = 0; w8 < 8; ++w8) { n_all += __float_as_int(misc[w8]); vmin = fminf(vmin, tiles[w8]); }
+            __syncthreads();
+            const float bm = warp_min(feas_min(n2, b2, n_all, feas_min(n1, b, n_all, INFINITY)));
+            if (lane == 0) misc[warp] = bm;
+            __syncthreads();
+#pragma unroll
+            for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
+            const float inv_lc = 1.0f / p.constraint_lambda;
+            if (tid < G) sc[tid] = feas_scale(n1, b, n_all, bb, inv_lambda, inv_lc);
+            if (tid + NT < G) sc[tid + NT] = feas_scale(n2, b2, n_all, bb, inv_lambda, inv_lc);
+        } else {
+            float bm = warp_min(fminf(b, b2));
+            if (lane == 0) misc[warp] = bm;
+            __syncthreads();
+#pragma unroll
+            for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
+            if (tid < G) sc[tid] = (b == INFINITY) ? 0.f : expf(-(b - bb) * inv_lambda);
+            if (tid + NT < G) sc[tid + NT] = (b2 == INFINITY) ? 0.f : expf(-(b2 - bb) * inv_lambda);
+        }
         __syncthreads();
         // parallel fold with deep memory-level parallelism: P4 = ceil(P/4) float4 columns x 4 CTA groups of 64 threads;
         // thread (cg, e4) sums CTAs c = cg, cg+4, ... with 8 independent 128-bit L2 loads in flight
@@ -694,7 +738,8 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
         const PeerRow row = peer_row(peers);
         for (int e = tid; e < P; e += NT) {
             const float v0 = fold[e] + fold[PP + e] + fold[2 * PP + e] + fold[3 * PP + e];
-            const float v = e == 0 ? bb : v0;
+            float v = e == 0 ? bb : v0;
+            if constexpr (FEAS) v = e == P - 2 ? __int_as_float(n_all) : e == P - 1 ? vmin : v;
             partial[e] = v;
             peer_store(peers, row, e, v);
         }
@@ -707,7 +752,7 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
             __threadfence();
             __syncthreads();
             if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, smooth);
-            else finalize_rows<R>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist);
+            else finalize_rows<R>(p, nu, partial, 1, P, fin_U, fin_action, fin_stats, fin_mirror, tiles, dist, nullptr, cstate);
             if constexpr (R == RULE_PLAIN) if (spline) spline_exec(p, nu, tiles, spline);
             if (tid == 0 && anneal) anneal[0] += 1.0f;                        // annealed MPPI: the next iteration's row (every CTA read it)
         }
@@ -743,7 +788,7 @@ struct WsLayout {
     __host__ __device__ WsLayout(int T, int Tc, int nu, int nstage, Rule row, bool update_cov, bool smooth = false, int nparts = -1, int modes = 1) {
         const int NR = Tc * nu, P4 = (shard_row_floats(row, Tc, nu, update_cov, 1, 0) + 3) & ~3;
         if (nparts < 0) nparts = nstage < WS_NCONS ? nstage : WS_NCONS;
-        const int ring = nstage * (NR + T) * WS_W, fold_floats = MAX_GRID + 4 * P4;
+        const int ring = nstage * (NR + (row == RULE_FEASIBLE ? 2 * T : T)) * WS_W, fold_floats = MAX_GRID + 4 * P4;   // FEASIBLE: + viol[T]
         g = ring > fold_floats ? ring : fold_floats;
         if (row == RULE_FULL && g < NR + 1 + full_fin_floats(T, nu)) g = NR + 1 + full_fin_floats(T, nu);
         if (modes > 1 && g < modes_fin_floats(NR, modes, 1)) g = modes_fin_floats(NR, modes, 1);   // the fused K4 of n_modes > 1
@@ -783,6 +828,10 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // row m*gx + x, and the last CTA folds every mode into block m of the row [M][2 + T*nu] (fold_modes_and_finish).
 // anneal (annealed MPPI, nullable): the registered schedule of anneal_n iterations; SIMPLE mode scales g_r by r[t] = 1 / s[t]^2 of the
 // iteration's row after the lambda product (a schedule of ones changes no bit), and the fused K4 advances the counter.
+// FEAS (constraint_mode): a third tensor map brings the T violation rows g of the tile (the tile is (NR + 2T)*32 floats); phase A sums
+// V_k = sum_t c[t][k] in t order beside S, phase B weights the tile's feasible lanes by S with lambda when the warp ballot finds one and
+// its valid lanes by V with lambda_c otherwise, and every fold merges (n_feasible, b, eta, W) by feas_min / feas_scale; the row is
+// (beta, eta, W, n_feasible bits, min V) and the fused K4 writes cstate.
 template <int RPL, Rule R, bool RISK>
 __global__ void __launch_bounds__(NT, 1)
 mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_c,
@@ -790,8 +839,9 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                        float* __restrict__ partial, const __grid_constant__ PeerArgs peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
                        float* __restrict__ fin_stats, float* __restrict__ fin_mirror, float* __restrict__ dist, float* __restrict__ hz_S,
                        const float* __restrict__ hz_g, float* __restrict__ smooth, float* __restrict__ anneal, int anneal_n,
-                       float* __restrict__ spline) {
+                       float* __restrict__ spline, const __grid_constant__ CUtensorMap tm_v, float* __restrict__ cstate) {
     constexpr bool ADAPT = rule_adapts(R), FULL = R == RULE_FULL, HZN = R == RULE_HORIZON, SMOOTH = R == RULE_SMOOTH, MODES = R == RULE_MODES;
+    constexpr bool FEAS = R == RULE_FEASIBLE;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int K = p.K, T = p.T, Tc = R == RULE_PLAIN ? ctrl_rows(p) : T, NR = Tc * nu;   // knots parameterise PLAIN only
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -803,7 +853,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
     const int P = shard_row_floats(k3_row_rule(R), Tc, nu, m2, 1, 0);
 
-    const int tile_floats = (NR + T) * WS_W;                                  // a multiple of 32 floats: stages stay 128-B aligned
+    const int tile_floats = (NR + (FEAS ? 2 * T : T)) * WS_W;                 // a multiple of 32 floats: stages stay 128-B aligned
     const int NR4 = (NR + 3) & ~3, T4 = (T + 3) & ~3, P4 = (P + 3) & ~3;
     const bool smooth_term = SMOOTH && p.smooth_weight != 0.f;
     const WsLayout L(T, Tc, nu, nstage, k3_row_rule(R), m2, smooth_term, -1, MODES ? p.n_modes : 1);
@@ -834,6 +884,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         mbar_expect_tx(&full[s], tile_bytes);
         for (int r0 = 0; r0 < NR; r0 += xbox_rows) tma_load_2d(dst + (size_t)r0 * WS_W, &tm_x, k0, r0, &full[s]);
         tma_load_2d(dst + (size_t)NR * WS_W, &tm_c, k0, 0, &full[s]);
+        if constexpr (FEAS) tma_load_2d(dst + (size_t)(NR + T) * WS_W, &tm_v, k0, 0, &full[s]);
     };
     if (tid == 0) {
         for (int s = 0; s < nstage; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
@@ -884,6 +935,8 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         const int c = warp - 1;
         float* wme = wk + warp * WS_W;
         float b_run = INFINITY, e_run = 0.f, w_run[RPL];
+        int nf_run = 0;                                                       // FEAS: feasible samples merged so far
+        float v_run = INFINITY;                                               // FEAS: min V over the valid samples seen
         float m2_run[ADAPT ? RPL : 1], c_row[ADAPT ? RPL : 1];               // second moment and its centre per row (update_cov)
         float c_run[FULL ? MAX_PAIRS : 1];                                    // FULL: this lane's lower triangle of C
 #pragma unroll
@@ -941,17 +994,40 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             // ---- B: tile minimum, weights, their sum
             const bool valid = (k0 + lane < K) && isfinite(sum) && (!MODES || (k0 + lane >= lo && k0 + lane < hi));
             float S = valid ? sum : INFINITY;
+            float inv_l = inv_lambda;
+            int nf_c = 0;
+            if constexpr (FEAS) {
+                const float* vs = cs + (size_t)T * WS_W;                      // [T][32] margins g
+                float V = 0.f;
+                for (int t = 0; t < T; ++t) V += feas_violation(vs[t * WS_W + lane]);
+                const bool ok = valid && isfinite(V);
+                const unsigned fb = __ballot_sync(0xffffffffu, ok && V <= p.constraint_tol);
+                nf_c = __popc(fb);
+                S = fb ? (((fb >> lane) & 1u) ? sum : INFINITY) : (ok ? V : INFINITY);
+                if (!fb) inv_l = 1.0f / p.constraint_lambda;
+                v_run = fminf(v_run, warp_min(ok ? V : INFINITY));
+            }
             if constexpr (RISK) S = risk_score(S, p.n_worlds, p.risk_tail, lane);
             if (HZN && k0 + lane < K) hz_S[k0 + lane] = S;
             const float b_c = warp_min(S);
-            const float w = (S == INFINITY) ? 0.f : expf(-(S - b_c) * inv_lambda);
+            const float w = (S == INFINITY) ? 0.f : expf(-(S - b_c) * inv_l);
             const float e_c = warp_sum(w);
-            if (b_c != INFINITY) {                                            // warp-uniform
+            // FEAS: a tile without a feasible sample adds nothing once the warp holds one (warp-uniform, like b_c)
+            if (b_c != INFINITY && (!FEAS || nf_c > 0 || nf_run == 0)) {
                 wme[lane] = w;
                 __syncwarp();
-                const float b_out = fminf(b_run, b_c);
-                const float s_old = (b_run == INFINITY) ? 0.f : expf(-(b_run - b_out) * inv_lambda);
-                const float s_new = expf(-(b_c - b_out) * inv_lambda);
+                float b_out, s_old, s_new;
+                if constexpr (FEAS) {
+                    const int n_out = nf_run + nf_c;
+                    b_out = feas_min(nf_c, b_c, n_out, feas_min(nf_run, b_run, n_out, INFINITY));
+                    s_old = feas_scale(nf_run, b_run, n_out, b_out, inv_lambda, 1.0f / p.constraint_lambda);
+                    s_new = feas_scale(nf_c, b_c, n_out, b_out, inv_lambda, 1.0f / p.constraint_lambda);
+                    nf_run = n_out;
+                } else {
+                    b_out = fminf(b_run, b_c);
+                    s_old = (b_run == INFINITY) ? 0.f : expf(-(b_run - b_out) * inv_lambda);
+                    s_new = expf(-(b_c - b_out) * inv_lambda);
+                }
                 // ---- C: weighted row sums, lane = row
                 const float4* w4 = reinterpret_cast<const float4*>(wme);
 #pragma unroll
@@ -1010,6 +1086,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         // this warp's partial -> shared memory
         float* mine = cpart + (size_t)c * P4;
         if (lane == 0) { mine[0] = b_run; mine[1] = e_run; }
+        if (FEAS && lane == 0) { mine[2 + NR] = __int_as_float(nf_run); mine[3 + NR] = v_run; }
 #pragma unroll
         for (int rr = 0; rr < RPL; ++rr) { const int r = lane + 32 * rr; if (r < NR) mine[2 + r] = w_run[rr]; }
         if (ADAPT && m2) {
@@ -1031,18 +1108,32 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     {
         float* mine = scratch + (size_t)(blockIdx.x + (MODES ? blockIdx.y * gridDim.x : 0u)) * P4;
         float bb = INFINITY;
-#pragma unroll
-        for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = fminf(bb, cpart[(size_t)c * P4]);
         float sc[WS_NCONS];
+        int n_all = 0;
+        float vmin = INFINITY;
+        if constexpr (FEAS) {
+            auto nf_of = [&](int c) { return c < ncons ? __float_as_int(cpart[(size_t)c * P4 + 2 + NR]) : 0; };
 #pragma unroll
-        for (int c = 0; c < WS_NCONS; ++c) {
-            const float bc = c < ncons ? cpart[(size_t)c * P4] : INFINITY;
-            sc[c] = (bc == INFINITY) ? 0.f : expf(-(bc - bb) * inv_lambda);
+            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) { n_all += nf_of(c); vmin = fminf(vmin, cpart[(size_t)c * P4 + 3 + NR]); }
+#pragma unroll
+            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = feas_min(nf_of(c), cpart[(size_t)c * P4], n_all, bb);
+#pragma unroll
+            for (int c = 0; c < WS_NCONS; ++c)
+                sc[c] = feas_scale(nf_of(c), c < ncons ? cpart[(size_t)c * P4] : INFINITY, n_all, bb, inv_lambda, 1.0f / p.constraint_lambda);
+        } else {
+#pragma unroll
+            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = fminf(bb, cpart[(size_t)c * P4]);
+#pragma unroll
+            for (int c = 0; c < WS_NCONS; ++c) {
+                const float bc = c < ncons ? cpart[(size_t)c * P4] : INFINITY;
+                sc[c] = (bc == INFINITY) ? 0.f : expf(-(bc - bb) * inv_lambda);
+            }
         }
         for (int e = tid; e < P; e += NT) {
             float v = 0.f;
 #pragma unroll
             for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) v += sc[c] * cpart[(size_t)c * P4 + e];
+            if constexpr (FEAS) v = e == 2 + NR ? __int_as_float(n_all) : e == 3 + NR ? vmin : v;
             mine[e] = e == 0 ? bb : v;
         }
     }
@@ -1056,7 +1147,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     // the horizon K3 folds as DIST's does; it gets no fin_U and no peers, the SYRK finishes its row
     if constexpr (MODES) fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
     else fold_and_finish<HZN ? RULE_DIST : R>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda,
-                                              dist, smooth, anneal, spline);
+                                              dist, smooth, anneal, spline, cstate);
 }
 
 // K4: combine G shard partials, U update, optional Savitzky-Golay (window 9, order 2, 'interp' edges), action out; DIST / FULL /
@@ -1068,7 +1159,7 @@ __global__ void __launch_bounds__(256)
 mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float* __restrict__ partials_in, int G,
                 float* __restrict__ U, float* __restrict__ action_out, float* __restrict__ stats, const __grid_constant__ PeerArgs peers,
                 float* __restrict__ action_mirror, float* __restrict__ dist, float* __restrict__ hz_sig, float* __restrict__ smooth,
-                float* __restrict__ anneal, float* __restrict__ spline) {
+                float* __restrict__ anneal, float* __restrict__ spline, float* __restrict__ cstate) {
     extern __shared__ float un[];   // [T*nu] then [G] scales (then [T*nu] variances with update_cov, or full_fin_floats with FULL)
     const float* partials = partials_in;
     int P = shard_row_floats(R, p, nu);                                       // row stride of the partials
@@ -1081,7 +1172,7 @@ mppib_finalize_kernel(const __grid_constant__ MppibParams p, int nu, const float
     }
     if constexpr (R == RULE_MODES) modes_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist);
     else if constexpr (R == RULE_SMOOTH) smooth_rows(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, smooth);
-    else finalize_rows<R>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig);
+    else finalize_rows<R>(p, nu, partials, G, P, U, action_out, stats, action_mirror, un, dist, hz_sig, cstate);
     if constexpr (R == RULE_PLAIN) if (spline) spline_exec(p, nu, un, spline);
     if (threadIdx.x == 0 && partials_in == nullptr) peer_consume(peers, seq);
     if (threadIdx.x == 0 && anneal) anneal[0] += 1.0f;
@@ -1311,12 +1402,18 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     int xbox_rows = NR < 256 ? NR : 256;
     while (NR % xbox_rows != 0) --xbox_rows;
     // tensor maps are rebuilt only when a buffer, the shape or the device changes (the eager / stepwise path calls this per plan)
-    struct MapCache { const void* x; const void* c; int K, T, NR, dev; CUtensorMap tm_x, tm_c; };
-    static thread_local MapCache mc = {nullptr, nullptr, 0, 0, 0, -1, {}, {}};
+    // FEASIBLE: the violation rows get a map of their own (tm_v), built like the cost's; the other rules pass the cost map in its place
+    struct MapCache { const void* x; const void* c; const void* v; int K, T, NR, dev; CUtensorMap tm_x, tm_c, tm_v; };
+    static thread_local MapCache mc = {nullptr, nullptr, nullptr, 0, 0, 0, -1, {}, {}, {}};
     if (mc.x != x || mc.c != cost || mc.K != K || mc.T != T || mc.NR != NR || mc.dev != c->device) {
         if (int rc = make_map(&mc.tm_x, x, NR, K, xbox_rows, WS_W)) return rc;
         if (int rc = make_map(&mc.tm_c, cost, T, K, T, WS_W)) return rc;
         mc.x = x; mc.c = cost; mc.K = K; mc.T = T; mc.NR = NR; mc.dev = c->device;
+        mc.v = nullptr;
+    }
+    if (R == RULE_FEASIBLE && mc.v != c->viol) {
+        if (int rc = make_map(&mc.tm_v, c->viol, T, K, T, WS_W)) return rc;
+        mc.v = c->viol;
     }
     const int ntiles = (K + WS_W - 1) / WS_W;
     int grid = ntiles < c->num_sms ? ntiles : c->num_sms;
@@ -1339,7 +1436,8 @@ int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const
     mppib_reduce_ws_kernel<RPL, R, RISK><<<dim3(grid, modes), NT, smem, s>>>(c->params, mc.tm_x, mc.tm_c, nu, xbox_rows, nstage, ncons, U, c->reduce_scratch,
                                                                              c->reduce_ticket, partial, peers, fin_U, fin_action, fin_stats,
                                                                              fin_U ? c->action_mirror : nullptr, c->dist, c->hz_S, c->hz_g, smooth, anneal,
-                                                                             c->anneal_n, R == RULE_PLAIN ? live_spline(c) : nullptr);
+                                                                             c->anneal_n, R == RULE_PLAIN ? live_spline(c) : nullptr,
+                                                                             R == RULE_FEASIBLE ? mc.tm_v : mc.tm_c, R == RULE_FEASIBLE ? c->cstate : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1453,6 +1551,9 @@ int launch_reduce(MppibContext* c, const float* cost, const float* x, const floa
         if (rc) return rc;
         return launch_syrk(c, x, U, partial, fin_U, fin_action, fin_stats, s);
     }
+    case RULE_FEASIBLE:
+        MPPIB_REQUIRE(reduce_ws_stages(c->params, nu, RULE_FEASIBLE) >= 2, "mppib_reduce: T = %d, nu = %d leaves room for fewer than two ring stages with the violation rows of constraint_mode", T, nu);
+        return launch_reduce_rule<RULE_FEASIBLE, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, nullptr, s);
     case RULE_FULL:
         return risk ? launch_reduce_rule<RULE_FULL, true>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s)
                     : launch_reduce_rule<RULE_FULL, false>(c, cost, x, U, partial, fin_U, fin_action, fin_stats, nullptr, c->anneal, s);
@@ -1470,7 +1571,7 @@ template <Rule R>
 static int launch_finalize_t(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, size_t smem, float* dist,
                              float* hz_sig, float* smooth, float* anneal, cudaStream_t s) {
     mppib_finalize_kernel<R><<<1, 256, smem, s>>>(c->params, c->model.nu, partials, G, U, action_out, stats, peer_args(c), c->action_mirror, dist, hz_sig,
-                                                  smooth, anneal, R == RULE_PLAIN ? live_spline(c) : nullptr);
+                                                  smooth, anneal, R == RULE_PLAIN ? live_spline(c) : nullptr, R == RULE_FEASIBLE ? c->cstate : nullptr);
     MPPIB_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1504,6 +1605,8 @@ int launch_finalize(MppibContext* c, const float* partials, int G, float* U, flo
     case RULE_DIST:
         return launch_finalize_t<RULE_DIST>(c, partials, G, U, action_out, stats, un + (adaptive_cov(c) ? NR : 0) * sizeof(float), c->dist, nullptr,
                                             nullptr, c->anneal, s);
+    case RULE_FEASIBLE:
+        return launch_finalize_t<RULE_FEASIBLE>(c, partials, G, U, action_out, stats, un, nullptr, nullptr, nullptr, nullptr, s);
     default:   // RULE_PLAIN
         return launch_finalize_t<RULE_PLAIN>(c, partials, G, U, action_out, stats, un, nullptr, nullptr, nullptr, c->anneal, s);
     }

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 22
+ABI_VERSION = 23
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -85,6 +85,7 @@ class MppibParams(C.Structure):
         ("du_min", f32 * MAX_NU), ("du_max", f32 * MAX_NU), ("smooth_weight", f32),
         ("n_worlds", i32), ("risk_tail", i32),
         ("n_modes", i32), ("mode_margin", f32), ("mode_samples", i32),
+        ("constraint_mode", i32), ("constraint_tol", f32), ("constraint_lambda", f32), ("constraint_pad", i32),
         ("control_knots", i32), ("spline_degree", i32),
     ]
 
@@ -633,6 +634,41 @@ def _spline_params(p: MppibParams, mppi_cfg, nu: int) -> None:
     p.control_knots, p.spline_degree = P, d
 
 
+def constraint_on(mppi_cfg) -> bool:
+    """True when the config asks for constrained MPPI (`constraint_mode: feasible_first`)."""
+    return str(getattr(mppi_cfg, "constraint_mode", "none")) == "feasible_first"
+
+
+def _constraint_params(p: MppibParams, mppi_cfg) -> None:
+    """The `constraint_mode` / `constraint_tol` / `constraint_lambda` keys of constrained MPPI (DESIGN.md section 2, "Constrained MPPI")
+    and what they exclude.  With the mode "none" the three fields stay 0, so the block is today's byte for byte."""
+    mode = str(getattr(mppi_cfg, "constraint_mode", "none"))
+    if mode not in ("none", "feasible_first"):
+        raise ValueError(f"unknown constraint_mode {mode!r} (none | feasible_first)")
+    if mode == "none":
+        return
+    tol = float(getattr(mppi_cfg, "constraint_tol", 0.0))
+    if not (math.isfinite(tol) and tol >= 0.0):
+        raise ValueError(f"constraint_tol = {tol} must be finite and >= 0")
+    lam_c = getattr(mppi_cfg, "constraint_lambda", None)
+    lam_c = float(p.lambda_ if lam_c is None else lam_c)
+    if not (math.isfinite(lam_c) and lam_c > 0.0):
+        raise ValueError(f"constraint_lambda = {lam_c} must be finite and > 0")
+    if p.mode == MODE_CEM or p.mode == MODE_SMOOTH:
+        raise ValueError("constraint_mode: feasible_first excludes mppi_mode cem and smooth")
+    if p.update_cov or p.update_lambda:
+        raise ValueError("constraint_mode: feasible_first excludes update_cov and update_lambda")
+    if p.n_modes > 1:
+        raise ValueError("constraint_mode: feasible_first excludes n_modes > 1")
+    if p.n_worlds > 1:
+        raise ValueError("constraint_mode: feasible_first excludes n_worlds > 1")
+    if anneal_on(mppi_cfg):
+        raise ValueError("constraint_mode: feasible_first excludes annealed MPPI")
+    if p.control_knots > 0:
+        raise ValueError("constraint_mode: feasible_first excludes control_knots > 0")
+    p.constraint_mode, p.constraint_tol, p.constraint_lambda = 1, tol, lam_c
+
+
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
     """MPPIConfig + IsaacGymConfig -> MppibParams (float32 block for the kernels)."""
     p = MppibParams()
@@ -713,6 +749,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     _modes_params(p, mppi_cfg)
     _anneal_params(p, mppi_cfg)
     _spline_params(p, mppi_cfg, nu)
+    _constraint_params(p, mppi_cfg)
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

@@ -46,6 +46,23 @@ class PandaReachObjective:
         return self.weights["robot_to_goal"] * dist + self.weights["robot_ori"] * ori
 
 
+class PandaReachKeepOutObjective(PandaReachObjective):
+    """The panda reach cost with a spherical keep-out region for the tip: ``compute_constraint`` returns the margin
+    radius - |p_ee - centre| per row (> 0 inside the sphere), for ``constraint_mode: feasible_first``."""
+
+    def __init__(self, cfg=None, centre=(0.5, 0.0, 0.5), radius: float = 0.1, **kw):
+        super().__init__(cfg, **kw)
+        self.centre = tuple(float(c) for c in centre)
+        self.radius = float(radius)
+        self._centre_t = None
+
+    def compute_constraint(self, sim):
+        ee = sim.get_actor_link_by_name(self.actor, self.link)
+        if self._centre_t is None or self._centre_t.device != ee.device:
+            self._centre_t = torch.tensor(self.centre, dtype=torch.float32, device=ee.device)
+        return self.radius - torch.linalg.norm(ee[:, 0:3] - self._centre_t, axis=1)
+
+
 class PointReachObjective:
     """Planar distance of a robot link to the goal actor (+ optional wall contact force)."""
 

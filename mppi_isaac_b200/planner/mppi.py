@@ -27,8 +27,8 @@ import os
 import torch
 
 from ..backend import shard_row_floats
-from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule, spline_basis, spline_initial_knots,
-                          spline_table)
+from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule, constraint_on, spline_basis,
+                          spline_initial_knots, spline_table)
 
 
 class _NoRange:
@@ -148,7 +148,7 @@ def _randomised(model) -> bool:
 class MPPIPlanner:
     def __init__(self, cfg, nx: int, dynamics: Callable, running_cost: Callable, prior: Optional[Callable] = None, *,
                  sim=None, rollout_mode: str = "auto", use_cuda_graph: bool = True, k_total: Optional[int] = None,
-                 k_offset: int = 0, process_group=None, seed: Optional[int] = None):
+                 k_offset: int = 0, process_group=None, seed: Optional[int] = None, running_constraint: Optional[Callable] = None):
         if sim is None:
             raise ValueError("MPPIPlanner needs the RolloutSim that owns the kernel handle (sim=...)")
         self.cfg = cfg
@@ -234,6 +234,14 @@ class MPPIPlanner:
         if self.control_knots > 0 and bool(getattr(cfg, "use_priors", False)) and prior is not None:
             raise ValueError("control_knots > 0 does not take a prior: the prior row is an action sequence and cannot be written as knots")
         self.backend = sim.backend
+        # constrained MPPI (DESIGN.md section 2, "Constrained MPPI"): running_constraint returns a signed margin per row (<= 0 satisfied),
+        # written into a (T, K) device buffer K3 reads; make_params checks the keys against the mode
+        self.constrained = constraint_on(cfg)
+        self._running_constraint = running_constraint
+        if self.constrained and running_constraint is None:
+            raise ValueError("constraint_mode: feasible_first needs a running_constraint (the Objective's compute_constraint)")
+        if self.constrained and not hasattr(self.backend, "set_constraint"):
+            raise ValueError(f"constraint_mode: feasible_first needs a backend with set_constraint ({type(self.backend).__name__} has none)")
         if self.control_knots > 0 and not hasattr(self.backend, "set_spline"):
             raise ValueError(f"control_knots > 0 needs a backend with set_spline ({type(self.backend).__name__} has none)")
         if self.adaptive and not hasattr(self.backend, "set_distribution"):
@@ -334,6 +342,15 @@ class MPPIPlanner:
         elif hasattr(self.backend, "set_spline"):
             self.backend.set_spline(None)
         self.cost = torch.zeros((T, K), **f32)
+        # constrained MPPI: the per-step margins g[T][K] K3 reads and the state (n_feasible as int32 bits, min V) K4 writes; a planner
+        # rebuilt with the mode off registers none
+        self.viol, self.cstate = None, None
+        if self.constrained:
+            self.viol = torch.zeros((T, K), **f32)
+            self.cstate = torch.zeros((2,), **f32)
+            self.backend.set_constraint(self.viol, self.cstate)
+        elif hasattr(self.backend, "set_constraint"):
+            self.backend.set_constraint(None)
         P = shard_row_floats(self.backend.params, nu)
         self.partial = torch.zeros((P,), **f32)
         self.partials = torch.zeros((self.world, P), **f32)
@@ -567,6 +584,24 @@ class MPPIPlanner:
         return self.dist[2:2 + E]
 
     @property
+    def violation(self):
+        """(T, K) device view of the last plan's per-step constraint margins g of constrained MPPI, as the Objective returned them (the
+        kernels count max(g, 0)); None with constraint_mode none."""
+        return self.viol
+
+    @property
+    def feasible_samples(self):
+        """The number of feasible samples of the last plan over every rank (an int, read from the device; None with constraint_mode
+        none)."""
+        return None if self.cstate is None else int(self.cstate[0:1].view(torch.int32).item())
+
+    @property
+    def min_violation(self):
+        """0-d device view of the smallest summed violation V_k of a valid sample in the last plan over every rank (+inf when no sample
+        was valid; None with constraint_mode none)."""
+        return None if self.cstate is None else self.cstate[1]
+
+    @property
     def perturbed_action(self):
         """(K, T, nu) view, the layout mppi_torch exposes."""
         return self.actions.permute(2, 0, 1)
@@ -624,6 +659,8 @@ class MPPIPlanner:
             self.sim.rollout_all(self.actions)
         with _nvtx("mppi/objective cost"):
             cost = self._cost_batched()
+            if self.viol is not None:
+                self.viol.copy_(self._running_constraint(None).reshape(self.T, self.K))
         x = self._weighted()
         with _nvtx("mppi/K3 reduce + exchange + K4 update"):
             if self.world == 1 and hasattr(be, "reduce_finalize"):
@@ -655,6 +692,8 @@ class MPPIPlanner:
                     u.copy_(u_out)                                   # "update action if there were changes"
             c = self._running_cost(state)
             self.cost[t].copy_(c.reshape(-1))
+            if self.viol is not None:
+                self.viol[t].copy_(self._running_constraint(state).reshape(-1))
         if self.use_priors and prior_local:
             row = self.K_total - 2 - self.k_offset
             self.noise[:, :, row] = self.actions[:, :, row] - self.U

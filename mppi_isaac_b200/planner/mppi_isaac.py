@@ -19,6 +19,7 @@ from typing import Callable, Optional
 
 import torch
 
+from ..model.blob import constraint_on
 from ..utils.transport import FastDecoder, FastEncoder, bytes_to_torch, torch_to_bytes
 from .mppi import MPPIPlanner, shard_samples
 from .rollout_sim import RolloutSim
@@ -57,8 +58,10 @@ class MPPIisaacPlanner(object):
             observe=observe,
             k_offset=self.k_offset,
         )
+        self.constrained = constraint_on(cfg.mppi)
+        self._check_constraint(objective)
         # which rows does the Objective read?  (one dry run against dummy rows)
-        self.sim.trace(lambda s: self.objective.compute_cost(s))
+        self._trace()
 
         if prior:
             self.prior = lambda state, t: prior.compute_command(self.sim)
@@ -86,6 +89,18 @@ class MPPIisaacPlanner(object):
             # the annealing schedule is rebuilt from the config, not carried over: a keep_U rebuild starts from the configured decays
             self.mppi.refresh_mean_action()              # spline MPPI: U_exec of the carried knots
 
+    def _check_constraint(self, objective):
+        if self.constrained and not callable(getattr(objective, "compute_constraint", None)):
+            raise ValueError(f"constraint_mode: feasible_first needs an Objective with compute_constraint(sim) ({type(objective).__name__} has none)")
+
+    def _trace(self):
+        """Record which rows the Objective reads: the cost and, with constrained MPPI, the constraint, so the plan observes their union."""
+        def observed(sim):
+            self.objective.compute_cost(sim)
+            if self.constrained:
+                self.objective.compute_constraint(sim)
+        self.sim.trace(observed)
+
     def _make_mppi(self):
         return MPPIPlanner(
             self.cfg.mppi,
@@ -96,12 +111,14 @@ class MPPIisaacPlanner(object):
             sim=self.sim,
             k_total=self.k_total,
             k_offset=self.k_offset,
+            running_constraint=self.running_constraint if self.constrained else None,
             **self._opts,
         )
 
     def update_objective(self, objective):
+        self._check_constraint(objective)
         self.objective = objective
-        self.sim.trace(lambda s: self.objective.compute_cost(s))
+        self._trace()
         self._build_mppi()
 
     def dynamics(self, _, u, t=None):
@@ -113,6 +130,9 @@ class MPPIisaacPlanner(object):
     def running_cost(self, _):
         return self.objective.compute_cost(self.sim)
 
+    def running_constraint(self, _):
+        return self.objective.compute_constraint(self.sim)
+
     def compute_action(self, q, qdot, obst=None, obst_tensor=None):
         self.sim.reset_root_state()
         self.sim.reset_robot_state(q, qdot)
@@ -122,7 +142,7 @@ class MPPIisaacPlanner(object):
                 # an obstacle was added / resized: the simulator was rebuilt (stop_sim / start_sim as isaacgym_wrapper.py:743-746),
                 # i.e. a new kernel handle, new buffers and scene-default joint states.  Re-trace, re-bind the planner to the new
                 # handle (action mirror, captured graph) and re-apply the robot state the caller has just handed over.
-                self.sim.trace(lambda s: self.objective.compute_cost(s))
+                self._trace()
                 self._build_mppi(keep_U=True)
                 self.sim.reset_robot_state(q, qdot)
         if obst_tensor is not None and len(obst_tensor) > 0:
@@ -163,7 +183,7 @@ class MPPIisaacPlanner(object):
 
     def add_to_env(self, env_cfg_additions):
         self.sim.add_to_envs(env_cfg_additions)
-        self.sim.trace(lambda s: self.objective.compute_cost(s))
+        self._trace()
         self._build_mppi(keep_U=True)
 
     def get_rollouts(self):

@@ -54,6 +54,9 @@ class MPPIConfig:
     anneal_horizon_decay: float = 1.0    # annealed MPPI: c_h in (0, 1], the noise std factor per step towards the start of the horizon
     control_knots: int = 0               # spline MPPI (DESIGN.md section 2): P control knots per horizon, interpolated to every step; 0 = off
     spline_degree: int = 1               # spline MPPI: B-spline degree d in 1 .. 3, P in d + 1 .. horizon
+    constraint_mode: str = "none"        # constrained MPPI (DESIGN.md section 2): "none" or "feasible_first" (needs Objective.compute_constraint)
+    constraint_tol: float = 0.0          # constrained MPPI: a sample is feasible when its summed violation is <= tol (finite, >= 0)
+    constraint_lambda: Optional[float] = None   # constrained MPPI: temperature of the fallback over violations when no sample is feasible; None: lambda_
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0
