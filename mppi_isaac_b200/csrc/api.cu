@@ -14,6 +14,39 @@ void mppib_set_error(const char* fmt, ...) {
 }
 
 
+// Which planning modes cannot run together (make_params refuses the same pairs): validate checks the block with anneal = false; a schedule
+// is checked with anneal = true at registration and at every launch, so that a later mppib_set_params cannot slip past it.
+enum Feature { F_CEM, F_SMOOTH, F_UPDATE_COV, F_UPDATE_LAMBDA, F_COV_HORIZON, F_FILTER_U, F_WORLDS, F_MODES, F_KNOTS, F_CONSTRAINT, F_ANNEAL };
+static const char* const kFeatureNames[] = {"mode cem", "mode smooth", "update_cov", "update_lambda", "cov_horizon", "filter_u", "n_worlds > 1",
+                                            "n_modes > 1", "control_knots > 0", "constraint_mode", "annealed MPPI"};
+#define FBIT(f) (1u << (f))
+static const unsigned F_CEM_SMOOTH = FBIT(F_CEM) | FBIT(F_SMOOTH), F_ADAPTIVE = FBIT(F_UPDATE_COV) | FBIT(F_UPDATE_LAMBDA);
+struct Exclusion { Feature feature; unsigned excludes; const char* why; };     // excludes: FBIT mask; why: "" or the reason
+static const Exclusion kExclusions[] = {
+    {F_SMOOTH, F_ADAPTIVE, ""},
+    {F_SMOOTH, FBIT(F_FILTER_U), " (the derivative is integrated, not smoothed)"},
+    {F_CEM, F_ADAPTIVE, ""},
+    {F_WORLDS, F_CEM_SMOOTH | FBIT(F_COV_HORIZON), ""},
+    {F_MODES, F_CEM_SMOOTH | FBIT(F_WORLDS), ""},
+    {F_MODES, F_ADAPTIVE, " (the adapted distribution belongs to one mean)"},
+    {F_KNOTS, F_CEM_SMOOTH | F_ADAPTIVE | FBIT(F_MODES) | FBIT(F_WORLDS), ""},
+    {F_KNOTS, FBIT(F_FILTER_U), ": the spline is smooth already, switch filter_u off"},
+    {F_CONSTRAINT, F_CEM_SMOOTH | F_ADAPTIVE | FBIT(F_MODES) | FBIT(F_WORLDS) | FBIT(F_KNOTS), ""},
+    {F_ANNEAL, FBIT(F_CEM), " (it has its own sigma)"},
+    {F_ANNEAL, FBIT(F_SMOOTH) | F_ADAPTIVE | FBIT(F_KNOTS) | FBIT(F_CONSTRAINT), ""},
+    {F_ANNEAL, FBIT(F_MODES), " (the Stein coupling's Sigma^-1 metric would need the schedule)"},
+};
+
+int check_exclusions(const MppibParams& p, bool anneal, const char* who) {
+    const bool on[] = {p.mode == MPPIB_MODE_CEM, p.mode == MPPIB_MODE_SMOOTH, p.update_cov != 0, p.update_lambda != 0, p.cov_horizon != 0,
+                       p.filter_u != 0, p.n_worlds > 1, p.n_modes > 1, p.control_knots > 0, p.constraint_mode != 0, anneal};
+    for (const Exclusion& e : kExclusions)
+        for (int f = 0; f <= F_ANNEAL; ++f)
+            MPPIB_REQUIRE(!(on[e.feature] && on[f] && (e.excludes & FBIT(f))), "%s%s%s excludes %s%s", who, *who ? ": " : "", kFeatureNames[e.feature],
+                          kFeatureNames[f], e.why);
+    return 0;
+}
+
 static int validate(const MppibModel* m, const MppibParams* p) {
     MPPIB_REQUIRE(m != nullptr && p != nullptr, "null model/params");
     MPPIB_REQUIRE(m->abi_version == MPPIB_ABI_VERSION, "model abi_version %d != library %d", m->abi_version, MPPIB_ABI_VERSION);
@@ -52,15 +85,12 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->dt > 0.f, "mode smooth: the integration step dt = %g must be positive", p->dt);
         for (int j = 0; j < m->nu; ++j)
             MPPIB_REQUIRE(p->du_min[j] <= p->du_max[j], "mode smooth: du_min[%d] = %g > du_max[%d] = %g", j, p->du_min[j], j, p->du_max[j]);
-        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "mode smooth excludes update_cov and update_lambda");
-        MPPIB_REQUIRE(!p->filter_u, "mode smooth excludes filter_u (the derivative is integrated, not smoothed)");
         MPPIB_REQUIRE(p->T <= 256 && p->T * m->nu <= 512, "mode smooth needs T <= 256 and T*nu <= 512, got T = %d, T*nu = %d", p->T, p->T * m->nu);
     }
     if (p->mode == MPPIB_MODE_CEM) {
         MPPIB_REQUIRE(p->n_elites >= 1 && p->n_elites <= MPPIB_CEM_MAX_ELITES, "mode cem: n_elites = %d out of range [1, %d]", p->n_elites, MPPIB_CEM_MAX_ELITES);
         MPPIB_REQUIRE(p->n_keep >= 0 && p->n_keep <= p->n_elites, "mode cem: n_keep = %d out of range [0, n_elites = %d]", p->n_keep, p->n_elites);
         MPPIB_REQUIRE(p->elite_alpha >= 0.f && p->elite_alpha <= 1.f, "mode cem: elite_alpha = %g outside [0, 1]", p->elite_alpha);
-        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "mode cem excludes update_cov and update_lambda");
         MPPIB_REQUIRE(p->T <= 256 && p->T * m->nu <= 512, "mode cem needs T <= 256 and T*nu <= 512, got T = %d, T*nu = %d", p->T, p->T * m->nu);
         for (int j = 0; j < m->nu; ++j)
             for (int i = 0; i < m->nu; ++i) MPPIB_REQUIRE(i == j || p->sigma_chol[j * m->nu + i] == 0.f, "mode cem needs a diagonal noise_sigma");
@@ -71,8 +101,6 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(p->risk_tail >= 1 && p->risk_tail <= R, "risk_tail = %d out of range [1, n_worlds = %d]", p->risk_tail, R);
         MPPIB_REQUIRE(p->K % R == 0 && p->k_offset % (uint32_t)R == 0, "n_worlds = %d: the shard K = %d, k_offset = %u must be multiples of it", R,
                       p->K, p->k_offset);
-        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "n_worlds > 1 excludes mode cem and mode smooth");
-        MPPIB_REQUIRE(!p->cov_horizon, "n_worlds > 1 excludes cov_horizon");
     }
     MPPIB_REQUIRE(p->n_modes >= 0 && p->n_modes <= MPPIB_MAX_MODES, "n_modes = %d out of range [1, %d]", p->n_modes, MPPIB_MAX_MODES);
     MPPIB_REQUIRE(isfinite(p->mode_margin) && p->mode_margin >= 0.f, "mode_margin = %g must be finite and >= 0", p->mode_margin);
@@ -82,9 +110,6 @@ static int validate(const MppibModel* m, const MppibParams* p) {
                       p->mode_samples);
         MPPIB_REQUIRE((uint64_t)p->k_offset + (uint64_t)p->K <= (uint64_t)M * (uint64_t)p->mode_samples,
                       "n_modes = %d: the shard [%u, +%d) exceeds n_modes * mode_samples = %d", M, p->k_offset, p->K, M * p->mode_samples);
-        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "n_modes > 1 excludes mode cem and mode smooth");
-        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "n_modes > 1 excludes update_cov and update_lambda (the adapted distribution belongs to one mean)");
-        MPPIB_REQUIRE(p->n_worlds <= 1, "n_modes > 1 excludes n_worlds > 1");
         MPPIB_REQUIRE(p->T * m->nu <= 512, "n_modes > 1 needs T*nu <= 512, got %d", p->T * m->nu);
     }
     MPPIB_REQUIRE(p->control_knots >= 0, "control_knots = %d must be >= 0", p->control_knots);
@@ -93,20 +118,13 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(d >= 1 && d <= MPPIB_MAX_SPLINE_DEGREE, "spline_degree = %d out of range [1, %d]", d, MPPIB_MAX_SPLINE_DEGREE);
         MPPIB_REQUIRE(P >= d + 1 && P <= p->T, "control_knots = %d out of range [spline_degree + 1 = %d, T = %d]", P, d + 1, p->T);
         MPPIB_REQUIRE(P * m->nu <= 512 && p->T <= 256, "control_knots needs P*nu <= 512 and T <= 256, got P*nu = %d, T = %d", P * m->nu, p->T);
-        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "control_knots > 0 excludes mode cem and mode smooth");
-        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "control_knots > 0 excludes update_cov and update_lambda");
-        MPPIB_REQUIRE(p->n_modes <= 1 && p->n_worlds <= 1, "control_knots > 0 excludes n_modes > 1 and n_worlds > 1");
-        MPPIB_REQUIRE(!p->filter_u, "control_knots > 0 excludes filter_u: the spline is smooth already, switch filter_u off");
     }
     MPPIB_REQUIRE(p->constraint_mode == 0 || p->constraint_mode == 1, "constraint_mode = %d must be 0 or 1", p->constraint_mode);
     if (p->constraint_mode) {
         MPPIB_REQUIRE(isfinite(p->constraint_tol) && p->constraint_tol >= 0.f, "constraint_tol = %g must be finite and >= 0", p->constraint_tol);
         MPPIB_REQUIRE(isfinite(p->constraint_lambda) && p->constraint_lambda > 0.f, "constraint_lambda = %g must be finite and > 0", p->constraint_lambda);
-        MPPIB_REQUIRE(p->mode == MPPIB_MODE_SIMPLE || p->mode == MPPIB_MODE_MEAN, "constraint_mode excludes mode cem and mode smooth");
-        MPPIB_REQUIRE(!p->update_cov && !p->update_lambda, "constraint_mode excludes update_cov and update_lambda");
-        MPPIB_REQUIRE(p->n_modes <= 1 && p->n_worlds <= 1, "constraint_mode excludes n_modes > 1 and n_worlds > 1");
-        MPPIB_REQUIRE(p->control_knots == 0, "constraint_mode excludes control_knots > 0");
     }
+    if (int rc = check_exclusions(*p, false, "")) return rc;
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
         MPPIB_REQUIRE(kd >= 0 && kd <= MPPIB_OBS_CONTACT, "obs[%d].kind invalid", i);
@@ -136,21 +154,11 @@ static int alloc_scratch(MppibContext* c) {
     return 0;
 }
 
-// Annealed MPPI: what a parameter block must leave out while a schedule is registered (checked at registration and at every launch,
-// so that a later mppib_set_params cannot slip past it)
-static int anneal_excludes(const MppibParams& p, const char* who) {
-    MPPIB_REQUIRE(p.mode == MPPIB_MODE_SIMPLE || p.mode == MPPIB_MODE_MEAN, "%s: annealed MPPI excludes mode cem (it has its own sigma) and mode smooth", who);
-    MPPIB_REQUIRE(!p.update_cov && !p.update_lambda, "%s: annealed MPPI excludes update_cov and update_lambda", who);
-    MPPIB_REQUIRE(p.n_modes <= 1, "%s: annealed MPPI excludes n_modes > 1 (the Stein coupling's Sigma^-1 metric would need the schedule)", who);
-    MPPIB_REQUIRE(p.control_knots == 0, "%s: annealed MPPI excludes control_knots > 0", who);
-    return 0;
-}
-
 int check_anneal(const MppibContext* c, const char* who) {
     if (!c->anneal) return 0;
     MPPIB_REQUIRE(c->params.T == c->anneal_T, "%s: the annealing schedule was registered for T = %d, the parameter block has T = %d; register a schedule "
                   "for the new horizon (mppib_set_anneal)", who, c->anneal_T, c->params.T);
-    return anneal_excludes(c->params, who);
+    return check_exclusions(c->params, true, who);
 }
 
 int check_spline(const MppibContext* c, const char* who) {
@@ -174,7 +182,7 @@ int check_constraint(const MppibContext* c, const char* who) {
     MPPIB_REQUIRE(c->viol != nullptr, "%s: constraint_mode needs its violation buffer registered (mppib_set_constraint)", who);
     MPPIB_REQUIRE(c->viol_T == p.T && c->viol_K == p.K, "%s: the violation buffer was registered for (T, K) = (%d, %d), the handle has (%d, %d); register a "
                   "buffer for the new block (mppib_set_constraint)", who, c->viol_T, c->viol_K, p.T, p.K);
-    MPPIB_REQUIRE(c->dist == nullptr && c->anneal == nullptr, "%s: constraint_mode runs plain MPPI; register no distribution and no annealing schedule", who);
+    MPPIB_REQUIRE(c->dist == nullptr, "%s: constraint_mode runs plain MPPI; register no distribution", who);
     return 0;
 }
 
@@ -441,7 +449,7 @@ int32_t mppib_set_anneal(MppibHandle h, float* state, int32_t n_iterations) {
     }
     MPPIB_REQUIRE(n_iterations >= 1 && n_iterations <= MPPIB_MAX_ANNEAL, "mppib_set_anneal: n_iterations = %d out of range [1, %d]", n_iterations,
                   MPPIB_MAX_ANNEAL);
-    if (int rc = anneal_excludes(h->params, "mppib_set_anneal")) return rc;
+    if (int rc = check_exclusions(h->params, true, "mppib_set_anneal")) return rc;
     h->anneal = state; h->anneal_n = n_iterations; h->anneal_T = h->params.T;
     return 0;
 }

@@ -189,6 +189,9 @@ __device__ __forceinline__ const float* anneal_row(const float* __restrict__ a, 
 }
 // the launch-time refusals of a registered schedule (api.cu)
 int check_anneal(const MppibContext* c, const char* who);
+// the first pair of the exclusion table (api.cu) a block breaks, with a registered schedule counted when anneal is set; who: "" or the
+// entry point the message names
+int check_exclusions(const MppibParams& p, bool anneal, const char* who);
 // Constrained MPPI (include/mppib.h "Constrained MPPI"): the feasibility-first merge of two or more states (n_feasible, b, eta, W).  The
 // merged state has n_all = the sum of the counts and b_all = feas_min over the states; a state's eta and W enter it times feas_scale.
 // A state with a feasible sample beats one without, which then weighs 0; states of one kind merge by today's online-softmax rescale

@@ -568,7 +568,7 @@ int k1_admit(const MppibContext* c, K1Entry e, bool args, uint32_t k_offset, uin
     if (e == K1_SMOOTH) {
         MPPIB_REQUIRE(d == DRAW_SMOOTH, "%s: needs mode smooth (MPPIB_MODE_SMOOTH), the handle has mode %d", who, c->params.mode);
         MPPIB_REQUIRE(c->smooth != nullptr, "%s: no smooth state registered (mppib_set_smooth_state)", who);
-        MPPIB_REQUIRE(c->anneal == nullptr, "%s: annealed MPPI excludes mode smooth", who);
+        if (int rc = check_exclusions(c->params, c->anneal != nullptr, who)) return rc;
         MPPIB_REQUIRE(T * nu <= SM_MAX_N, "%s: needs T*nu <= %d, got %d", who, SM_MAX_N, T * nu);
         return 0;
     }

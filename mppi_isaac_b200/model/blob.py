@@ -12,7 +12,7 @@ import ctypes as C
 import math
 import os
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -384,7 +384,7 @@ def build_scene(actor_cfgs: list, gravity=(0.0, 0.0, -9.8), assets_dirs=None, su
 
 def _cem_params(p: MppibParams, mppi_cfg, nu: int) -> None:
     """The `mppi_mode: cem` keys (DESIGN.md section 2, "Cross-entropy planning"): E elites, momentum alpha, E_keep = floor(xi E)
-    carried elites, I iterations per plan; the refusals of the mode."""
+    carried elites, I iterations per plan."""
     E = int(getattr(mppi_cfg, "n_elites", 10))
     alpha = float(getattr(mppi_cfg, "elite_momentum", 0.1))
     xi = float(getattr(mppi_cfg, "keep_elites", 0.3))
@@ -401,21 +401,15 @@ def _cem_params(p: MppibParams, mppi_cfg, nu: int) -> None:
     keep = int(math.floor(xi * E))
     if E + keep + 2 > k_total:
         raise ValueError(f"mppi_mode: cem needs n_elites + floor(keep_elites * n_elites) + 2 <= num_samples; {E} + {keep} + 2 > {k_total}")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("mppi_mode: cem has its own update rule and excludes update_cov and update_lambda")
-    if str(getattr(mppi_cfg, "sampling_method", "halton")) not in ("random", "colored"):
-        raise ValueError("mppi_mode: cem samples with sampling_method random or colored, not halton")
     sigma = np.asarray(mppi_cfg.noise_sigma, np.float64).reshape(nu, nu)
     if np.any(sigma != np.diag(np.diag(sigma))):
         raise ValueError("mppi_mode: cem adapts a diagonal per-step sigma: noise_sigma must be diagonal")
-    if p.T > 256 or p.T * nu > 512:
-        raise ValueError(f"mppi_mode: cem needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
     p.n_elites, p.n_keep, p.elite_alpha = E, keep, alpha
 
 
 def _smooth_params(p: MppibParams, mppi_cfg, nu: int, bc) -> None:
     """The `mppi_mode: smooth` keys (DESIGN.md section 2, "Smooth MPPI"): the smoothness weight omega and the derivative bounds
-    du_min / du_max (length 1 broadcasts, None is unbounded); the refusals of the mode."""
+    du_min / du_max (length 1 broadcasts, None is unbounded)."""
     w = float(getattr(mppi_cfg, "smooth_weight", 0.0))
     if not (math.isfinite(w) and w >= 0.0):
         raise ValueError(f"smooth_weight = {w} must be finite and >= 0")
@@ -427,15 +421,6 @@ def _smooth_params(p: MppibParams, mppi_cfg, nu: int, bc) -> None:
             raise ValueError(f"du_min[{j}] = {dlo[j]} must not exceed du_max[{j}] = {dhi[j]}")
     if not p.dt > 0.0:
         raise ValueError(f"mppi_mode: smooth integrates the derivative over isaacgym.dt, which must be positive; dt = {p.dt}")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("mppi_mode: smooth excludes update_cov and update_lambda")
-    if p.filter_u:
-        raise ValueError("mppi_mode: smooth excludes filter_u: the actions are already smooth, switch filter_u off")
-    method = str(getattr(mppi_cfg, "sampling_method", "halton"))
-    if method != "random":
-        raise ValueError(f"mppi_mode: smooth samples its derivative with sampling_method random, not {method}")
-    if p.T > 256 or p.T * nu > 512:
-        raise ValueError(f"mppi_mode: smooth needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
     p.smooth_weight = w
     for j in range(nu):
         p.du_min[j], p.du_max[j] = dlo[j], dhi[j]
@@ -448,7 +433,7 @@ def risk_tail(n_worlds: int, alpha: float) -> int:
 
 def _risk_params(p: MppibParams, mppi_cfg, K_local: int) -> None:
     """The risk-aware MPPI keys (DESIGN.md section 2, "Risk-aware MPPI"): R = n_worlds rollouts per control sample, scored by the mean
-    of their m = ceil(cvar_alpha R) largest costs; the refusals of the mode.  n_worlds = 1 leaves the block as it was."""
+    of their m = ceil(cvar_alpha R) largest costs.  n_worlds = 1 leaves the block as it was."""
     R = int(getattr(mppi_cfg, "n_worlds", 1))
     if R == 1:
         return
@@ -462,16 +447,12 @@ def _risk_params(p: MppibParams, mppi_cfg, K_local: int) -> None:
         raise ValueError(f"n_worlds = {R} needs num_samples = {k_total} to be a multiple of it with at least two control samples")
     if K_local % R != 0:
         raise ValueError(f"n_worlds = {R}: the shard of {K_local} samples must hold whole groups of worlds")
-    if p.mode in (MODE_CEM, MODE_SMOOTH):
-        raise ValueError("n_worlds > 1 excludes mppi_mode cem and smooth")
-    if p.cov_horizon:
-        raise ValueError("n_worlds > 1 excludes cov_type: horizon")
     p.n_worlds, p.risk_tail = R, risk_tail(R, alpha)
 
 
 def _modes_params(p: MppibParams, mppi_cfg) -> None:
     """The multi-modal MPPI keys (DESIGN.md section 2, "Multi-modal MPPI"): M = n_modes nominal sequences, each drawn around by its
-    block of Kc = K_total / M samples, and the switching margin; the refusals of the mode.  n_modes = 1 leaves the block as it was."""
+    block of Kc = K_total / M samples, and the switching margin.  n_modes = 1 leaves the block as it was."""
     M = int(getattr(mppi_cfg, "n_modes", 1))
     margin = float(getattr(mppi_cfg, "mode_switch_margin", 0.0))
     if not 1 <= M <= MAX_MODES:
@@ -483,12 +464,6 @@ def _modes_params(p: MppibParams, mppi_cfg) -> None:
     k_total = int(mppi_cfg.num_samples)
     if k_total % M != 0 or k_total // M < 32:
         raise ValueError(f"n_modes = {M} needs num_samples = {k_total} to be a multiple of it with at least 32 samples per mode")
-    if p.mode in (MODE_CEM, MODE_SMOOTH):
-        raise ValueError("n_modes > 1 excludes mppi_mode cem and smooth")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("n_modes > 1 excludes update_cov and update_lambda: the adapted distribution belongs to one mean")
-    if p.n_worlds > 1:
-        raise ValueError("n_modes > 1 excludes n_worlds > 1")
     p.n_modes, p.mode_margin, p.mode_samples = M, margin, k_total // M
 
 
@@ -514,7 +489,7 @@ def anneal_on(mppi_cfg) -> bool:
 
 
 def _anneal_params(p: MppibParams, mppi_cfg) -> None:
-    """The refusals of annealed MPPI (DESIGN.md section 2, "Annealed MPPI").  The schedule itself is a device buffer the planner registers
+    """The annealed-MPPI keys (DESIGN.md section 2, "Annealed MPPI").  The schedule itself is a device buffer the planner registers
     (mppib_set_anneal), so the parameter block does not change."""
     n, ci, ch = anneal_config(mppi_cfg)
     if not 1 <= n <= MAX_ANNEAL:
@@ -528,17 +503,6 @@ def _anneal_params(p: MppibParams, mppi_cfg) -> None:
     if s.min() < ANNEAL_MIN_SCALE:
         raise ValueError(f"annealed MPPI: the smallest noise scale c_i^(N-1) c_h^(T-1) = {s.min():.3g} is below 2^-20 (anneal_iterations = {n}, "
                          f"anneal_iter_decay = {ci}, anneal_horizon_decay = {ch}, horizon = {p.T})")
-    if p.mode == MODE_CEM:
-        raise ValueError("annealed MPPI excludes mppi_mode cem, which has its own sigma")
-    if p.mode == MODE_SMOOTH:
-        raise ValueError("annealed MPPI excludes mppi_mode smooth")
-    if str(getattr(mppi_cfg, "sampling_method", "halton")) == "halton":
-        raise ValueError("annealed MPPI excludes sampling_method halton: the library is drawn once, so every iteration would reuse the same "
-                         "directions; use random or colored")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("annealed MPPI excludes update_cov and update_lambda (and so every cov_type)")
-    if p.n_modes > 1:
-        raise ValueError("annealed MPPI excludes n_modes > 1: the Stein coupling's Sigma^-1 metric would need the schedule")
 
 
 def spline_knot_vector(T: int, P: int, d: int):
@@ -604,9 +568,9 @@ def spline_initial_knots(T: int, P: int, d: int, U_init):
     return np.stack([np.interp(xi, np.arange(T, dtype=np.float64), U[:, j]) for j in range(U.shape[1])], axis=1).astype(np.float32)
 
 
-def _spline_params(p: MppibParams, mppi_cfg, nu: int) -> None:
-    """The `control_knots` / `spline_degree` keys of spline MPPI (DESIGN.md section 2, "Spline MPPI") and what they exclude.  P = 0 leaves
-    both fields 0, so the block is today's byte for byte."""
+def _spline_params(p: MppibParams, mppi_cfg) -> None:
+    """The `control_knots` / `spline_degree` keys of spline MPPI (DESIGN.md section 2, "Spline MPPI").  P = 0 leaves both fields 0, so the
+    block is today's byte for byte."""
     P, d = int(getattr(mppi_cfg, "control_knots", 0)), int(getattr(mppi_cfg, "spline_degree", 1))
     if P < 0:
         raise ValueError(f"control_knots = {P} must be >= 0 (0: off)")
@@ -616,21 +580,6 @@ def _spline_params(p: MppibParams, mppi_cfg, nu: int) -> None:
         raise ValueError(f"spline_degree = {d} must be 1, 2 or 3")
     if not d + 1 <= P <= p.T:
         raise ValueError(f"control_knots = {P} must lie in spline_degree + 1 = {d + 1} .. horizon = {p.T}")
-    if P * nu > 512 or p.T > 256:
-        raise ValueError(f"control_knots needs control_knots * nu <= 512 and horizon <= 256; P*nu = {P * nu}, T = {p.T}")
-    method = str(getattr(mppi_cfg, "sampling_method", "halton"))
-    if method in ("halton", "colored"):
-        raise ValueError(f"control_knots > 0 samples its knots with sampling_method random, not {method}")
-    if p.mode == MODE_CEM or p.mode == MODE_SMOOTH:
-        raise ValueError("control_knots > 0 excludes mppi_mode cem and smooth")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("control_knots > 0 excludes update_cov and update_lambda")
-    if p.n_modes > 1 or p.n_worlds > 1:
-        raise ValueError("control_knots > 0 excludes n_modes > 1 and n_worlds > 1")
-    if anneal_on(mppi_cfg):
-        raise ValueError("control_knots > 0 excludes annealed MPPI")
-    if p.filter_u:
-        raise ValueError("control_knots > 0 excludes filter_u: the spline is smooth already, switch filter_u off")
     p.control_knots, p.spline_degree = P, d
 
 
@@ -640,8 +589,8 @@ def constraint_on(mppi_cfg) -> bool:
 
 
 def _constraint_params(p: MppibParams, mppi_cfg) -> None:
-    """The `constraint_mode` / `constraint_tol` / `constraint_lambda` keys of constrained MPPI (DESIGN.md section 2, "Constrained MPPI")
-    and what they exclude.  With the mode "none" the three fields stay 0, so the block is today's byte for byte."""
+    """The `constraint_mode` / `constraint_tol` / `constraint_lambda` keys of constrained MPPI (DESIGN.md section 2, "Constrained MPPI").
+    With the mode "none" the three fields stay 0, so the block is today's byte for byte."""
     mode = str(getattr(mppi_cfg, "constraint_mode", "none"))
     if mode not in ("none", "feasible_first"):
         raise ValueError(f"unknown constraint_mode {mode!r} (none | feasible_first)")
@@ -654,19 +603,82 @@ def _constraint_params(p: MppibParams, mppi_cfg) -> None:
     lam_c = float(p.lambda_ if lam_c is None else lam_c)
     if not (math.isfinite(lam_c) and lam_c > 0.0):
         raise ValueError(f"constraint_lambda = {lam_c} must be finite and > 0")
-    if p.mode == MODE_CEM or p.mode == MODE_SMOOTH:
-        raise ValueError("constraint_mode: feasible_first excludes mppi_mode cem and smooth")
-    if p.update_cov or p.update_lambda:
-        raise ValueError("constraint_mode: feasible_first excludes update_cov and update_lambda")
-    if p.n_modes > 1:
-        raise ValueError("constraint_mode: feasible_first excludes n_modes > 1")
-    if p.n_worlds > 1:
-        raise ValueError("constraint_mode: feasible_first excludes n_worlds > 1")
-    if anneal_on(mppi_cfg):
-        raise ValueError("constraint_mode: feasible_first excludes annealed MPPI")
-    if p.control_knots > 0:
-        raise ValueError("constraint_mode: feasible_first excludes control_knots > 0")
     p.constraint_mode, p.constraint_tol, p.constraint_lambda = 1, tol, lam_c
+
+
+class Feature(NamedTuple):
+    name: str                                     # how the messages name it
+    on: Callable                                  # (params, mppi_cfg or None) -> bool; without a config the block alone decides
+    limit: Optional[Tuple[Optional[int], int, str]] = None   # (largest horizon or None, largest rows * nu, the rows: "T" or "control_knots")
+    no_prior: Optional[str] = None                # why the planner refuses a prior with it; None: it takes one
+    setter: Optional[str] = None                  # the backend method that registers its device state
+
+
+CEM, SMOOTH, HALTON, COLORED = "mppi_mode: cem", "mppi_mode: smooth", "sampling_method: halton", "sampling_method: colored"
+WORLDS, MODES, ANNEALED, KNOTS, CONSTRAINED = "n_worlds > 1", "n_modes > 1", "annealed MPPI", "control_knots > 0", "constraint_mode: feasible_first"
+FEATURES = (
+    Feature(CEM, lambda p, c: p.mode == MODE_CEM, (256, 512, "T"), setter="set_distribution"),
+    Feature(SMOOTH, lambda p, c: p.mode == MODE_SMOOTH, (256, 512, "T"),
+            "the prior row would be an action, the samples are derivatives", "set_smooth_state"),
+    Feature(HALTON, lambda p, c: c is not None and str(getattr(c, "sampling_method", "halton")) == "halton"),
+    Feature(COLORED, lambda p, c: c is not None and str(getattr(c, "sampling_method", "halton")) == "colored", (256, 512, "T")),
+    Feature("update_cov", lambda p, c: bool(p.update_cov), setter="set_distribution"),
+    Feature("update_lambda", lambda p, c: bool(p.update_lambda), setter="set_distribution"),
+    Feature("cov_type: horizon", lambda p, c: bool(p.cov_horizon)),
+    Feature("filter_u", lambda p, c: bool(p.filter_u)),
+    Feature(WORLDS, lambda p, c: p.n_worlds > 1, no_prior="the prior row would have to fill a whole group of worlds"),
+    Feature(MODES, lambda p, c: p.n_modes > 1, (None, 512, "T"), "the prior row would belong to no mode", "set_distribution"),
+    Feature(ANNEALED, lambda p, c: c is not None and anneal_on(c), setter="set_anneal"),
+    Feature(KNOTS, lambda p, c: p.control_knots > 0, (256, 512, "control_knots"),
+            "the prior row is an action sequence and cannot be written as knots", "set_spline"),
+    Feature(CONSTRAINED, lambda p, c: bool(p.constraint_mode), setter="set_constraint"),
+)
+_CEM_SMOOTH, _ADAPTIVE = (CEM, SMOOTH), ("update_cov", "update_lambda")
+# (features, what each of them excludes, the wording after its name); mode_refusal reports the first that applies.  csrc/api.cu: the same pairs
+EXCLUSIONS = (
+    ((COLORED,), ("cov_type: horizon",), "excludes cov_type: horizon, whose Sigma_H already models the time correlation"),
+    ((CEM,), _ADAPTIVE, "has its own update rule and excludes update_cov and update_lambda"),
+    ((CEM,), (HALTON,), "samples with sampling_method random or colored, not halton"),
+    ((SMOOTH, KNOTS, CONSTRAINED), _ADAPTIVE, "excludes update_cov and update_lambda"),
+    ((SMOOTH,), ("filter_u",), "excludes filter_u: the actions are already smooth, switch filter_u off"),
+    ((SMOOTH,), (HALTON,), "samples its derivative with sampling_method random, not halton"),
+    ((SMOOTH,), (COLORED,), "samples its derivative with sampling_method random, not colored"),
+    ((WORLDS, MODES, KNOTS, CONSTRAINED), _CEM_SMOOTH, "excludes mppi_mode cem and smooth"),
+    ((WORLDS,), ("cov_type: horizon",), "excludes cov_type: horizon"),
+    ((MODES,), _ADAPTIVE, "excludes update_cov and update_lambda: the adapted distribution belongs to one mean"),
+    ((MODES, CONSTRAINED), (WORLDS,), "excludes n_worlds > 1"),
+    ((ANNEALED,), (CEM,), "excludes mppi_mode cem, which has its own sigma"),
+    ((ANNEALED,), (SMOOTH,), "excludes mppi_mode smooth"),
+    ((ANNEALED,), (HALTON,), "excludes sampling_method halton: the library is drawn once, so every iteration would reuse the same directions; use random or colored"),
+    ((ANNEALED,), _ADAPTIVE, "excludes update_cov and update_lambda (and so every cov_type)"),
+    ((ANNEALED,), (MODES,), "excludes n_modes > 1: the Stein coupling's Sigma^-1 metric would need the schedule"),
+    ((KNOTS,), (HALTON,), "samples its knots with sampling_method random, not halton"),
+    ((KNOTS,), (COLORED,), "samples its knots with sampling_method random, not colored"),
+    ((KNOTS,), (MODES, WORLDS), "excludes n_modes > 1 and n_worlds > 1"),
+    ((KNOTS, CONSTRAINED), (ANNEALED,), "excludes annealed MPPI"),
+    ((KNOTS,), ("filter_u",), "excludes filter_u: the spline is smooth already, switch filter_u off"),
+    ((CONSTRAINED,), (MODES,), "excludes n_modes > 1"),
+    ((CONSTRAINED,), (KNOTS,), "excludes control_knots > 0"),
+)
+
+
+def mode_refusal(p: MppibParams, nu: int, mppi_cfg=None, anneal: bool = False) -> Optional[str]:
+    """Why the FEATURES a block switches on cannot run together, or None: the first size limit, then the first exclusion.  mppi_cfg adds
+    the sampling and annealing keys; anneal=True counts a registered annealing schedule as on."""
+    on = [f for f in FEATURES if f.on(p, mppi_cfg) or (anneal and f.name == ANNEALED)]
+    for f in on:
+        if f.limit:
+            t_max, n_max, rows = f.limit
+            n = getattr(p, rows) * nu
+            if p.T > (t_max or p.T) or n > n_max:
+                need = (f"horizon <= {t_max} and " if t_max else "") + ("horizon" if rows == "T" else rows) + f" * nu <= {n_max}"
+                return f"{f.name} needs {need}; T = {p.T}, {rows}*nu = {n}"
+    names = {f.name for f in on}
+    for subjects, group, text in EXCLUSIONS:
+        for name in subjects:
+            if name in names and names.intersection(group):
+                return f"{name} {text}"
+    return None
 
 
 def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tuple]) -> MppibParams:
@@ -707,11 +719,6 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     beta = float(getattr(mppi_cfg, "noise_beta", 2.0))
     if not (math.isfinite(beta) and beta >= 0.0):
         raise ValueError(f"noise_beta = {beta} must be finite and >= 0")
-    if str(getattr(mppi_cfg, "sampling_method", "halton")) == "colored":
-        if p.cov_horizon:
-            raise ValueError("sampling_method: colored excludes cov_type: horizon, whose Sigma_H already models the time correlation")
-        if p.T > 256 or p.T * nu > 512:
-            raise ValueError(f"sampling_method: colored needs horizon <= 256 and horizon * nu <= 512; T = {p.T}, T*nu = {p.T * nu}")
     if p.mode == MODE_CEM:
         _cem_params(p, mppi_cfg, nu)
     p.u_scale = float(mppi_cfg.u_scale)
@@ -748,8 +755,11 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     _risk_params(p, mppi_cfg, int(K_local))
     _modes_params(p, mppi_cfg)
     _anneal_params(p, mppi_cfg)
-    _spline_params(p, mppi_cfg, nu)
+    _spline_params(p, mppi_cfg)
     _constraint_params(p, mppi_cfg)
+    why = mode_refusal(p, nu, mppi_cfg)
+    if why:
+        raise ValueError(why)
     p.rand_seed = int(getattr(mppi_cfg, "seed_val", 0)) & 0xFFFFFFFF
     p.nobs = len(obs_items)
     for i, (kind, index) in enumerate(obs_items):

@@ -27,8 +27,8 @@ import os
 import torch
 
 from ..backend import shard_row_floats
-from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, anneal_config, anneal_on, anneal_schedule, constraint_on, spline_basis,
-                          spline_initial_knots, spline_table)
+from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, FEATURES, anneal_config, anneal_on, anneal_schedule, constraint_on,
+                          spline_basis, spline_initial_knots, spline_table)
 
 
 class _NoRange:
@@ -189,29 +189,19 @@ class MPPIPlanner:
         # Smooth MPPI (DESIGN.md section 2, "Smooth MPPI"): U is the control derivative; K1 integrates it from the last executed action
         # (the smooth state, a device buffer K4 updates), so the executed command changes by at most du_max * dt per plan
         self.smooth = str(getattr(cfg, "mppi_mode", "")) == "smooth"
-        if self.smooth and bool(getattr(cfg, "use_priors", False)) and prior is not None:
-            raise ValueError("mppi_mode: smooth does not take a prior: the prior row would be an action, the samples are derivatives")
         if self.smooth and self.u_per_command > 1:
             raise ValueError("mppi_mode: smooth executes one action per plan (u_per_command = 1): U holds derivatives, not actions")
         # risk-aware MPPI (DESIGN.md section 2, "Risk-aware MPPI"): the K rollouts are K / R control samples, each rolled out in the
         # same R randomised worlds and scored by the CVaR of its R costs; make_params checks the keys against the mode
         self.n_worlds = int(getattr(cfg, "n_worlds", 1))
         self.control_samples = self.K_total // max(1, self.n_worlds)
-        if self.n_worlds > 1:
-            if bool(getattr(cfg, "use_priors", False)) and prior is not None:
-                raise ValueError("n_worlds > 1 does not take a prior: the prior row would have to fill a whole group of worlds")
-            if not _randomised(sim.scene.model):
-                raise ValueError("n_worlds > 1 needs a scene that randomises its rollouts (noise_percentage_mass, noise_percentage_friction "
-                                 "or noise_sigma_size on some actor): without it the worlds would be identical copies")
+        if self.n_worlds > 1 and not _randomised(sim.scene.model):
+            raise ValueError("n_worlds > 1 needs a scene that randomises its rollouts (noise_percentage_mass, noise_percentage_friction "
+                             "or noise_sigma_size on some actor): without it the worlds would be identical copies")
         # multi-modal MPPI (DESIGN.md section 2, "Multi-modal MPPI"): M nominal sequences side by side, each sampled by its block of
         # K_total / M samples and coupled by a Stein-variational step on the device; the mode state (active mode, F[M], U_exec) is a device
         # buffer K4 writes; make_params checks the keys against the mode
         self.n_modes = int(getattr(cfg, "n_modes", 1))
-        if self.n_modes > 1:
-            if bool(getattr(cfg, "use_priors", False)) and prior is not None:
-                raise ValueError("n_modes > 1 does not take a prior: the prior row would belong to no mode")
-            if not hasattr(sim.backend, "set_distribution"):
-                raise ValueError(f"n_modes > 1 needs a backend with set_distribution ({type(sim.backend).__name__} has none)")
         # adaptive MPPI (DESIGN.md section 2): the live (lambda, cov) pair is a device buffer that K1 / K3 read and K4 updates, so a
         # captured plan graph follows it without re-capture
         self.update_cov = bool(getattr(cfg, "update_cov", False))
@@ -231,8 +221,6 @@ class MPPIPlanner:
         # the knots and interpolates the actions, K3 / K4 run on the knots; make_params checks the keys against the mode
         self.control_knots = int(getattr(cfg, "control_knots", 0))
         self.spline_degree = int(getattr(cfg, "spline_degree", 1))
-        if self.control_knots > 0 and bool(getattr(cfg, "use_priors", False)) and prior is not None:
-            raise ValueError("control_knots > 0 does not take a prior: the prior row is an action sequence and cannot be written as knots")
         self.backend = sim.backend
         # constrained MPPI (DESIGN.md section 2, "Constrained MPPI"): running_constraint returns a signed margin per row (<= 0 satisfied),
         # written into a (T, K) device buffer K3 reads; make_params checks the keys against the mode
@@ -240,18 +228,6 @@ class MPPIPlanner:
         self._running_constraint = running_constraint
         if self.constrained and running_constraint is None:
             raise ValueError("constraint_mode: feasible_first needs a running_constraint (the Objective's compute_constraint)")
-        if self.constrained and not hasattr(self.backend, "set_constraint"):
-            raise ValueError(f"constraint_mode: feasible_first needs a backend with set_constraint ({type(self.backend).__name__} has none)")
-        if self.control_knots > 0 and not hasattr(self.backend, "set_spline"):
-            raise ValueError(f"control_knots > 0 needs a backend with set_spline ({type(self.backend).__name__} has none)")
-        if self.adaptive and not hasattr(self.backend, "set_distribution"):
-            raise ValueError(f"update_cov / update_lambda need a backend with set_distribution ({type(self.backend).__name__} has none)")
-        if self.cem and not hasattr(self.backend, "set_distribution"):
-            raise ValueError(f"mppi_mode: cem needs a backend with set_distribution ({type(self.backend).__name__} has none)")
-        if self.annealed and not hasattr(self.backend, "set_anneal"):
-            raise ValueError(f"annealed MPPI needs a backend with set_anneal ({type(self.backend).__name__} has none)")
-        if self.smooth and not hasattr(self.backend, "set_smooth_state"):
-            raise ValueError(f"mppi_mode: smooth needs a backend with set_smooth_state ({type(self.backend).__name__} has none)")
         self._peer_exchange = False
         self._peer_capable = (self.world > 1 and getattr(self.backend, "name", "") == "cuda"
                               and os.environ.get("MPPIB_EXCHANGE", "peer") == "peer")
@@ -260,6 +236,11 @@ class MPPIPlanner:
         sim.configure(mppi_cfg=cfg, horizon=self.T)      # (re)bakes Sigma / bounds / lambda into the kernel parameter block
         use_prior = bool(getattr(cfg, "use_priors", False)) and prior is not None
         self.use_priors = use_prior
+        for f in [f for f in FEATURES if f.on(self.backend.params, cfg)]:    # make_params has refused the modes that exclude each other
+            if use_prior and f.no_prior:
+                raise ValueError(f"{f.name} does not take a prior: {f.no_prior}")
+            if f.setter and not hasattr(self.backend, f.setter):
+                raise ValueError(f"{f.name} needs a backend with {f.setter} ({type(self.backend).__name__} has none)")
         if rollout_mode == "auto":
             rollout_mode = "stepwise" if use_prior else "batched"
         if rollout_mode not in ("batched", "stepwise"):

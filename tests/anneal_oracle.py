@@ -14,7 +14,7 @@ import torch
 
 import colored_oracle as co
 import risk_oracle as ro
-from mppi_isaac_b200.model.blob import MAX_ANNEAL, MODE_MEAN, MODE_SIMPLE, anneal_schedule
+from mppi_isaac_b200.model.blob import MAX_ANNEAL, MODE_SIMPLE, anneal_schedule, mode_refusal
 from oracle.backend import _np
 
 
@@ -86,15 +86,9 @@ def reduce(params, nu, cost, x, U, r_row):
     return np.concatenate([[beta, w.sum()], np.einsum("tjk,k->tj", xr, w).reshape(-1)]).astype(np.float32)
 
 
-def refusal(params):
+def refusal(params, nu):
     """The library's refusal of a parameter block while a schedule is registered, or None."""
-    if params.mode not in (MODE_SIMPLE, MODE_MEAN):
-        return "annealed MPPI excludes mode cem and mode smooth"
-    if params.update_cov or params.update_lambda:
-        return "annealed MPPI excludes update_cov and update_lambda"
-    if params.n_modes > 1:
-        return "annealed MPPI excludes n_modes > 1"
-    return None
+    return mode_refusal(params, nu, anneal=True)
 
 
 class AnnealOracleBackend(ro.RiskOracleBackend):
@@ -112,7 +106,7 @@ class AnnealOracleBackend(ro.RiskOracleBackend):
             raise RuntimeError(f"mppib_set_anneal: n_iterations = {n_iterations} out of range [1, {MAX_ANNEAL}]")
         if state.numel() != 1 + 2 * int(n_iterations) * int(self.params.T):
             raise RuntimeError("mppib_set_anneal: the buffer does not hold 1 + 2*N*T floats")
-        why = refusal(self.params)
+        why = refusal(self.params, self.model.nu)
         if why:
             raise RuntimeError(f"mppib_set_anneal: {why}")
         self.anneal, self.anneal_n, self.anneal_T = state, int(n_iterations), int(self.params.T)
@@ -122,7 +116,7 @@ class AnnealOracleBackend(ro.RiskOracleBackend):
             return False
         if int(self.params.T) != self.anneal_T:
             raise RuntimeError(f"{who}: the annealing schedule was registered for T = {self.anneal_T}, the parameter block has T = {self.params.T}")
-        why = refusal(self.params)
+        why = refusal(self.params, self.model.nu)
         if why:
             raise RuntimeError(f"{who}: {why}")
         return True
