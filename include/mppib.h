@@ -54,7 +54,7 @@
 extern "C" {
 #endif
 
-#define MPPIB_ABI_VERSION 23
+#define MPPIB_ABI_VERSION 24
 
 #define MPPIB_MAX_BODIES 16   /* moving (1-DoF) bodies of the articulation            */
 #define MPPIB_MAX_LINKS  32   /* URDF links whose state can be observed               */
@@ -98,6 +98,9 @@ extern "C" {
 #define MPPIB_MAX_MODES 16    /* multi-modal MPPI: largest n_modes */
 #define MPPIB_MAX_ANNEAL 16   /* annealed MPPI: largest number of MPPI iterations per plan */
 #define MPPIB_MAX_SPLINE_DEGREE 3   /* spline MPPI: largest spline_degree */
+#define MPPIB_ESS_GRID 65           /* ESS-targeted temperature: grid temperatures lambda_j = lambda_ 2^((j - 32)/4), j = 0 .. 64 */
+#define MPPIB_ESS_ROW_FLOATS 196    /* its shard row: (n_valid as int32 bits, (m_j, s1_j, s2_j)[65]) */
+#define MPPIB_ESS_STATE_FLOATS 197  /* its state: (lambda_j[65], 1/lambda_j[65], n_valid as int32 bits, lambda, ESS_j[65]) */
 
 typedef struct MppibModel {
     int32_t abi_version;
@@ -241,6 +244,10 @@ typedef struct MppibParams {
     float   constraint_tol;    /* a sample is feasible when its total violation V_k <= tol; finite and >= 0                             */
     float   constraint_lambda; /* lambda_c: the temperature of the violation fallback; finite and > 0                                    */
     int32_t constraint_pad;    /* 0; keeps the spline fields below at the 8-byte alignment they had before the constraint fields       */
+    /* ESS-targeted temperature (see "ESS-targeted temperature" below); lambda_ess = 0 (and a zero-initialised block) keeps today's planner;
+       the two fields sit before the spline fields, so those keep their 8-byte alignment and stay the last of the block */
+    int32_t lambda_ess;        /* 1: every plan chooses lambda on the device so that the weights keep ess_target of the valid samples     */
+    float   ess_target;        /* rho in (0, 1], finite, read only when lambda_ess = 1                                                   */
     /* spline MPPI (see "Spline MPPI" below); control_knots = 0 (and a zero-initialised block) keeps today's planner                   */
     int32_t control_knots;     /* P: U, the samples K3 weights and the shard row hold P knots per control instead of T steps            */
     int32_t spline_degree;     /* d in 1 .. MPPIB_MAX_SPLINE_DEGREE, read only when control_knots > 0; P in d + 1 .. T, P*nu <= 512   */
@@ -567,6 +574,39 @@ int32_t mppib_sample_spline(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  * today's bit for bit.  Registration records (T, K); reduce and finalize refuse a handle whose constraint_mode and registration disagree
  * or whose T or K changed since, and one with a distribution or annealing schedule registered.  NULL switches it off.             */
 int32_t mppib_set_constraint(MppibHandle h, const float* viol, float* cstate);
+
+/* ESS-targeted temperature (lambda_ess = 1, ess_target = rho; modes SIMPLE and MEAN, fixed, diagonal or full Sigma, any K1 but smooth's,
+ * filter_u, the null / prior rows and any number of ranks; no update_lambda, cov_horizon, cem, smooth, n_worlds > 1, n_modes > 1,
+ * control_knots > 0, constraint_mode or annealing).  Every plan chooses its temperature from its own costs, after the Objective's cost
+ * (and the stepwise prior row's noise rewrite) and before K3:
+ *   per sample  C_k = sum_t gamma^t c[t][k], q_k = sum_r (Sigma^-1 U)_r x[r][k] in SIMPLE mode (Sigma^-1 = K3's: sigma_inv, diag(1/cov)
+ *               with update_cov, dist's full one with cov_full), q_k = 0 in MEAN mode, so S_k(lambda) = C_k + lambda q_k is K3's S; a
+ *               sample is valid when k < K and C_k and q_k are finite
+ *   grid        lambda_j = lambda_ 2^((j - 32)/4), j = 0 .. 64, and 1/lambda_j, each computed in float64 and rounded once by the caller
+ *               into the state
+ *   curve       a_jk = C_k / lambda_j + q_k; ESS_j = (sum_k e^-a_jk)^2 / sum_k e^-2a_jk over the valid samples of every rank, shifted by
+ *               m_j = min_k a_jk; N = the valid samples of every rank
+ *   rule        tau = rho N, j* = the first j with ESS_j >= tau: lambda = lambda_64 if there is none, lambda_0 if j* = 0, otherwise
+ *               lambda_{j*-1} 2^(theta/4), theta = (ln tau - ln ESS_{j*-1}) / (ln ESS_{j*} - ln ESS_{j*-1}); N = 0 keeps dist[0]
+ *   result      dist[0] <- lambda; K1 .. K4 and the shift then run the registered distribution's path (update_lambda is off, so K4 leaves
+ *               dist[0] as it is, and K1 keeps the fixed Sigma unless update_cov is on)
+ * The distribution (mppib_set_distribution, (lambda, cov[nu]) or cov_full's layout) is registered even with both adaptive flags off, and
+ * the state is a device buffer registered with mppib_set_temperature (caller-owned; the caller fills the grid):
+ *   state    [MPPIB_ESS_STATE_FLOATS]  (lambda_j[65], 1/lambda_j[65], n_valid as int32 bits, lambda chosen, ESS_j[65]); the solve writes
+ *            the last three
+ *   row      [MPPIB_ESS_ROW_FLOATS]    (n_valid as int32 bits, (m_j, s1_j, s2_j)[65]) of one shard; s1 = sum e^-(a - m),
+ *            s2 = sum e^-2(a - m)
+ * Every rank combines the rows in rank order (CTA partials in CTA order) with the same float32 arithmetic, so all choose the same bits.
+ * Reduce and finalize refuse lambda_ess = 1 while no distribution or no state is registered: they would weight with lambda_. */
+int32_t mppib_set_temperature(MppibHandle h, float* state);
+/* The temperature pass <- the fixed mppi_torch `lambda_` of _exp_util (call site mppi_isaac.py:113): per-CTA curves over the shard, folded
+ * by the last CTA into `row` (device, MPPIB_ESS_ROW_FLOATS floats).  solve = 1: the last CTA also applies the rule -- to its own row
+ * without peers, or, with the peer window open, after publishing the row into every rank's window and acquiring every rank's row (a second
+ * exchange per plan on the window K3 / K4 use).  solve = 0 writes the row only, for an all-gather and mppib_temperature_solve.  x is the
+ * noise K3 weights in SIMPLE mode (not read in MEAN mode, may be NULL there).  Needs T <= 256 and T*nu <= 512. */
+int32_t mppib_temperature(MppibHandle h, const float* cost, const float* x, const float* U, float* row, int32_t solve, void* stream);
+/* The rule over G rows[G][MPPIB_ESS_ROW_FLOATS] (device, rank order) <- the same as above, one warp: the multi-GPU path without peers. */
+int32_t mppib_temperature_solve(MppibHandle h, const float* rows, int32_t G, void* stream);
 
 #ifdef __cplusplus
 }

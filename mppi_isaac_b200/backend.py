@@ -14,7 +14,7 @@ import weakref
 
 import torch
 
-from .model.blob import ABI_VERSION, MODE_CEM, MODE_SMOOTH, MppibModel, MppibParams
+from .model.blob import ABI_VERSION, ESS_ROW_FLOATS, ESS_STATE_FLOATS, MODE_CEM, MODE_SIMPLE, MODE_SMOOTH, MppibModel, MppibParams
 
 _LIB_PATH = os.environ.get("MPPIB_LIB") or os.path.join(os.path.dirname(os.path.abspath(__file__)), "libmppib.so")   # MPPIB_LIB: tuning builds
 _lib = None
@@ -25,7 +25,7 @@ SYMBOLS = [
     "mppib_reduce", "mppib_finalize", "mppib_shift", "mppib_noise_library", "mppib_sample_library",
     "mppib_peer_alloc", "mppib_peer_open", "mppib_peer_close", "mppib_cost_pose", "mppib_set_action_mirror", "mppib_reduce_finalize", "mppib_rollout_smem_bytes", "mppib_rollout_mapping", "mppib_rollout_mapping_for_model",
     "mppib_set_distribution", "mppib_sample_colored", "mppib_set_smooth_state", "mppib_sample_smooth", "mppib_set_anneal",
-    "mppib_set_spline", "mppib_sample_spline", "mppib_set_constraint",
+    "mppib_set_spline", "mppib_sample_spline", "mppib_set_constraint", "mppib_set_temperature", "mppib_temperature", "mppib_temperature_solve",
 ]
 
 
@@ -96,6 +96,12 @@ def shard_row_floats(params, nu):
     return 4 + n if params.constraint_mode else 2 + n
 
 
+def temperature_row_floats():
+    """Floats of one shard row of the temperature pass of lambda_mode ess: (n_valid as int32 bits, (m_j, s1_j, s2_j)[65]).  The library
+    sizes its scratch and peer window for the longer of this row and K3's."""
+    return ESS_ROW_FLOATS
+
+
 def smooth_state_floats(T, nu):
     """Floats of the smooth state of mppi_mode smooth: (a_prev[nu], A[T][nu])."""
     return int(nu) + int(T) * int(nu)
@@ -148,6 +154,7 @@ class CudaBackend:
         self._anneal_keepalive = None     # (state, N)
         self._spline_keepalive = None     # the registered spline table
         self._constraint_keepalive = None  # (viol, cstate) of constrained MPPI
+        self._temperature_keepalive = None  # the state of lambda_mode ess
         self.launches = 0   # kernels launched through this handle (bench.py's gpu_launches)
 
     # -- lifetime -------------------------------------------------------------------------------
@@ -182,6 +189,8 @@ class CudaBackend:
             if not (params.constraint_mode and viol.numel() == int(params.T) * int(params.K)
                     and self.lib.mppib_set_constraint(self.handle, _ptr(viol), _ptr(cstate)) == 0):
                 self._constraint_keepalive = None
+        if self._temperature_keepalive is not None:      # ... and its temperature state
+            self._check(self.lib.mppib_set_temperature(self.handle, _ptr(self._temperature_keepalive)), "mppib_set_temperature")
 
     def destroy(self):
         if self.handle:
@@ -371,6 +380,31 @@ class CudaBackend:
                 raise RuntimeError("mppib_set_constraint: cstate must be a float32 tensor of 2 values")
         self._check(self.lib.mppib_set_constraint(self.handle, _ptr(viol), _ptr(None if viol is None else cstate)), "mppib_set_constraint")
         self._constraint_keepalive = None if viol is None else (viol, cstate)
+
+    def set_temperature(self, state):
+        """lambda_mode ess: register the float32 device tensor (lambda_j[65], 1/lambda_j[65], n_valid bits, lambda, ESS_j[65]) whose grid
+        the caller filled (``blob.ess_grid``); the solve writes the rest and dist[0] (None switches it off)."""
+        if state is not None and (state.numel() != ESS_STATE_FLOATS or state.dtype != torch.float32 or not state.is_contiguous()):
+            raise RuntimeError(f"mppib_set_temperature: the state holds {ESS_STATE_FLOATS} contiguous float32 values, got {state.dtype} {state.numel()}")
+        self._check(self.lib.mppib_set_temperature(self.handle, _ptr(state)), "mppib_set_temperature")
+        self._temperature_keepalive = state
+
+    def temperature(self, cost, x, U, row, solve=True):
+        """lambda_mode ess: the temperature pass over this shard's (T, K) cost and, in SIMPLE mode, the noise K3 weights; writes the shard
+        row into ``row`` (196 floats).  solve: the last CTA also applies the rule (one rank, or every rank through the open peer window);
+        otherwise gather the rows and call ``temperature_solve``."""
+        if row is None or row.numel() != ESS_ROW_FLOATS or row.dtype != torch.float32:
+            raise RuntimeError(f"mppib_temperature: row must be a float32 tensor of {ESS_ROW_FLOATS} values")
+        self.launches += 1
+        self._check(self.lib.mppib_temperature(self.handle, _ptr(cost), _ptr(x if self.params.mode == MODE_SIMPLE else None), _ptr(U), _ptr(row),
+                                               C.c_int32(1 if solve else 0), self._stream()), "mppib_temperature")
+
+    def temperature_solve(self, rows, G):
+        """lambda_mode ess: the rule over the (G, 196) float32 device rows of every rank, in rank order."""
+        if rows.dtype != torch.float32 or not rows.is_contiguous() or rows.numel() < int(G) * ESS_ROW_FLOATS:
+            raise RuntimeError(f"mppib_temperature_solve: rows must be a contiguous float32 (G, {ESS_ROW_FLOATS}) tensor")
+        self.launches += 1
+        self._check(self.lib.mppib_temperature_solve(self.handle, _ptr(rows), C.c_int32(int(G)), self._stream()), "mppib_temperature_solve")
 
     def sample_spline(self, seed, plan_idx, k_offset, k_total, U, actions, xk, plan_ctr=None):
         """K1 of spline MPPI: knots theta~ = clamp(U + L0 z) per sample, xk[P][nu][K] = theta~ - U (SIMPLE) or theta~ (MEAN), and

@@ -16,9 +16,10 @@ void mppib_set_error(const char* fmt, ...) {
 
 // Which planning modes cannot run together (make_params refuses the same pairs): validate checks the block with anneal = false; a schedule
 // is checked with anneal = true at registration and at every launch, so that a later mppib_set_params cannot slip past it.
-enum Feature { F_CEM, F_SMOOTH, F_UPDATE_COV, F_UPDATE_LAMBDA, F_COV_HORIZON, F_FILTER_U, F_WORLDS, F_MODES, F_KNOTS, F_CONSTRAINT, F_ANNEAL };
+enum Feature { F_CEM, F_SMOOTH, F_UPDATE_COV, F_UPDATE_LAMBDA, F_COV_HORIZON, F_FILTER_U, F_WORLDS, F_MODES, F_KNOTS, F_CONSTRAINT, F_ANNEAL,
+               F_ESS, F_COUNT };
 static const char* const kFeatureNames[] = {"mode cem", "mode smooth", "update_cov", "update_lambda", "cov_horizon", "filter_u", "n_worlds > 1",
-                                            "n_modes > 1", "control_knots > 0", "constraint_mode", "annealed MPPI"};
+                                            "n_modes > 1", "control_knots > 0", "constraint_mode", "annealed MPPI", "lambda_mode: ess"};
 #define FBIT(f) (1u << (f))
 static const unsigned F_CEM_SMOOTH = FBIT(F_CEM) | FBIT(F_SMOOTH), F_ADAPTIVE = FBIT(F_UPDATE_COV) | FBIT(F_UPDATE_LAMBDA);
 struct Exclusion { Feature feature; unsigned excludes; const char* why; };     // excludes: FBIT mask; why: "" or the reason
@@ -35,13 +36,17 @@ static const Exclusion kExclusions[] = {
     {F_ANNEAL, FBIT(F_CEM), " (it has its own sigma)"},
     {F_ANNEAL, FBIT(F_SMOOTH) | F_ADAPTIVE | FBIT(F_KNOTS) | FBIT(F_CONSTRAINT), ""},
     {F_ANNEAL, FBIT(F_MODES), " (the Stein coupling's Sigma^-1 metric would need the schedule)"},
+    {F_ESS, FBIT(F_UPDATE_LAMBDA), " (two rules for one temperature)"},
+    {F_ESS, FBIT(F_COV_HORIZON), " (the shift computes lambda Sigma_H^-1 U before the temperature is known)"},
+    {F_ESS, F_CEM_SMOOTH, " (it does not weight the samples with the temperature)"},
+    {F_ESS, FBIT(F_WORLDS) | FBIT(F_MODES) | FBIT(F_KNOTS) | FBIT(F_CONSTRAINT) | FBIT(F_ANNEAL), ""},
 };
 
 int check_exclusions(const MppibParams& p, bool anneal, const char* who) {
     const bool on[] = {p.mode == MPPIB_MODE_CEM, p.mode == MPPIB_MODE_SMOOTH, p.update_cov != 0, p.update_lambda != 0, p.cov_horizon != 0,
-                       p.filter_u != 0, p.n_worlds > 1, p.n_modes > 1, p.control_knots > 0, p.constraint_mode != 0, anneal};
+                       p.filter_u != 0, p.n_worlds > 1, p.n_modes > 1, p.control_knots > 0, p.constraint_mode != 0, anneal, p.lambda_ess != 0};
     for (const Exclusion& e : kExclusions)
-        for (int f = 0; f <= F_ANNEAL; ++f)
+        for (int f = 0; f < F_COUNT; ++f)
             MPPIB_REQUIRE(!(on[e.feature] && on[f] && (e.excludes & FBIT(f))), "%s%s%s excludes %s%s", who, *who ? ": " : "", kFeatureNames[e.feature],
                           kFeatureNames[f], e.why);
     return 0;
@@ -124,6 +129,9 @@ static int validate(const MppibModel* m, const MppibParams* p) {
         MPPIB_REQUIRE(isfinite(p->constraint_tol) && p->constraint_tol >= 0.f, "constraint_tol = %g must be finite and >= 0", p->constraint_tol);
         MPPIB_REQUIRE(isfinite(p->constraint_lambda) && p->constraint_lambda > 0.f, "constraint_lambda = %g must be finite and > 0", p->constraint_lambda);
     }
+    MPPIB_REQUIRE(p->lambda_ess == 0 || p->lambda_ess == 1, "lambda_ess = %d must be 0 or 1", p->lambda_ess);
+    if (p->lambda_ess)
+        MPPIB_REQUIRE(isfinite(p->ess_target) && p->ess_target > 0.f && p->ess_target <= 1.f, "ess_target = %g must be finite and in (0, 1]", p->ess_target);
     if (int rc = check_exclusions(*p, false, "")) return rc;
     for (int i = 0; i < p->nobs; ++i) {
         const int kd = p->obs[i].kind, ix = p->obs[i].index;
@@ -183,6 +191,13 @@ int check_constraint(const MppibContext* c, const char* who) {
     MPPIB_REQUIRE(c->viol_T == p.T && c->viol_K == p.K, "%s: the violation buffer was registered for (T, K) = (%d, %d), the handle has (%d, %d); register a "
                   "buffer for the new block (mppib_set_constraint)", who, c->viol_T, c->viol_K, p.T, p.K);
     MPPIB_REQUIRE(c->dist == nullptr, "%s: constraint_mode runs plain MPPI; register no distribution", who);
+    return 0;
+}
+
+int check_temperature(const MppibContext* c, const char* who) {
+    if (!c->params.lambda_ess) return 0;
+    MPPIB_REQUIRE(c->dist != nullptr && c->temp != nullptr, "%s: lambda_mode ess needs a distribution (mppib_set_distribution) and a temperature "
+                  "state (mppib_set_temperature) registered; without them K3 would weight with the fixed lambda_", who);
     return 0;
 }
 
@@ -374,6 +389,7 @@ int32_t mppib_reduce(MppibHandle h, const float* cost, const float* x, const flo
     if (int rc = check_anneal(h, "mppib_reduce")) return rc;
     if (int rc = check_spline(h, "mppib_reduce")) return rc;
     if (int rc = check_constraint(h, "mppib_reduce")) return rc;
+    if (int rc = check_temperature(h, "mppib_reduce")) return rc;
     MPPIB_REQUIRE(((uintptr_t)cost & 15) == 0 && ((uintptr_t)x & 15) == 0, "mppib_reduce: cost/x must be 16-byte aligned");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, nullptr, nullptr, nullptr, (cudaStream_t)stream);
@@ -384,6 +400,7 @@ int32_t mppib_reduce_finalize(MppibHandle h, const float* cost, const float* x, 
     if (int rc = check_anneal(h, "mppib_reduce_finalize")) return rc;
     if (int rc = check_spline(h, "mppib_reduce_finalize")) return rc;
     if (int rc = check_constraint(h, "mppib_reduce_finalize")) return rc;
+    if (int rc = check_temperature(h, "mppib_reduce_finalize")) return rc;
     MPPIB_REQUIRE(h->peer_world <= 1, "mppib_reduce_finalize is the single-GPU plan tail; with an open peer window use mppib_reduce + mppib_finalize");
     MPPIB_ON_DEVICE(h);
     return launch_reduce(h, cost, x, U, partial, U, action_out, stats, (cudaStream_t)stream);
@@ -394,6 +411,7 @@ int32_t mppib_finalize(MppibHandle h, const float* partials, int32_t G, float* U
     if (int rc = check_anneal(h, "mppib_finalize")) return rc;
     if (int rc = check_spline(h, "mppib_finalize")) return rc;
     if (int rc = check_constraint(h, "mppib_finalize")) return rc;
+    if (int rc = check_temperature(h, "mppib_finalize")) return rc;
     if (!partials) {
         MPPIB_REQUIRE(h->peer_world >= 2 && G == h->peer_world, "mppib_finalize: partials == NULL needs an open peer window and G == world (G=%d, world=%d)", G, h->peer_world);
         for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_finalize: peer %d is not open", g);
@@ -478,6 +496,30 @@ int32_t mppib_set_constraint(MppibHandle h, const float* viol, float* cstate) {
     MPPIB_REQUIRE(((uintptr_t)viol & 15) == 0, "mppib_set_constraint: viol must be 16-byte aligned");
     h->viol = viol; h->cstate = cstate; h->viol_T = h->params.T; h->viol_K = h->params.K;
     return 0;
+}
+
+int32_t mppib_set_temperature(MppibHandle h, float* state) {
+    MPPIB_REQUIRE(h != nullptr, "null handle");
+    h->temp = state;
+    return 0;
+}
+
+int32_t mppib_temperature(MppibHandle h, const float* cost, const float* x, const float* U, float* row, int32_t solve, void* stream) {
+    MPPIB_REQUIRE(h && cost && U && row && (x || h->params.mode != MPPIB_MODE_SIMPLE), "mppib_temperature: null argument");
+    MPPIB_REQUIRE(h->params.lambda_ess, "mppib_temperature: the parameter block has lambda_ess = 0");
+    if (int rc = check_temperature(h, "mppib_temperature")) return rc;
+    if (solve && h->peer_world > 1)
+        for (int g = 0; g < h->peer_world; ++g) MPPIB_REQUIRE(h->peer_win[g] != nullptr, "mppib_temperature: peer %d is not open", g);
+    MPPIB_ON_DEVICE(h);
+    return launch_temperature(h, cost, x, U, row, solve != 0, (cudaStream_t)stream);
+}
+
+int32_t mppib_temperature_solve(MppibHandle h, const float* rows, int32_t G, void* stream) {
+    MPPIB_REQUIRE(h && rows && G >= 1, "mppib_temperature_solve: bad argument");
+    MPPIB_REQUIRE(h->params.lambda_ess, "mppib_temperature_solve: the parameter block has lambda_ess = 0");
+    if (int rc = check_temperature(h, "mppib_temperature_solve")) return rc;
+    MPPIB_ON_DEVICE(h);
+    return launch_temperature_solve(h, rows, G, (cudaStream_t)stream);
 }
 
 int32_t mppib_shift(MppibHandle h, float* U, uint32_t* plan_ctr, void* stream) {

@@ -55,6 +55,7 @@ struct MppibContext {
     const float* viol;                         // constrained MPPI: device g[T][K] K3 reads (nullable)
     float* cstate;                             // constrained MPPI: device (n_feasible as int bits, min V), written by K4
     int viol_T, viol_K;                        // the (T, K) the buffer was registered for
+    float* temp;                               // ESS-targeted temperature: device (lambda_j, 1/lambda_j, n_valid, lambda, ESS_j), written by the solve (nullable)
     // adaptive MPPI with cov_horizon (update_cov): device buffers owned by the handle, sized for (K, n = T*nu) by alloc_horizon
     float* hz_S;                               // [K] S_k of the last K3, read by the SYRK
     float* hz_g;                               // [n] lambda Sigma_H^-1 U of the last mppib_shift (K3 reads it in SIMPLE mode)
@@ -173,7 +174,11 @@ static inline Rule configured_rule(const MppibParams& p) {
     if (p.constraint_mode) return RULE_FEASIBLE;
     return RULE_PLAIN;
 }
-static inline int partial_row_capacity(const MppibParams& p, int nu) { return shard_row_floats(configured_rule(p), p, nu); }
+// ESS-targeted temperature: its shard row travels through the same scratch and peer window, so they hold the longer of the two rows
+static inline int partial_row_capacity(const MppibParams& p, int nu) {
+    const int P = shard_row_floats(configured_rule(p), p, nu);
+    return p.lambda_ess && P < MPPIB_ESS_ROW_FLOATS ? MPPIB_ESS_ROW_FLOATS : P;
+}
 // Risk-aware MPPI (n_worlds = R > 1, a power of two): global rollout kg = c*R + r runs control sample c in world r.  K1 keys its draws
 // and its null / prior rows by c, K2 keys the per-rollout randomisation by r.  R <= 1 (and a zero-initialised block) keeps kg for both.
 __device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
@@ -206,6 +211,8 @@ __device__ __forceinline__ float feas_scale(int nf, float b, int n_all, float b_
 __device__ __forceinline__ float feas_violation(float g) { return g <= 0.f ? 0.f : g; }
 // the launch-time refusals of constrained MPPI (api.cu): the mode and the registration must agree, for the registered (T, K)
 int check_constraint(const MppibContext* c, const char* who);
+// the launch-time refusal of the ESS-targeted temperature (api.cu): lambda_ess needs a registered distribution and state
+int check_temperature(const MppibContext* c, const char* who);
 #define MPPIB_HZ_MAX_N 256                    // cov_horizon: largest n = T*nu (the packed n x n triangle K4 factors in shared memory)
 #define HZ_TILE 64                             // SYRK output tile
 #define HZ_MAX_TILES 10                        // lower-triangle tiles of a 256 x 256 C
@@ -330,6 +337,9 @@ int launch_elite(MppibContext* c, const float* cost, const float* x, float* part
                  cudaStream_t s);
 int launch_cem_finalize(MppibContext* c, const float* partials, int G, float* U, float* action_out, float* stats, cudaStream_t s);
 int launch_cem_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t s);
+// lambda_mode ess (temperature.cu): the temperature pass (+ the solve when `solve`), and the solve over G explicit rows
+int launch_temperature(MppibContext* c, const float* cost, const float* x, const float* U, float* row, bool solve, cudaStream_t s);
+int launch_temperature_solve(MppibContext* c, const float* rows, int G, cudaStream_t s);
 int alloc_horizon(MppibContext* c);           // (re)sizes the hz_* buffers for the handle's K and T*nu (frees them without cov_horizon)
 long long rollout_smem_bytes(const MppibModel& m);
 // K2, lanes-per-rollout mapping for serial chains without contacts (rollout_lanes.cu)

@@ -18,7 +18,7 @@ import numpy as np
 
 from .urdf import RobotModel, compile_urdf, load_compiled, quat_xyzw_to_R, R_to_quat_xyzw
 
-ABI_VERSION = 23
+ABI_VERSION = 24
 MAX_BODIES, MAX_LINKS, MAX_NU, MAX_OBS, MAX_FREE, MAX_SHAPES = 16, 32, 16, 64, 4, 24
 MAX_CONTACTS, MAX_SLOTS = 24, 8
 HZ_MAX_N = 256                                  # cov_type horizon: largest T*nu
@@ -35,6 +35,7 @@ MAX_MODES = 16                                  # multi-modal MPPI: largest n_mo
 MAX_ANNEAL = 16                                 # annealed MPPI: largest anneal_iterations
 ANNEAL_MIN_SCALE = 2.0 ** -20                   # annealed MPPI: smallest noise scale, so that r = 1 / s^2 stays finite in float32
 MAX_SPLINE_DEGREE = 3                           # spline MPPI: largest spline_degree
+ESS_GRID, ESS_ROW_FLOATS, ESS_STATE_FLOATS = 65, 196, 197   # ESS-targeted temperature: grid points, shard row, state (include/mppib.h)
 
 f32, i32 = C.c_float, C.c_int32
 
@@ -86,6 +87,7 @@ class MppibParams(C.Structure):
         ("n_worlds", i32), ("risk_tail", i32),
         ("n_modes", i32), ("mode_margin", f32), ("mode_samples", i32),
         ("constraint_mode", i32), ("constraint_tol", f32), ("constraint_lambda", f32), ("constraint_pad", i32),
+        ("lambda_ess", i32), ("ess_target", f32),
         ("control_knots", i32), ("spline_degree", i32),
     ]
 
@@ -606,6 +608,33 @@ def _constraint_params(p: MppibParams, mppi_cfg) -> None:
     p.constraint_mode, p.constraint_tol, p.constraint_lambda = 1, tol, lam_c
 
 
+def ess_on(mppi_cfg) -> bool:
+    """True when the config asks for the ESS-targeted temperature (`lambda_mode: ess`)."""
+    return str(getattr(mppi_cfg, "lambda_mode", "fixed")) == "ess"
+
+
+def _ess_params(p: MppibParams, mppi_cfg) -> None:
+    """The `lambda_mode` / `ess_target` keys of the ESS-targeted temperature (DESIGN.md section 2, "ESS-targeted temperature").  With
+    lambda_mode fixed both fields stay 0, so the block is today's byte for byte."""
+    mode = str(getattr(mppi_cfg, "lambda_mode", "fixed"))
+    if mode not in ("fixed", "ess"):
+        raise ValueError(f"unknown lambda_mode {mode!r} (fixed | ess)")
+    if mode == "fixed":
+        return
+    rho = float(getattr(mppi_cfg, "ess_target", 0.01))
+    if not (math.isfinite(rho) and 0.0 < rho <= 1.0):
+        raise ValueError(f"ess_target = {rho} must be finite and in (0, 1]")
+    p.lambda_ess, p.ess_target = 1, rho
+
+
+def ess_grid(lambda0: float):
+    """(65,) float32 grid temperatures lambda_j = lambda0 2^((j - 32)/4) and (65,) float32 1/lambda_j, each computed in float64 from the
+    float32 lambda0 of the parameter block and rounded once: the first 130 floats of the temperature state."""
+    lam0 = float(np.float32(lambda0))
+    lam = lam0 * 2.0 ** ((np.arange(ESS_GRID, dtype=np.float64) - 32.0) / 4.0)
+    return lam.astype(np.float32), (1.0 / lam).astype(np.float32)
+
+
 class Feature(NamedTuple):
     name: str                                     # how the messages name it
     on: Callable                                  # (params, mppi_cfg or None) -> bool; without a config the block alone decides
@@ -616,6 +645,7 @@ class Feature(NamedTuple):
 
 CEM, SMOOTH, HALTON, COLORED = "mppi_mode: cem", "mppi_mode: smooth", "sampling_method: halton", "sampling_method: colored"
 WORLDS, MODES, ANNEALED, KNOTS, CONSTRAINED = "n_worlds > 1", "n_modes > 1", "annealed MPPI", "control_knots > 0", "constraint_mode: feasible_first"
+ESS = "lambda_mode: ess"
 FEATURES = (
     Feature(CEM, lambda p, c: p.mode == MODE_CEM, (256, 512, "T"), setter="set_distribution"),
     Feature(SMOOTH, lambda p, c: p.mode == MODE_SMOOTH, (256, 512, "T"),
@@ -632,6 +662,7 @@ FEATURES = (
     Feature(KNOTS, lambda p, c: p.control_knots > 0, (256, 512, "control_knots"),
             "the prior row is an action sequence and cannot be written as knots", "set_spline"),
     Feature(CONSTRAINED, lambda p, c: bool(p.constraint_mode), setter="set_constraint"),
+    Feature(ESS, lambda p, c: bool(p.lambda_ess), setter="set_temperature"),
 )
 _CEM_SMOOTH, _ADAPTIVE = (CEM, SMOOTH), ("update_cov", "update_lambda")
 # (features, what each of them excludes, the wording after its name); mode_refusal reports the first that applies.  csrc/api.cu: the same pairs
@@ -659,6 +690,17 @@ EXCLUSIONS = (
     ((KNOTS,), ("filter_u",), "excludes filter_u: the spline is smooth already, switch filter_u off"),
     ((CONSTRAINED,), (MODES,), "excludes n_modes > 1"),
     ((CONSTRAINED,), (KNOTS,), "excludes control_knots > 0"),
+    # the library names the excluded features in its own words (csrc/api.cu kFeatureNames); these texts repeat them, so both sides refuse a
+    # block with lambda_mode: ess with the same message
+    ((ESS,), ("update_lambda",), "excludes update_lambda (two rules for one temperature)"),
+    ((ESS,), ("cov_type: horizon",), "excludes cov_horizon (the shift computes lambda Sigma_H^-1 U before the temperature is known)"),
+    ((ESS,), (CEM,), "excludes mode cem (it does not weight the samples with the temperature)"),
+    ((ESS,), (SMOOTH,), "excludes mode smooth (it does not weight the samples with the temperature)"),
+    ((ESS,), (WORLDS,), "excludes n_worlds > 1"),
+    ((ESS,), (MODES,), "excludes n_modes > 1"),
+    ((ESS,), (KNOTS,), "excludes control_knots > 0"),
+    ((ESS,), (CONSTRAINED,), "excludes constraint_mode"),
+    ((ESS,), (ANNEALED,), "excludes annealed MPPI"),
 )
 
 
@@ -757,6 +799,7 @@ def make_params(mppi_cfg, sim_cfg, nu: int, K_local: int, obs_items: Sequence[tu
     _anneal_params(p, mppi_cfg)
     _spline_params(p, mppi_cfg)
     _constraint_params(p, mppi_cfg)
+    _ess_params(p, mppi_cfg)
     why = mode_refusal(p, nu, mppi_cfg)
     if why:
         raise ValueError(why)

@@ -27,8 +27,8 @@ import os
 import torch
 
 from ..backend import shard_row_floats
-from ..model.blob import (ANNEAL_MIN_SCALE, MODE_SIMPLE, MODE_SMOOTH, FEATURES, anneal_config, anneal_on, anneal_schedule, constraint_on,
-                          spline_basis, spline_initial_knots, spline_table)
+from ..model.blob import (ANNEAL_MIN_SCALE, ESS_GRID, ESS_ROW_FLOATS, ESS_STATE_FLOATS, MODE_SIMPLE, MODE_SMOOTH, FEATURES, anneal_config,
+                          anneal_on, anneal_schedule, constraint_on, ess_grid, ess_on, spline_basis, spline_initial_knots, spline_table)
 
 
 class _NoRange:
@@ -207,6 +207,10 @@ class MPPIPlanner:
         self.update_cov = bool(getattr(cfg, "update_cov", False))
         self.update_lambda = bool(getattr(cfg, "update_lambda", False))
         self.adaptive = self.update_cov or self.update_lambda
+        # ESS-targeted temperature (DESIGN.md section 2, "ESS-targeted temperature"): every plan chooses lambda on the device so that the
+        # Kish ESS of its weights is ess_target of the valid samples; it lives in dist[0] like the adaptive one, so the distribution is
+        # registered even with both adaptive flags off; make_params checks the keys against the modes
+        self.ess = ess_on(cfg)
         # cov_type chooses the update rule of update_cov: "diag" adapts diag(Sigma), "full" the whole Sigma with its Cholesky factor
         # and inverse (DESIGN.md section 2); make_params rejects other values, full without update_cov and a Sigma that is not SPD
         self.cov_full = self.update_cov and str(getattr(cfg, "cov_type", "diag")) == "full"
@@ -361,9 +365,9 @@ class MPPIPlanner:
             # the mode state (active mode, F[M], U_exec[T][nu]): mode 0 executed, no free energy yet, U_exec = mode 0
             self.mode_state = torch.cat([torch.zeros(1), torch.full((M,), float("inf")), U0.detach().cpu().reshape(-1)]).to(**f32)
             self.backend.set_distribution(self.mode_state)
-        elif not self.adaptive and hasattr(self.backend, "set_distribution"):
+        elif not (self.adaptive or self.ess) and hasattr(self.backend, "set_distribution"):
             self.backend.set_distribution(None)          # a planner rebuilt with the flags off must not inherit the previous one's buffer
-        if self.adaptive:
+        if self.adaptive or self.ess:
             sigma = torch.as_tensor(self.cfg.noise_sigma, dtype=torch.float64).reshape(nu, nu)
             if self.cov_horizon:
                 sigma = torch.kron(torch.eye(T, dtype=torch.float64), sigma)       # Sigma_H = I_T (x) Sigma
@@ -374,6 +378,20 @@ class MPPIPlanner:
                 parts = [torch.diagonal(sigma)]
             self.dist = torch.cat([torch.tensor([self.lambda_], dtype=torch.float64), *parts]).to(**f32)
             self.backend.set_distribution(self.dist)
+        # ESS-targeted temperature: the state (lambda_j, 1/lambda_j, n_valid, lambda, ESS_j) with the grid around lambda_, and the shard rows
+        self.temp_state, self.temp_row, self.temp_rows = None, None, None
+        if self.ess:
+            lam, inv = ess_grid(self.backend.params.lambda_)
+            state = torch.zeros((ESS_STATE_FLOATS,), dtype=torch.float32)
+            state[:ESS_GRID] = torch.from_numpy(lam)
+            state[ESS_GRID:2 * ESS_GRID] = torch.from_numpy(inv)
+            state[2 * ESS_GRID + 1] = float(self.dist[0])
+            self.temp_state = state.to(dev)
+            self.temp_row = torch.zeros((ESS_ROW_FLOATS,), **f32)
+            self.temp_rows = torch.zeros((self.world, ESS_ROW_FLOATS), **f32)
+            self.backend.set_temperature(self.temp_state)
+        elif hasattr(self.backend, "set_temperature"):
+            self.backend.set_temperature(None)
         # Smooth MPPI: the state (a_prev[nu], A[T][nu]) starts at a_prev = clamp(0, u_min, u_max), A = a_prev at every step
         self.smooth_state = None
         if self.smooth:
@@ -544,8 +562,25 @@ class MPPIPlanner:
 
     @property
     def current_lambda(self):
-        """0-d device view of the live temperature of adaptive MPPI (None without update_cov / update_lambda, and with mppi_mode cem)."""
+        """0-d device view of the live temperature of adaptive MPPI, or the one the last plan chose with lambda_mode ess (None without
+        update_cov / update_lambda / lambda_mode ess, and with mppi_mode cem)."""
         return None if self.dist is None or self.cem else self.dist[0]
+
+    @property
+    def ess_curve(self):
+        """(65,) device view of the Kish ESS of the last plan's weights at each grid temperature, over every rank (None unless lambda_mode
+        ess; zeros when no sample was valid)."""
+        return None if self.temp_state is None else self.temp_state[2 * ESS_GRID + 2:]
+
+    @property
+    def ess_grid(self):
+        """(65,) device view of the grid temperatures lambda_j = lambda_ 2^((j - 32)/4) (None unless lambda_mode ess)."""
+        return None if self.temp_state is None else self.temp_state[:ESS_GRID]
+
+    @property
+    def valid_samples(self):
+        """The number of valid samples of the last plan over every rank (an int, read from the device; None unless lambda_mode ess)."""
+        return None if self.temp_state is None else int(self.temp_state[2 * ESS_GRID:2 * ESS_GRID + 1].view(torch.int32).item())
 
     @property
     def elites(self):
@@ -619,6 +654,20 @@ class MPPIPlanner:
             torch.distributed.all_gather(rows, self.partial, group=self.pg)
         return self.partials, self.world
 
+    def _temperature(self, cost, x):
+        """lambda_mode ess: choose this plan's temperature into dist[0] before K3 -- in the pass itself with one rank or the peer window,
+        after an all-gather of the shard rows otherwise."""
+        be = self.backend
+        if self.world == 1 or self._peer_exchange:
+            be.temperature(cost, x, self.U, self.temp_row, solve=True)
+            return
+        be.temperature(cost, x, self.U, self.temp_row, solve=False)
+        if torch.distributed.get_backend(self.pg) == "nccl":
+            torch.distributed.all_gather_into_tensor(self.temp_rows.view(-1), self.temp_row, group=self.pg)
+        else:
+            torch.distributed.all_gather([self.temp_rows[g] for g in range(self.world)], self.temp_row, group=self.pg)
+        be.temperature_solve(self.temp_rows, self.world)
+
     def _weighted(self):
         """The samples K3 weights: the knot samples with control_knots > 0, else noise (SIMPLE, smooth) or actions (MEAN)."""
         if self.xk is not None:
@@ -643,6 +692,9 @@ class MPPIPlanner:
             if self.viol is not None:
                 self.viol.copy_(self._running_constraint(None).reshape(self.T, self.K))
         x = self._weighted()
+        if self.ess:
+            with _nvtx("mppi/temperature"):
+                self._temperature(cost, x)
         with _nvtx("mppi/K3 reduce + exchange + K4 update"):
             if self.world == 1 and hasattr(be, "reduce_finalize"):
                 be.reduce_finalize(cost, x, self.U, self.partial, self._action, self.stats)      # K3 + K4 in one launch
@@ -679,6 +731,8 @@ class MPPIPlanner:
             row = self.K_total - 2 - self.k_offset
             self.noise[:, :, row] = self.actions[:, :, row] - self.U
         x = self._weighted()
+        if self.ess:
+            self._temperature(self.cost, x)
         be.reduce(self.cost, x, self.U, self.partial)
         partials, G = self._exchange()
         be.finalize(partials, G, self.U, self._action, self.stats)

@@ -57,6 +57,8 @@ class MPPIConfig:
     constraint_mode: str = "none"        # constrained MPPI (DESIGN.md section 2): "none" or "feasible_first" (needs Objective.compute_constraint)
     constraint_tol: float = 0.0          # constrained MPPI: a sample is feasible when its summed violation is <= tol (finite, >= 0)
     constraint_lambda: Optional[float] = None   # constrained MPPI: temperature of the fallback over violations when no sample is feasible; None: lambda_
+    lambda_mode: str = "fixed"           # ESS-targeted temperature (DESIGN.md section 2): "fixed" (lambda_) or "ess" (chosen on the device every plan)
+    ess_target: float = 0.01             # lambda_mode ess: rho in (0, 1], the share of the valid samples the weights keep (Kish ESS = rho N)
     u_min: Optional[List[float]] = None
     u_max: Optional[List[float]] = None
     u_init: float = 0.0

@@ -3,7 +3,8 @@
 library), K2 (lanes-per-rollout chain kernel, team kernel on contact scenes of small and large robots, thread-per-rollout chain / tree /
 contact kernels), fused cost, K3 (warp-specialised
 ring, ragged last tile), K4, shift, the cov_type horizon kernels (horizon-colour K1, SYRK, its fused K4), the colored K1, the mppi_mode cem kernels (CEM K1, elite kernel with its last-CTA merge, CEM K4 and shift), the mppi_mode smooth kernels (smooth K1,
-K3 with the smoothness cost and the fused smooth K4), the risk-aware K1 / K2 / K3 (n_worlds), and whole plans (eager and CUDA-graph replay).  Sizes are
+K3 with the smoothness cost and the fused smooth K4), the risk-aware K1 / K2 / K3 (n_worlds), the temperature pass of lambda_mode ess (with its
+fused solve, or the split solve after an all-gather), and whole plans (eager and CUDA-graph replay).  Sizes are
 small: the sanitizer serialises the GPU.  With WORLD_SIZE > 1 (torchrun) the plans also run the peer-memory exchange."""
 import os
 import sys
@@ -52,6 +53,12 @@ CASES = [
                                  smooth_weight=0.5, du_min=[-1.0], du_max=[1.0]), PandaReachObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]),
     ("heijn push, n_worlds 8 (K1 keyed by the control sample, team K2 keyed by the world, RISK K3 with the fused K4)",
      lambda: push_cfg(K=256 * world, T=10, device=dev, n_worlds=8, cvar_alpha=0.25), PushObjective, [0.0, 0.0, 0.0]),
+    ("panda reach, lambda_mode ess (temperature pass: ragged last 256-sample tile, fused solve; RULE_DIST K3 / K4 with both flags off)",
+     lambda: panda_cfg(K=4100 * world, T=30, device=dev, sampling_method="random", lambda_mode="ess", ess_target=0.05), PandaReachObjective,
+     [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0]),
+    ("point robot, lambda_mode ess with cov_type full, MEAN mode (temperature pass without the noise rows)",
+     lambda: point_cfg(K=300 * world, T=12, device=dev, mppi_mode="halton-spline", update_cov=True, cov_type="full", lambda_mode="ess"),
+     PointReachObjective, [0.1, 0.0, 0.0]),
     ("panda pick (team K2: contacts, 16-lane articulation in 2 passes, compact layout)", lambda: pick_cfg(K=64 * world, T=9, device=dev), PandaPickObjective, [0.0, -0.94, 0.0, -2.8, 0.0, 1.8675, 0.0, 0.02, 0.02]),
 ]
 for name, mk, obj, q in CASES:
