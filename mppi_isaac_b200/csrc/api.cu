@@ -128,6 +128,9 @@ static int validate(const MppibModel* m, const MppibParams* p) {
     if (p->constraint_mode) {
         MPPIB_REQUIRE(isfinite(p->constraint_tol) && p->constraint_tol >= 0.f, "constraint_tol = %g must be finite and >= 0", p->constraint_tol);
         MPPIB_REQUIRE(isfinite(p->constraint_lambda) && p->constraint_lambda > 0.f, "constraint_lambda = %g must be finite and > 0", p->constraint_lambda);
+        // a tile carries T violation rows beside the cost rows: (T*nu + 2T) * 32 floats per ring stage, and K3 needs two stages
+        MPPIB_REQUIRE(reduce_ws_stages(*p, m->nu, RULE_FEASIBLE) >= 2, "constraint_mode needs two ring stages of (T*nu + 2T) * 32 floats in "
+                      "K3's shared memory; T = %d, nu = %d leaves room for fewer", p->T, m->nu);
     }
     MPPIB_REQUIRE(p->lambda_ess == 0 || p->lambda_ess == 1, "lambda_ess = %d must be 0 or 1", p->lambda_ess);
     if (p->lambda_ess)

@@ -341,6 +341,8 @@ int launch_cem_shift(MppibContext* c, float* U, uint32_t* plan_ctr, cudaStream_t
 int launch_temperature(MppibContext* c, const float* cost, const float* x, const float* U, float* row, bool solve, cudaStream_t s);
 int launch_temperature_solve(MppibContext* c, const float* rows, int G, cudaStream_t s);
 int alloc_horizon(MppibContext* c);           // (re)sizes the hz_* buffers for the handle's K and T*nu (frees them without cov_horizon)
+// K3's ring depth for the shard row of `row` (reduce.cu): a launch needs two stages at least, and validate refuses constraint_mode with fewer
+int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth = false);
 long long rollout_smem_bytes(const MppibModel& m);
 // K2, lanes-per-rollout mapping for serial chains without contacts (rollout_lanes.cu)
 bool rollout_lanes_eligible(const MppibModel& m);

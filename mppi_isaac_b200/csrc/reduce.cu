@@ -1372,16 +1372,6 @@ int make_map(CUtensorMap* tm, const float* base, int rows, int K, int box_rows, 
     return 0;
 }
 
-// The ring depth: the deepest ring (<= 8 stages) that fits next to seven warp partials of the rule's row, the depths every shape was
-// tuned at.  Where that leaves fewer than two stages (the second-moment row at T = 256, T*nu = 512), two stages fit next to their two
-// consumers'.
-static int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth = false) {
-    int ns = 8;
-    while (ns > 1 && WsLayout(p.T, ctrl_rows(p), nu, ns, row, p.update_cov, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
-    if (ns < 2 && WsLayout(p.T, ctrl_rows(p), nu, 2, row, p.update_cov, smooth).bytes <= 224 * 1024) ns = 2;
-    return ns;
-}
-
 // smooth, anneal: the state of mode smooth and the annealing schedule, for the rules that read them (nullptr otherwise)
 template <int RPL, Rule R, bool RISK>
 int launch_reduce_ws_t(MppibContext* c, const float* cost, const float* x, const float* U, float* partial, float* fin_U, float* fin_action,
@@ -1484,6 +1474,16 @@ int launch_syrk(MppibContext* c, const float* x, const float* U, float* partial,
 }
 
 }  // namespace
+
+// The ring depth: the deepest ring (<= 8 stages) that fits next to seven warp partials of the rule's row, the depths every shape was
+// tuned at.  Where that leaves fewer than two stages (the second-moment row at T = 256, T*nu = 512), two stages fit next to their two
+// consumers'.
+int reduce_ws_stages(const MppibParams& p, int nu, Rule row, bool smooth) {
+    int ns = 8;
+    while (ns > 1 && WsLayout(p.T, ctrl_rows(p), nu, ns, row, p.update_cov, smooth, WS_NCONS).bytes > 224 * 1024) --ns;
+    if (ns < 2 && WsLayout(p.T, ctrl_rows(p), nu, 2, row, p.update_cov, smooth).bytes <= 224 * 1024) ns = 2;
+    return ns;
+}
 
 int alloc_horizon(MppibContext* c) {
     const bool on = c->params.update_cov && c->params.cov_horizon;

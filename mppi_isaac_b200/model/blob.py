@@ -665,6 +665,17 @@ FEATURES = (
     Feature(ESS, lambda p, c: bool(p.lambda_ess), setter="set_temperature"),
 )
 _CEM_SMOOTH, _ADAPTIVE = (CEM, SMOOTH), ("update_cov", "update_lambda")
+K3_SMEM = 224 * 1024                              # the shared memory K3 sizes its ring in (reduce_ws_stages, csrc/reduce.cu)
+
+
+def feasible_k3_bytes(T: int, nu: int) -> int:
+    """Shared memory of constraint_mode's K3 at its smallest ring, two stages next to two warp partials (``WsLayout`` of RULE_FEASIBLE in
+    csrc/reduce.cu): a stage holds T*nu control, T cost and T violation rows of 32 samples; the shard row is 4 + T*nu floats.  The
+    library refuses the mode where this exceeds K3_SMEM (validate, csrc/api.cu), so a horizon too long for the ring is refused here too."""
+    NR = T * nu
+    P4 = (4 + NR + 3) & ~3
+    floats = max(2 * (NR + 2 * T) * 32, 512 + 4 * P4) + ((NR + 3) & ~3) + ((T + 3) & ~3) + 8 * 32 + 2 * P4 + 8
+    return ((floats * 4 + 15) & ~15) + 2 * 8 * 2 + 128
 # (features, what each of them excludes, the wording after its name); mode_refusal reports the first that applies.  csrc/api.cu: the same pairs
 EXCLUSIONS = (
     ((COLORED,), ("cov_type: horizon",), "excludes cov_type: horizon, whose Sigma_H already models the time correlation"),
@@ -715,6 +726,9 @@ def mode_refusal(p: MppibParams, nu: int, mppi_cfg=None, anneal: bool = False) -
             if p.T > (t_max or p.T) or n > n_max:
                 need = (f"horizon <= {t_max} and " if t_max else "") + ("horizon" if rows == "T" else rows) + f" * nu <= {n_max}"
                 return f"{f.name} needs {need}; T = {p.T}, {rows}*nu = {n}"
+    if any(f.name == CONSTRAINED for f in on) and feasible_k3_bytes(p.T, nu) > K3_SMEM:
+        return (f"{CONSTRAINED} needs two K3 ring stages of (horizon * nu + 2 * horizon) * 32 floats, with their working set, in shared memory "
+                f"<= {K3_SMEM} bytes; T = {p.T}, T*nu = {p.T * nu} needs {feasible_k3_bytes(p.T, nu)}")
     names = {f.name for f in on}
     for subjects, group, text in EXCLUSIONS:
         for name in subjects:

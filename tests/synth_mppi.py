@@ -41,8 +41,12 @@ WS_W, WS_NCONS, MAX_GRID, SMEM_CAP = 32, 7, 512, 224 * 1024
 SMEM_OPTIN, MAX_NU = 227 * 1024, 16    # the H100's opt-in shared memory per CTA; MPPIB_MAX_NU
 
 
-def row_floats(T, nu, kind):
-    NR = T * nu
+def row_floats(T, nu, kind, Tc=None, feasible=False):
+    """Floats of the shard row (``shard_row_floats``): Tc control rows (default T; knots: P); `feasible`: the FEASIBLE row
+    (beta, eta, W[Tc*nu], n_feasible, min V)."""
+    NR = (T if Tc is None else Tc) * nu
+    if feasible:
+        return 4 + NR
     return 2 + NR + (NR if kind == "M2" else nu * (nu + 1) // 2 if kind == "C" else NR * (NR + 1) // 2 if kind == "H" else 0)
 
 
@@ -52,12 +56,13 @@ def modes_fin_floats(NR, M, G):
     return 3 * M * NR + MAX_NU * MAX_NU + M * G + 4 * M + 2 * M * M + 4
 
 
-def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False, modes=1):
+def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False, modes=1, Tc=None, feasible=False):
     """Bytes of ``WsLayout``: nparts warp partials (default one per consumer, min(nstage, 7)); smooth adds the [NR4] U region; with
-    modes = M > 1 the ring region holds at least modes_fin_floats(NR, M, 1), where the fused K4 runs ``modes_rows``."""
-    NR = T * nu
-    P4 = (row_floats(T, nu, kind) + 3) & ~3
-    ring, fold = nstage * (NR + T) * WS_W, MAX_GRID + 4 * P4
+    modes = M > 1 the ring region holds at least modes_fin_floats(NR, M, 1), where the fused K4 runs ``modes_rows``.  A tile holds
+    NR = Tc*nu control rows and T cost rows, and with `feasible` T violation rows more."""
+    NR = (T if Tc is None else Tc) * nu
+    P4 = (row_floats(T, nu, kind, Tc, feasible) + 3) & ~3
+    ring, fold = nstage * (NR + (2 * T if feasible else T)) * WS_W, MAX_GRID + 4 * P4
     g = max(ring, fold)
     if kind == "C":
         g = max(g, NR + 1 + 2 * NR + nu * (nu + 1) // 2 + 3 * nu * nu)
@@ -71,31 +76,34 @@ def _ws_bytes(T, nu, nstage, kind, nparts=None, smooth=False, modes=1):
     return bar + 2 * 8 * nstage + 128
 
 
-def ws_stages(T, nu, kind, smooth=False):
+def ws_stages(T, nu, kind, smooth=False, Tc=None, feasible=False):
     """The ring depth rule of ``reduce_ws_stages``: the deepest ring next to seven warp partials, else two stages next to two."""
     ns = 8
-    while ns > 1 and _ws_bytes(T, nu, ns, kind, WS_NCONS, smooth) > SMEM_CAP:
+    while ns > 1 and _ws_bytes(T, nu, ns, kind, WS_NCONS, smooth, Tc=Tc, feasible=feasible) > SMEM_CAP:
         ns -= 1
-    if ns < 2 and _ws_bytes(T, nu, 2, kind, None, smooth) <= SMEM_CAP:
+    if ns < 2 and _ws_bytes(T, nu, 2, kind, None, smooth, Tc=Tc, feasible=feasible) <= SMEM_CAP:
         ns = 2
     return ns
 
 
-def ws_layout(T, nu, kind, smooth=False, modes=1):
+def ws_layout(T, nu, kind, smooth=False, modes=1, Tc=None, feasible=False):
     """(rows of W per lane, consumer warps, ring stages, rows per x TMA box) of the K3 launch, or None if the shape is refused.
     `smooth`: the layout of mode smooth (row W, plus the U region of the smoothness cost).  `modes` = M > 1: the MODES launch (row W
-    per mode): the ring depth is chosen without the modes_rows floor, and the launch, floor included, must fit the opt-in limit."""
-    NR = T * nu
+    per mode): the ring depth is chosen without the modes_rows floor, and the launch, floor included, must fit the opt-in limit.
+    `Tc`: the control rows (knots: P; default T).  `feasible`: the FEASIBLE launch of constraint_mode (row W, T violation rows more
+    per tile, the row 4 + T*nu)."""
+    Tc = T if Tc is None else Tc
+    NR = Tc * nu
     if kind == "H":
         if NR > HZ_MAX_N:
             return None
         kind = "M2"                    # the host sizes the horizon K3 (row W only) with the update_cov rule's M2 layout
-    if NR > 512 or T > 256 or ws_stages(T, nu, "W") < 2 or ws_stages(T, nu, kind, smooth) < 2:
+    if NR > 512 or T > 256 or ws_stages(T, nu, "W", Tc=Tc) < 2 or ws_stages(T, nu, kind, smooth, Tc, feasible) < 2:
         return None
-    ns = ws_stages(T, nu, kind, smooth)
+    ns = ws_stages(T, nu, kind, smooth, Tc, feasible)
     ncons = min(ns, WS_NCONS)
     nstage = ncons * (ns // ncons)
-    if modes > 1 and _ws_bytes(T, nu, nstage, kind, None, smooth, modes) > SMEM_OPTIN:
+    if modes > 1 and _ws_bytes(T, nu, nstage, kind, None, smooth, modes, Tc, feasible) > SMEM_OPTIN:
         return None
     xbox = min(NR, 256)
     while NR % xbox:
@@ -121,9 +129,9 @@ def modes_grid(K, k_offset, Kc, M, sms=NUM_SMS):
     return max(1, min(tmax, sms // M))
 
 
-def wrap_K(T, nu, kind, sms=NUM_SMS, smooth=False):
+def wrap_K(T, nu, kind, sms=NUM_SMS, smooth=False, Tc=None, feasible=False):
     """A ragged K (multiple of 4) whose every CTA streams more than three full rings of tiles."""
-    _, _, nstage, _ = ws_layout(T, nu, kind, smooth)
+    _, _, nstage, _ = ws_layout(T, nu, kind, smooth, Tc=Tc, feasible=feasible)
     return WS_W * sms * (3 * nstage + 1) - 12
 
 
@@ -207,6 +215,11 @@ class Case:
     def n(self):
         return self.T * self.nu
 
+    @property
+    def Tc(self):
+        """The control rows of x and U: the knots P with control_knots > 0, else T."""
+        return int(self.params.control_knots) or self.T
+
     def chol(self):
         """The float32 lower factor K1 colours with (n x n for H)."""
         nu, n = self.nu, self.n
@@ -287,17 +300,17 @@ def k3_id(T, nu, K, kind, tag):
 
 
 def k3_inputs(case, seed=0, spread=4.0, favour_tail=True):
-    """cost [T][K], x [T][nu][K] and U [T][nu] (float32) of a K3 case.
+    """cost [T][K], x [Tc][nu][K] and U [Tc][nu] (float32) of a K3 case (Tc: the control rows, ``Case.Tc``).
 
     S_k spans about `spread` * lambda over the samples and sum_t |gamma^t c_tk| stays a few lambda, so the float32 error of S
     stays far below lambda (the gate then tests the weights, not only the argmin).  With `favour_tail` the samples of the last
     (ragged) tile get S lower by 2 lambda: they carry a share of the weight that a kernel dropping them cannot hide.
     For H the noise is coloured by L_H over the whole horizon, and the last step of U is u_init = 0: U is what mppib_shift leaves
     (``shifted_from``), which is where the device computes the SIMPLE-mode g = lambda Sigma_H^-1 U."""
-    T, nu, K, lam = case.T, case.nu, case.K, case.lam
+    T, Tc, nu, K, lam = case.T, case.Tc, case.nu, case.K, case.lam
     rng = np.random.default_rng(seed)
     L = case.chol().astype(np.float64)
-    NR = T * nu
+    NR = Tc * nu
     if case.kind == "H":
         if case.simple:
             U = (L @ rng.normal(0, 0.5 / math.sqrt(NR), NR)).reshape(T, nu)
@@ -305,14 +318,14 @@ def k3_inputs(case, seed=0, spread=4.0, favour_tail=True):
             U = rng.normal(0, 0.1, (T, nu))
         U[-1] = 0.0
     elif case.simple:
-        U = np.einsum("ij,tj->ti", L, rng.normal(0, 0.5 / math.sqrt(NR), (T, nu)))      # |L^-1 U| ~ 0.5: g.x ~ lambda / 2
+        U = np.einsum("ij,tj->ti", L, rng.normal(0, 0.5 / math.sqrt(NR), (Tc, nu)))     # |L^-1 U| ~ 0.5: g.x ~ lambda / 2
     else:
-        U = rng.normal(0, 0.1, (T, nu))
+        U = rng.normal(0, 0.1, (Tc, nu))
     U = U.astype(np.float32)
     if case.kind == "H":
         noise = (L @ rng.standard_normal((NR, K))).reshape(T, nu, K).astype(np.float32)
     else:
-        noise = np.einsum("ij,tjk->tik", L, rng.standard_normal((T, nu, K))).astype(np.float32)
+        noise = np.einsum("ij,tjk->tik", L, rng.standard_normal((Tc, nu, K))).astype(np.float32)
     x = noise if case.simple else (U[:, :, None] + noise).astype(np.float32)
     g = 1.0 if case.simple else float(case.params.gamma)
     Gam = sum(abs(g) ** t for t in range(T)) if g != 0 else 1.0
@@ -339,10 +352,10 @@ def _gammas(case):
 
 def k3_restate(case, cost, x, U, keep=None):
     """float64 K3 of the case: S[K], w[K] and the shard row of its kind.  `keep`: mask of the samples that take part."""
-    T, nu, K, lam = case.T, case.nu, case.K, case.lam
+    T, Tc, nu, K, lam = case.T, case.Tc, case.nu, case.K, case.lam
     c64 = np.asarray(cost, np.float64).reshape(T, K)
-    x64 = np.asarray(x, np.float64).reshape(T * nu, K)
-    U64 = np.asarray(U, np.float64).reshape(T, nu)
+    x64 = np.asarray(x, np.float64).reshape(Tc * nu, K)
+    U64 = np.asarray(U, np.float64).reshape(Tc, nu)
     with np.errstate(invalid="ignore"):
         S = (_gammas(case)[:, None] * c64).sum(0)
     if case.simple:
@@ -381,10 +394,10 @@ def hz_C(case, x, U, w, k0=0, k1=None):
 
 def k3_S32(case, cost, x, U):
     """float32 restatement of phase A of the kernel: gamma^t = exp2(log2(gamma) t) (1 at t = 0), g = lambda Sigma^-1 U, and S_k as
-    four interleaved accumulation chains, (a0 + a1) + (a2 + a3)."""
+    four interleaved accumulation chains, (a0 + a1) + (a2 + a3), over the T cost terms and then the Tc*nu control terms."""
     f = np.float32
-    T, nu, K = case.T, case.nu, case.K
-    NR = T * nu
+    T, Tc, nu, K = case.T, case.Tc, case.nu, case.K
+    NR = Tc * nu
     gam = f(1.0) if case.simple else f(case.params.gamma)
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         lg = np.log2(gam)
@@ -402,9 +415,9 @@ def k3_S32(case, cost, x, U):
         terms += [(g[r], xr[r]) for r in range(NR)]
         terms += [(f(0), xr[NR - 1])] * (((NR + 3) & ~3) - NR)
     elif case.simple:
-        si, Uf = case.sinv().astype(f), np.asarray(U, f).reshape(T, nu)
+        si, Uf = case.sinv().astype(f), np.asarray(U, f).reshape(Tc, nu)
         g = np.zeros(NR, f)
-        for t in range(T):
+        for t in range(Tc):
             for i in range(nu):
                 acc = f(0)
                 for j in range(nu):
@@ -421,9 +434,9 @@ def k3_S32(case, cost, x, U):
 
 
 def k3_dS(case, cost, x, U):
-    """Per-sample bound on |S_kernel - S| (float32 kernel against the float64 restatement)."""
+    """Per-sample bound on |S_kernel - S| (float32 kernel against the float64 restatement): T cost terms, Tc*nu control terms."""
     T, nu, K, lam = case.T, case.nu, case.K, case.lam
-    NR = T * nu
+    NR = case.Tc * nu
     gam = 1.0 if case.simple else float(case.params.gamma)
     lg = abs(math.log2(gam)) if gam > 0 else 0.0
     gamma_t = np.abs(_gammas(case))
@@ -440,6 +453,14 @@ def k3_dS(case, cost, x, U):
     return EPS * dS
 
 
+def v_dS(g):
+    """Per-sample bound on the float32 error of V_k = sum_t max(g_tk, 0) summed in t order (constraint_mode's K3):
+    (T + 2) eps sum_t max(g_tk, 0)."""
+    g = np.asarray(g, np.float64)
+    with np.errstate(invalid="ignore"):
+        return (g.shape[0] + 2) * EPS * np.where(g > 0, g, 0.0).sum(0)
+
+
 def k3_gate(case, cost, x, U, S, w, sms=NUM_SMS):
     """Element-wise bound on |row_kernel - row_reference| for the case's row kind (S, w: of ``k3_restate``; sms: of the device).
 
@@ -447,8 +468,8 @@ def k3_gate(case, cost, x, U, S, w, sms=NUM_SMS):
     spread of S and beta (w_hi - w) plus a few roundings; each entry is then a sample-ordered FFMA sum over a chunk of kchunk
     samples and a fold of ksplit chunk sums:  |dC_ij| <= sum_k |dx_ik| |dx_jk| (dw_k + (kchunk + ksplit + 4) eps w_k)."""
     T, nu, K, lam = case.T, case.nu, case.K, case.lam
-    NR = T * nu
-    _, ncons, _, _ = ws_layout(T, nu, case.kind)
+    NR = case.Tc * nu
+    _, ncons, _, _ = ws_layout(T, nu, case.kind, Tc=case.Tc)
     ntiles = (K + WS_W - 1) // WS_W
     grid = min(ntiles, sms)
     per_cta = -(-ntiles // grid)

@@ -279,11 +279,20 @@ def test_library_refusals():
     be.destroy()
 
 
-def test_a_horizon_without_room_for_two_ring_stages_is_refused():
-    """T = 256, nu = 2: a tile of (T*nu + 2T)*32 floats leaves room for one ring stage only, so the library refuses the launch."""
+def test_a_horizon_without_room_for_two_ring_stages_is_refused_at_create():
+    """T = 256, nu = 2: a tile of (T*nu + 2T)*32 floats leaves room for one ring stage only, so make_params and mppib_create refuse the
+    block before any plan; a handle created without the mode cannot take it on through mppib_set_params either."""
+    from mppi_isaac_b200.backend import CudaBackend
     nu, T, K = 2, 256, 1028
-    cost, x, U, g = inputs(nu, T, K, "simple", "all", 5)
-    be, _ = backend(nu, params(nu, T, K), dev(g))
-    with pytest.raises(RuntimeError, match="fewer than two ring stages"):
-        be.reduce(dev(cost), dev(x), dev(U), torch.zeros(4 + T * nu, device=DEV))
+    with pytest.raises(ValueError, match="ring stages"):
+        params(nu, T, K)
+    p = params(nu, T, K, on=False)
+    p.constraint_mode, p.constraint_tol, p.constraint_lambda = 1, 0.05, 0.2
+    be = CudaBackend(DEV)
+    with pytest.raises(RuntimeError, match="ring stages"):
+        be.create(nu_model(nu), p)
+    ok = params(nu, 216, K)                                                   # T = 216 fits two stages
+    be.create(nu_model(nu), ok)
+    with pytest.raises(RuntimeError, match="ring stages"):
+        be.set_params(p)
     be.destroy()

@@ -164,6 +164,10 @@ LIMITS = {
     ('knots', 64, 16, 33): True,
     ('knots', 256, 1, 4): False,
     ('knots', 257, 1, 4): True,
+    # constraint_mode: two ring stages of (T*nu + 2T) * 32 floats fit up to T = 216 at nu = 2 (the library refused T = 217 at the first
+    # plan before make_params and mppib_create refused it too)
+    ('constraint', 216, 2, None): False,
+    ('constraint', 217, 2, None): True,
 }
 LIMIT_FIXED = {("n_modes", 65, 8, None)}
 
@@ -271,6 +275,7 @@ def block_cases():
     for name in ("cem", "smooth", "control_knots"):                               # T = 256 | 257
         cases += [((name,), dict(T=256, nu=1)), ((name,), dict(T=257, nu=1))]
     cases += [(("control_knots",), dict(T=64, nu=16, control_knots=32)), (("control_knots",), dict(T=64, nu=16, control_knots=33))]
+    cases += [(("constraint_mode",), dict(T=216, nu=2)), (("constraint_mode",), dict(T=217, nu=2))]    # two FEASIBLE ring stages | one
     return cases
 
 
@@ -284,6 +289,26 @@ def test_the_table_and_the_library_refuse_the_same_blocks(names, shape):
     rc = create(lib, p, nu)
     assert rc in (-1, 0, -2), lib.mppib_last_error().decode()
     assert (rc == -1) == (why is not None), (why, lib.mppib_last_error().decode())
+
+
+def test_constrained_horizons_are_refused_where_the_feasible_ring_holds_one_stage():
+    """Every (T, nu) with T <= 256 and T*nu <= 512 under constraint_mode: make_params, mppib_create (-1 refused, else admitted) and the
+    restatement of the FEASIBLE K3 layout (synth_mppi.ws_layout) refuse the same shapes, which are nu = 2 with 217 <= T <= 256."""
+    from synth_mppi import ws_layout
+    lib = library()
+    by_params, by_create, by_layout = set(), set(), set()
+    for nu in range(1, 17):
+        for T in range(1, min(256, 512 // nu) + 1):
+            if refusal(FEATURES["constraint"], T=T, nu=nu) is not None:
+                by_params.add((T, nu))
+            rc = create(lib, block(["constraint_mode"], T=T, nu=nu), nu)
+            assert rc in (-1, 0, -2), lib.mppib_last_error().decode()
+            if rc == -1:
+                by_create.add((T, nu))
+                assert "ring stages" in lib.mppib_last_error().decode()
+            if ws_layout(T, nu, "W", feasible=True) is None:
+                by_layout.add((T, nu))
+    assert by_params == by_create == by_layout == {(T, 2) for T in range(217, 257)}
 
 
 @pytest.mark.gpu
