@@ -565,7 +565,7 @@ int32_t mppib_sample_spline(MppibHandle h, uint64_t seed, uint64_t plan_idx, con
  *          samples by exp(-(S_k - b)/lambda) (S_k as today); one without weights its valid samples by exp(-(V_k - b)/lambda_c) (no
  *          control cost, no gamma^t).  The states (n_feasible, b, eta, W) merge lexicographically: one with n_feasible > 0 beats one
  *          with 0 (which then weighs 0), two of one kind merge by today's rescale with their temperature and add their counts
- *          (feas_scale in csrc/common.cuh, the same function at every fold).  The shard row is
+ *          (merge_scale in csrc/common.cuh, the same function at every fold).  The shard row is
  *   partial  [4 + T*nu]  (beta, eta, W[T*nu], n_feasible as int32 bits, min V over the shard's valid samples (+inf: none))
  *   K4     mppib_finalize (or the fused tail) merges the G rows the same way, then today's update, Savitzky-Golay, clamp, action, mirror;
  *          stats = (beta, eta) of the kind that won, cstate = (sum n_feasible, min V).  No valid sample anywhere: U unchanged.

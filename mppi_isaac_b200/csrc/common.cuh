@@ -197,15 +197,37 @@ int check_anneal(const MppibContext* c, const char* who);
 // the first pair of the exclusion table (api.cu) a block breaks, with a registered schedule counted when anneal is set; who: "" or the
 // entry point the message names
 int check_exclusions(const MppibParams& p, bool anneal, const char* who);
-// Constrained MPPI (include/mppib.h "Constrained MPPI"): the feasibility-first merge of two or more states (n_feasible, b, eta, W).  The
-// merged state has n_all = the sum of the counts and b_all = feas_min over the states; a state's eta and W enter it times feas_scale.
-// A state with a feasible sample beats one without, which then weighs 0; states of one kind merge by today's online-softmax rescale
-// with their temperature (lambda for the feasible kind, lambda_c for the violation kind).  One accumulator suffices: once any state
-// holds a feasible sample the violation kind can never win again, so its sums are dropped.  Empty states (b = +inf) weigh 0.
-__device__ __forceinline__ float feas_min(int nf, float b, int n_all, float b_acc) { return (nf > 0) == (n_all > 0) ? fminf(b_acc, b) : b_acc; }
-__device__ __forceinline__ float feas_scale(int nf, float b, int n_all, float b_all, float inv_lambda, float inv_lambda_c) {
-    if ((nf > 0) != (n_all > 0) || b == INFINITY) return 0.f;
+// The merge of two or more partial states (n_feasible, b, eta, W) that every fold of every rule uses: tile into warp, warps into the
+// CTA partial, CTA partials into the shard row, shard rows in K4.  The merged state has n_all = the sum of the counts and b_all =
+// merge_min over the states; a state's eta and W enter it times merge_scale.  Constrained MPPI (include/mppib.h "Constrained MPPI") is
+// the feasibility-first merge: a state with a feasible sample beats one without, which then weighs 0; states of one kind merge by the
+// online-softmax rescale with their temperature (lambda for the feasible kind, lambda_c for the violation kind).  One accumulator
+// suffices: once any state holds a feasible sample the violation kind can never win again, so its sums are dropped.  Every other rule
+// is the case with every count 0 and lambda in both temperature slots: b_all = min b, scale = exp(-(b - b_all)/lambda).  An empty
+// state weighs 0; each level tests for one itself (b = +inf in the kernel's folds, eta = 0 in K4) and does not call merge_scale on it.
+// merge_min(nf, b, n_all): the b one state brings into the minimum (+inf when the other kind wins); with b_acc: folded into b_acc
+__device__ __forceinline__ float merge_min(int nf, float b, int n_all) { return (nf > 0) == (n_all > 0) ? b : INFINITY; }
+__device__ __forceinline__ float merge_min(int nf, float b, int n_all, float b_acc) { return (nf > 0) == (n_all > 0) ? fminf(b_acc, b) : b_acc; }
+__device__ __forceinline__ float merge_scale(int nf, float b, int n_all, float b_all, float inv_lambda, float inv_lambda_c) {
+    if ((nf > 0) != (n_all > 0)) return 0.f;
     return expf(-(b - b_all) * (n_all > 0 ? inv_lambda : inv_lambda_c));
+}
+// The election of the CTA that folds a grid's partials: every CTA calls it once its partial is written, and it returns true in the one
+// CTA whose atomicAdd takes ticket value count - 1.  The fence before the ticket makes this CTA's partial visible to the others, the
+// one after it orders the winner's reads of theirs.  Resetting the ticket is the caller's.  A CTA may call it twice with one flag (the
+// SYRK): every thread has read the flag before the second call's first __syncthreads, and thread 0 writes it only after that barrier.
+// (A template so that the compiler emits the flag after the calling kernel's own shared arrays: placed before an 8-byte aligned one,
+// it would cost 4 bytes of padding.)
+template <int = 0>
+__device__ __forceinline__ bool last_cta(unsigned int* ticket, unsigned int count) {
+    __shared__ unsigned int s_last;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == count - 1u ? 1u : 0u;
+    __syncthreads();
+    if (!s_last) return false;
+    __threadfence();
+    return true;
 }
 // the per-step violation a margin g contributes: g where g > 0, 0 where g <= 0; NaN stays NaN, so the sample becomes invalid
 __device__ __forceinline__ float feas_violation(float g) { return g <= 0.f ? 0.f : g; }

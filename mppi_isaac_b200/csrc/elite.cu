@@ -133,7 +133,6 @@ mppib_elite_kernel(const __grid_constant__ MppibParams p, int nu, const float* _
     __shared__ unsigned long long keys[EL_BUF];
     __shared__ float gp[256];
     __shared__ float un[EL_MAX_NR];
-    __shared__ unsigned int s_last;
     const int K = p.K, T = p.T, NR = T * nu, E = p.n_elites, tid = threadIdx.x;
     const int P = shard_row_floats(RULE_CEM, T, nu, false, 0, E);
     {
@@ -158,12 +157,7 @@ mppib_elite_kernel(const __grid_constant__ MppibParams p, int nu, const float* _
     }
     unsigned long long* mine = reinterpret_cast<unsigned long long*>(scratch + (size_t)blockIdx.x * P);   // P is a multiple of 4
     for (int e = tid; e < E; e += EL_NT) mine[e] = keys[e];
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
+    if (!last_cta(ticket, gridDim.x)) return;
     // the last CTA: merge the per-CTA lists, as many as fit next to the running list per pass
     const int G = (int)gridDim.x, per = EL_NEW / E;
     for (int i = tid; i < EL_KEEP; i += EL_NT) keys[i] = KEY_NONE;

@@ -99,6 +99,27 @@ __constant__ float c_sg_edge[4][9] = {{763.f, 441.f, 189.f, 7.f, -105.f, -147.f,
                                       {441.f, 322.f, 220.5f, 136.5f, 70.f, 21.f, -10.5f, -24.5f, -21.f},
                                       {189.f, 220.5f, 232.f, 223.5f, 195.f, 146.5f, 78.f, -10.5f, -119.f},
                                       {7.f, 136.5f, 223.5f, 268.f, 270.f, 229.5f, 146.5f, 21.f, -147.f}};
+// Savitzky-Golay (window 9, order 2, 'interp' edges) of the [T][nu] sequence u at element r = t*nu + j: the window's products summed
+// in window order, then one scaling
+__device__ __forceinline__ float savgol(const float* u, int T, int nu, int r) {
+    const int t = r / nu, j = r % nu;
+    float s = 0.f;
+    if (t < 4) {
+#pragma unroll
+        for (int i = 0; i < 9; ++i) s += c_sg_edge[t][i] * u[i * nu + j];
+        s *= (1.0f / 1155.0f);
+    } else if (t >= T - 4) {
+        const int ee = T - 1 - t;
+#pragma unroll
+        for (int i = 0; i < 9; ++i) s += c_sg_edge[ee][i] * u[(T - 1 - i) * nu + j];
+        s *= (1.0f / 1155.0f);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 9; ++i) s += c_sg_mid[i] * u[(t - 4 + i) * nu + j];
+        s *= (1.0f / 231.0f);
+    }
+    return s;
+}
 
 // K4 of cov_horizon (dist = (lambda, Sigma_H, L_H, Sigma_H^-1), n = T*nu, after the U update, e = eta > 0), one CTA:
 //   1. Sigma' = shift((1 - s) Sigma_H + s V + kappa I),  V = C/eta - (m1 d^T + d m1^T - d d^T),  C = sum_g scale_g C_g:
@@ -194,8 +215,35 @@ __device__ __noinline__ void horizon_update(const MppibParams& p, int nu, const 
     }
 }
 
-// combine G rows (beta_g, eta_g, W_g) of stride P, update U (+ Savitzky-Golay, clamp), first action, statistics; one CTA of 256
-// threads, `un` = [T*nu + G] floats of shared memory (+ T*nu with update_cov).
+// K4's merge of G rows (beta_g, eta_g, W_g, ...) of stride P by merge_min / merge_scale (a row with eta_g = 0 is empty): the minimum
+// into b, the scale of every row into sg[G], and the return value eta = sum_g sg_g eta_g in g order.  The caller sums W (and what else
+// its rows carry) under the same scales.  FEAS: the rows carry (n_feasible bits, min V) after W[NR]; thread 0 writes cstate = (sum
+// n_feasible, min V) (nullable).  A CTA-wide call: sg is complete when it returns.
+template <bool FEAS>
+__device__ __forceinline__ float merge_rows(const MppibParams& p, int NR, const float* __restrict__ partials, int G, int P, float inv_lambda, float* sg,
+                                            float& b, float* __restrict__ cstate) {
+    auto nf_of = [&](int gidx) { return FEAS ? __float_as_int(__ldcg(&partials[(size_t)gidx * P + 2 + NR])) : 0; };
+    int n_all = 0;
+    if constexpr (FEAS) {
+        float vmin = INFINITY;
+        for (int gidx = 0; gidx < G; ++gidx) { n_all += nf_of(gidx); vmin = fminf(vmin, __ldcg(&partials[(size_t)gidx * P + 3 + NR])); }
+        if (threadIdx.x == 0 && cstate) { cstate[0] = __int_as_float(n_all); cstate[1] = vmin; }
+    }
+    const float inv_lc = FEAS ? 1.0f / p.constraint_lambda : inv_lambda;
+    b = INFINITY;
+    for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = merge_min(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b);
+    for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
+        const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
+        sg[gidx] = eg > 0.f ? merge_scale(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b, inv_lambda, inv_lc) : 0.f;
+    }
+    __syncthreads();
+    float e = 0.f;
+    for (int gidx = 0; gidx < G; ++gidx) e += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 1]);
+    return e;
+}
+
+// combine G rows (beta_g, eta_g, W_g) of stride P (merge_rows), update U (+ Savitzky-Golay, clamp), first action, statistics; one CTA of
+// 256 threads, `un` = [T*nu + G] floats of shared memory (+ T*nu with update_cov).
 // ADAPT (a distribution is registered): lambda comes from dist[0]; after the U update the CTA updates dist in place --
 //   update_cov:    the rows carry M2_g after W_g; m1 = W/eta - c, m2 = M2/eta, d = U_new - U_old (before Savitzky-Golay),
 //                  var = max(m2 - 2 d m1 + d^2, 0), cov_j <- (1 - s) cov_j + s mean_t var[t][j] + kappa
@@ -210,8 +258,8 @@ __device__ __noinline__ void horizon_update(const MppibParams& p, int nu, const 
 // Sigma^-1 as they were.  The diagonal equals the diagonal rule above without its clamp at 0.
 // HZN (update_cov with cov_horizon): the rows carry C_g[n(n+1)/2] over the whole sequence; m1 and d are kept as n-vectors and
 // horizon_update does the rest.
-// FEAS (constraint_mode): the rows carry (n_feasible bits, min V) after W_g; they merge by feas_min / feas_scale instead of the minimum
-// and today's scales, then the update is today's; thread 0 writes cstate = (sum n_feasible, min V) (nullable).
+// FEAS (constraint_mode): the rows carry (n_feasible bits, min V) after W_g and merge feasibility-first, then the update is today's;
+// thread 0 writes cstate = (sum n_feasible, min V) (nullable).
 template <Rule R>
 __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, const float* __restrict__ partials, int G, int P, float* __restrict__ U,
                                               float* __restrict__ action_out, float* __restrict__ stats, float* __restrict__ action_mirror, float* un,
@@ -230,28 +278,8 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
     float* sn = cc + npairs;
     float* Lm = sn + nu * nu;
     float* Mi = Lm + nu * nu;
-    float b = INFINITY;
-    if constexpr (FEAS) {
-        auto nf_of = [&](int gidx) { return __float_as_int(__ldcg(&partials[(size_t)gidx * P + 2 + NR])); };
-        int n_all = 0;
-        float vmin = INFINITY;
-        for (int gidx = 0; gidx < G; ++gidx) { n_all += nf_of(gidx); vmin = fminf(vmin, __ldcg(&partials[(size_t)gidx * P + 3 + NR])); }
-        for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = feas_min(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b);
-        for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
-            const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
-            sg[gidx] = eg > 0.f ? feas_scale(nf_of(gidx), __ldcg(&partials[(size_t)gidx * P]), n_all, b, inv_lambda, 1.0f / p.constraint_lambda) : 0.f;
-        }
-        if (threadIdx.x == 0 && cstate) { cstate[0] = __int_as_float(n_all); cstate[1] = vmin; }
-    } else {
-        for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
-        for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
-            const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
-            sg[gidx] = eg > 0.f ? expf(-(__ldcg(&partials[(size_t)gidx * P]) - b) * inv_lambda) : 0.f;
-        }
-    }
-    __syncthreads();
-    float e = 0.f;
-    for (int gidx = 0; gidx < G; ++gidx) e += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 1]);
+    float b;
+    const float e = merge_rows<FEAS>(p, NR, partials, G, P, inv_lambda, sg, b, cstate);
     for (int r = threadIdx.x; r < NR; r += blockDim.x) {
         float w = 0.f;
         for (int gidx = 0; gidx < G; ++gidx) w += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + r]);
@@ -280,23 +308,8 @@ __device__ __forceinline__ void finalize_rows(const MppibParams& p, int nu, cons
     for (int r = threadIdx.x; r < NR; r += blockDim.x) {
         float out = un[r];
         if (p.filter_u) {
-            const int t = r / nu, j = r % nu;
-            float s = 0.f;
-            if (t < 4) {
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_edge[t][i] * un[i * nu + j];
-                s *= (1.0f / 1155.0f);
-            } else if (t >= T - 4) {
-                const int ee = T - 1 - t;
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_edge[ee][i] * un[(T - 1 - i) * nu + j];
-                s *= (1.0f / 1155.0f);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_mid[i] * un[(t - 4 + i) * nu + j];
-                s *= (1.0f / 231.0f);
-            }
-            out = fminf(fmaxf(s, p.u_min[j]), p.u_max[j]);   // smoothing may overshoot the bounds at the edges
+            const int j = r % nu;
+            out = fminf(fmaxf(savgol(un, T, nu, r), p.u_min[j]), p.u_max[j]);   // smoothing may overshoot the bounds at the edges
         }
         U[r] = out;
         if (r < nu) { action_out[r] = out; if (action_mirror) action_mirror[r] = out; }
@@ -390,7 +403,7 @@ __device__ __forceinline__ void spline_exec(const MppibParams& p, int nu, const 
     for (int r = threadIdx.x; r < T * nu; r += blockDim.x) ue[r] = spline_apply(spline + (r / nu) * S, un + r % nu, nu);
 }
 
-// K4 of mode smooth (smooth = (a_prev[nu], A[T][nu])): combine G rows (beta_g, eta_g, W_g) of stride P as finalize_rows does, the SIMPLE
+// K4 of mode smooth (smooth = (a_prev[nu], A[T][nu])): combine G rows (beta_g, eta_g, W_g) of stride P (merge_rows), the SIMPLE
 // update of the derivative U' = U + W/eta (U' = U when eta = 0), clamped to du_min / du_max; then one thread per j integrates it in t
 // order from a = a_prev: A_t = clamp(fmaf(U'_t, dt, a), u_min, u_max), U'_t := (A_t - a)/dt where that clamp bound, a = A_t.  U <- U',
 // A stored, the action, its mirror and a_prev <- A_0; stats = (beta, eta).  Thread j alone reads and writes column j of the state, and
@@ -400,16 +413,8 @@ __device__ __forceinline__ void smooth_rows(const MppibParams& p, int nu, const 
                                             float* __restrict__ smooth) {
     const int T = p.T, NR = T * nu;
     float* sg = un + NR;
-    const float inv_lambda = 1.0f / p.lambda_;
-    float b = INFINITY;
-    for (int gidx = 0; gidx < G; ++gidx) if (__ldcg(&partials[(size_t)gidx * P + 1]) > 0.f) b = fminf(b, __ldcg(&partials[(size_t)gidx * P]));
-    for (int gidx = threadIdx.x; gidx < G; gidx += blockDim.x) {
-        const float eg = __ldcg(&partials[(size_t)gidx * P + 1]);
-        sg[gidx] = eg > 0.f ? expf(-(__ldcg(&partials[(size_t)gidx * P]) - b) * inv_lambda) : 0.f;
-    }
-    __syncthreads();
-    float e = 0.f;
-    for (int gidx = 0; gidx < G; ++gidx) e += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 1]);
+    float b;
+    const float e = merge_rows<false>(p, NR, partials, G, P, 1.0f / p.lambda_, sg, b, nullptr);
     for (int r = threadIdx.x; r < NR; r += blockDim.x) {
         float w = 0.f;
         for (int gidx = 0; gidx < G; ++gidx) w += sg[gidx] * __ldcg(&partials[(size_t)gidx * P + 2 + r]);
@@ -469,7 +474,7 @@ __device__ __noinline__ void modes_rows(const MppibParams& p, int nu, const floa
         float b = INFINITY;
         for (int g = 0; g < G; ++g) {
             const float* row = partials + (size_t)g * P + (size_t)m * P1;
-            if (__ldcg(row + 1) > 0.f) b = fminf(b, __ldcg(row));
+            if (__ldcg(row + 1) > 0.f) b = merge_min(0, __ldcg(row), 0, b);
         }
         bm[m] = b;
     }
@@ -478,7 +483,7 @@ __device__ __noinline__ void modes_rows(const MppibParams& p, int nu, const floa
         const int m = q / G, g = q % G;
         const float* row = partials + (size_t)g * P + (size_t)m * P1;
         const float eg = __ldcg(row + 1);
-        sg[q] = eg > 0.f ? expf(-(__ldcg(row) - bm[m]) * inv_lambda) : 0.f;
+        sg[q] = eg > 0.f ? merge_scale(0, __ldcg(row), 0, bm[m], inv_lambda, inv_lambda) : 0.f;
     }
     __syncthreads();
     for (int m = tid; m < M; m += nt) {
@@ -560,27 +565,10 @@ __device__ __noinline__ void modes_rows(const MppibParams& p, int nu, const floa
     }
     __syncthreads();
     for (int q = tid; q < MN; q += nt) {                                      // Savitzky-Golay (filter_u) and the clamp, every mode
-        const int m = q / NR, r = q % NR, t = r / nu, j = r % nu;
+        const int m = q / NR, r = q % NR, j = r % nu;
         const float* u = un + (size_t)m * NR;
         float out = u[r];
-        if (p.filter_u) {
-            float s = 0.f;
-            if (t < 4) {
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_edge[t][i] * u[i * nu + j];
-                s *= (1.0f / 1155.0f);
-            } else if (t >= T - 4) {
-                const int ee = T - 1 - t;
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_edge[ee][i] * u[(T - 1 - i) * nu + j];
-                s *= (1.0f / 1155.0f);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 9; ++i) s += c_sg_mid[i] * u[(t - 4 + i) * nu + j];
-                s *= (1.0f / 231.0f);
-            }
-            out = s;
-        }
+        if (p.filter_u) out = savgol(u, T, nu, r);
         out = fminf(fmaxf(out, p.u_min[j]), p.u_max[j]);
         dd[q] = out;
         U[q] = out;
@@ -619,13 +607,13 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
     __syncthreads();
     for (int m = tid; m < M; m += NT) {
         float b = INFINITY;
-        for (int g = 0; g < gx; ++g) b = fminf(b, sc[m * gx + g]);
+        for (int g = 0; g < gx; ++g) b = merge_min(0, sc[m * gx + g], 0, b);
         bb[m] = b;
     }
     __syncthreads();
     for (int q = tid; q < nrow; q += NT) {
         const float b = sc[q];
-        sc[q] = b == INFINITY ? 0.f : expf(-(b - bb[q / gx]) * inv_lambda);
+        sc[q] = b == INFINITY ? 0.f : merge_scale(0, b, 0, bb[q / gx], inv_lambda, inv_lambda);
     }
     __syncthreads();
     const PeerRow row = peer_row(peers);
@@ -651,8 +639,8 @@ __device__ __forceinline__ void fold_modes_and_finish(const MppibParams& p, int 
 
 // The last CTA of a K3 launch: fold the per-CTA partials (128-bit L2 loads, 8 in flight per thread), write the shard row, push it into
 // every rank's peer window (multi-GPU) and, for single-GPU plans, do K4's work in place.  `tiles` = the idle ring, WsLayout::fold_floats
-// at least, `misc` = 8 floats.  FEASIBLE: the CTA scales come from feas_min / feas_scale over (n_feasible, beta) of every CTA, and the
-// row's last two entries are the summed count and the minimum of min V.
+// at least, `misc` = 8 floats.  The CTA scales come from merge_min / merge_scale over (beta, and with FEASIBLE n_feasible) of every CTA,
+// two CTAs per thread; FEASIBLE's row ends with the summed count and the minimum of min V.
 template <Rule R>
 __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, int P, float* __restrict__ scratch, unsigned int* __restrict__ ticket,
                                                 float* __restrict__ partial, const PeerArgs& peers, float* __restrict__ fin_U, float* __restrict__ fin_action,
@@ -668,12 +656,12 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
         float b = (tid < G) ? __ldcg(scratch + (size_t)tid * ((((P + 3) >> 2) << 2))) : INFINITY;
         const float b2 = (tid + NT < G) ? __ldcg(scratch + (size_t)(tid + NT) * ((((P + 3) >> 2) << 2))) : INFINITY;   // CTAs 256..511
         float bb = INFINITY;
-        int n_all = 0;
+        int n1 = 0, n2 = 0, n_all = 0;
         float vmin = INFINITY;
         if constexpr (FEAS) {
             const size_t PP = ((P + 3) >> 2) << 2;
-            const int n1 = tid < G ? __float_as_int(__ldcg(scratch + (size_t)tid * PP + P - 2)) : 0;
-            const int n2 = tid + NT < G ? __float_as_int(__ldcg(scratch + (size_t)(tid + NT) * PP + P - 2)) : 0;
+            n1 = tid < G ? __float_as_int(__ldcg(scratch + (size_t)tid * PP + P - 2)) : 0;
+            n2 = tid + NT < G ? __float_as_int(__ldcg(scratch + (size_t)(tid + NT) * PP + P - 2)) : 0;
             const float v1 = tid < G ? __ldcg(scratch + (size_t)tid * PP + P - 1) : INFINITY;
             const float v2 = tid + NT < G ? __ldcg(scratch + (size_t)(tid + NT) * PP + P - 1) : INFINITY;
             int ns = n1 + n2;
@@ -685,23 +673,15 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
 #pragma unroll
             for (int w8 = 0; w8 < 8; ++w8) { n_all += __float_as_int(misc[w8]); vmin = fminf(vmin, tiles[w8]); }
             __syncthreads();
-            const float bm = warp_min(feas_min(n2, b2, n_all, feas_min(n1, b, n_all, INFINITY)));
-            if (lane == 0) misc[warp] = bm;
-            __syncthreads();
-#pragma unroll
-            for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
-            const float inv_lc = 1.0f / p.constraint_lambda;
-            if (tid < G) sc[tid] = feas_scale(n1, b, n_all, bb, inv_lambda, inv_lc);
-            if (tid + NT < G) sc[tid + NT] = feas_scale(n2, b2, n_all, bb, inv_lambda, inv_lc);
-        } else {
-            float bm = warp_min(fminf(b, b2));
-            if (lane == 0) misc[warp] = bm;
-            __syncthreads();
-#pragma unroll
-            for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
-            if (tid < G) sc[tid] = (b == INFINITY) ? 0.f : expf(-(b - bb) * inv_lambda);
-            if (tid + NT < G) sc[tid + NT] = (b2 == INFINITY) ? 0.f : expf(-(b2 - bb) * inv_lambda);
         }
+        const float bm = warp_min(merge_min(n2, b2, n_all, merge_min(n1, b, n_all)));
+        if (lane == 0) misc[warp] = bm;
+        __syncthreads();
+#pragma unroll
+        for (int w8 = 0; w8 < 8; ++w8) bb = fminf(bb, misc[w8]);
+        const float inv_lc = FEAS ? 1.0f / p.constraint_lambda : inv_lambda;
+        if (tid < G) sc[tid] = (b == INFINITY) ? 0.f : merge_scale(n1, b, n_all, bb, inv_lambda, inv_lc);
+        if (tid + NT < G) sc[tid + NT] = (b2 == INFINITY) ? 0.f : merge_scale(n2, b2, n_all, bb, inv_lambda, inv_lc);
         __syncthreads();
         // parallel fold with deep memory-level parallelism: P4 = ceil(P/4) float4 columns x 4 CTA groups of 64 threads;
         // thread (cg, e4) sums CTAs c = cg, cg+4, ... with 8 independent 128-bit L2 loads in flight
@@ -768,8 +748,9 @@ __device__ __forceinline__ void fold_and_finish(const MppibParams& p, int nu, in
 //   per tile and warp: phase A lane = sample (S_k = sum_t gamma^t c[t][k] + sum_r g[r] x[r][k], conflict-free column reads),
 //                      phase B warp shuffles (min, exp, sum), weights to a 32-float per-warp strip,
 //                      phase C lane = row (r = lane, lane + 32, ...: W[r] += sum_k w_k x[r][k], rotated LDS.128, conflict-free)
-// After the loop the seven warp partials are merged once through shared memory; the per-CTA partial, the ticket and the
-// last-CTA fold / exchange / fused K4 follow (fold_and_finish).
+// After the loop the seven warp partials are merged once through shared memory; the per-CTA partial, the ticket (last_cta) and
+// the last-CTA fold / exchange / fused K4 follow (fold_and_finish).  Every one of these merges, the per-tile one included, is
+// merge_min / merge_scale (common.cuh), with the counts 0 but under FEAS.
 constexpr int WS_W = 32;          // samples per tile
 constexpr int WS_NCONS = 7;       // consumer warps (warp 0 is the producer)
 
@@ -830,7 +811,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // iteration's row after the lambda product (a schedule of ones changes no bit), and the fused K4 advances the counter.
 // FEAS (constraint_mode): a third tensor map brings the T violation rows g of the tile (the tile is (NR + 2T)*32 floats); phase A sums
 // V_k = sum_t c[t][k] in t order beside S, phase B weights the tile's feasible lanes by S with lambda when the warp ballot finds one and
-// its valid lanes by V with lambda_c otherwise, and every fold merges (n_feasible, b, eta, W) by feas_min / feas_scale; the row is
+// its valid lanes by V with lambda_c otherwise, and every fold merges (n_feasible, b, eta, W) feasibility-first; the row is
 // (beta, eta, W, n_feasible bits, min V) and the fused K4 writes cstate.
 template <int RPL, Rule R, bool RISK>
 __global__ void __launch_bounds__(NT, 1)
@@ -848,6 +829,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
     if constexpr (MODES) U += (size_t)blockIdx.y * NR;                       // this CTA's mode
     const float lam = ADAPT ? dist[0] : p.lambda_;
     const float inv_lambda = 1.0f / lam;
+    const float inv_lc = FEAS ? 1.0f / p.constraint_lambda : inv_lambda;     // the merge's violation-kind temperature
     const bool simple = SMOOTH || p.mode == MPPIB_MODE_SIMPLE;
     const bool m2 = R == RULE_DIST && p.update_cov;
     const int npairs = FULL ? nu * (nu + 1) / 2 : 0;
@@ -1004,7 +986,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
                 const unsigned fb = __ballot_sync(0xffffffffu, ok && V <= p.constraint_tol);
                 nf_c = __popc(fb);
                 S = fb ? (((fb >> lane) & 1u) ? sum : INFINITY) : (ok ? V : INFINITY);
-                if (!fb) inv_l = 1.0f / p.constraint_lambda;
+                if (!fb) inv_l = inv_lc;
                 v_run = fminf(v_run, warp_min(ok ? V : INFINITY));
             }
             if constexpr (RISK) S = risk_score(S, p.n_worlds, p.risk_tail, lane);
@@ -1016,18 +998,11 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             if (b_c != INFINITY && (!FEAS || nf_c > 0 || nf_run == 0)) {
                 wme[lane] = w;
                 __syncwarp();
-                float b_out, s_old, s_new;
-                if constexpr (FEAS) {
-                    const int n_out = nf_run + nf_c;
-                    b_out = feas_min(nf_c, b_c, n_out, feas_min(nf_run, b_run, n_out, INFINITY));
-                    s_old = feas_scale(nf_run, b_run, n_out, b_out, inv_lambda, 1.0f / p.constraint_lambda);
-                    s_new = feas_scale(nf_c, b_c, n_out, b_out, inv_lambda, 1.0f / p.constraint_lambda);
-                    nf_run = n_out;
-                } else {
-                    b_out = fminf(b_run, b_c);
-                    s_old = (b_run == INFINITY) ? 0.f : expf(-(b_run - b_out) * inv_lambda);
-                    s_new = expf(-(b_c - b_out) * inv_lambda);
-                }
+                const int n_out = nf_run + nf_c;
+                const float b_out = merge_min(nf_c, b_c, n_out, merge_min(nf_run, b_run, n_out));
+                const float s_old = (b_run == INFINITY) ? 0.f : merge_scale(nf_run, b_run, n_out, b_out, inv_lambda, inv_lc);
+                const float s_new = merge_scale(nf_c, b_c, n_out, b_out, inv_lambda, inv_lc);
+                nf_run = n_out;
                 // ---- C: weighted row sums, lane = row
                 const float4* w4 = reinterpret_cast<const float4*>(wme);
 #pragma unroll
@@ -1111,23 +1086,17 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
         float sc[WS_NCONS];
         int n_all = 0;
         float vmin = INFINITY;
+        auto nf_of = [=](int c) { return FEAS && c < ncons ? __float_as_int(cpart[(size_t)c * P4 + 2 + NR]) : 0; };
         if constexpr (FEAS) {
-            auto nf_of = [&](int c) { return c < ncons ? __float_as_int(cpart[(size_t)c * P4 + 2 + NR]) : 0; };
 #pragma unroll
             for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) { n_all += nf_of(c); vmin = fminf(vmin, cpart[(size_t)c * P4 + 3 + NR]); }
+        }
 #pragma unroll
-            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = feas_min(nf_of(c), cpart[(size_t)c * P4], n_all, bb);
+        for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = merge_min(nf_of(c), cpart[(size_t)c * P4], n_all, bb);
 #pragma unroll
-            for (int c = 0; c < WS_NCONS; ++c)
-                sc[c] = feas_scale(nf_of(c), c < ncons ? cpart[(size_t)c * P4] : INFINITY, n_all, bb, inv_lambda, 1.0f / p.constraint_lambda);
-        } else {
-#pragma unroll
-            for (int c = 0; c < WS_NCONS; ++c) if (c < ncons) bb = fminf(bb, cpart[(size_t)c * P4]);
-#pragma unroll
-            for (int c = 0; c < WS_NCONS; ++c) {
-                const float bc = c < ncons ? cpart[(size_t)c * P4] : INFINITY;
-                sc[c] = (bc == INFINITY) ? 0.f : expf(-(bc - bb) * inv_lambda);
-            }
+        for (int c = 0; c < WS_NCONS; ++c) {
+            const float bc = c < ncons ? cpart[(size_t)c * P4] : INFINITY;
+            sc[c] = (bc == INFINITY) ? 0.f : merge_scale(nf_of(c), bc, n_all, bb, inv_lambda, inv_lc);
         }
         for (int e = tid; e < P; e += NT) {
             float v = 0.f;
@@ -1137,13 +1106,7 @@ mppib_reduce_ws_kernel(const __grid_constant__ MppibParams p, const __grid_const
             mine[e] = e == 0 ? bb : v;
         }
     }
-    __threadfence();
-    __syncthreads();
-    __shared__ unsigned int s_last_ws;
-    if (tid == 0) s_last_ws = atomicAdd(ticket, 1u) == (MODES ? gridDim.x * gridDim.y : gridDim.x) - 1 ? 1u : 0u;
-    __syncthreads();
-    if (!s_last_ws) return;
-    __threadfence();
+    if (!last_cta(ticket, MODES ? gridDim.x * gridDim.y : gridDim.x)) return;
     // the horizon K3 folds as DIST's does; it gets no fin_U and no peers, the SYRK finishes its row
     if constexpr (MODES) fold_modes_and_finish(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, inv_lambda, dist);
     else fold_and_finish<HZN ? RULE_DIST : R>(p, nu, P, scratch, ticket, partial, peers, fin_U, fin_action, fin_stats, fin_mirror, tiles, misc, inv_lambda,
@@ -1261,13 +1224,7 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
 #pragma unroll
     for (int a = 0; a < 4; ++a)
         reinterpret_cast<float4*>(mine + (ty * 4 + a) * HZ_TILE)[tx] = make_float4(acc[a][0], acc[a][1], acc[a][2], acc[a][3]);
-    __threadfence();
-    __syncthreads();
-    __shared__ unsigned int s_last;
-    if (tid == 0) s_last = atomicAdd(&ticket[tile], 1u) == (unsigned)ksplit - 1u ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
+    if (!last_cta(&ticket[tile], (unsigned)ksplit)) return;
     // the tile's last CTA: fold the splits in order, write the packed lower-triangle entries of the tile
     const float* base = scr + (size_t)tile * ksplit * (HZ_TILE * HZ_TILE);
     for (int q = tid; q < HZ_TILE * HZ_TILE; q += blockDim.x) {
@@ -1278,12 +1235,7 @@ mppib_syrk_kernel(const __grid_constant__ MppibParams p, int nu, int ksplit, int
         partial[2 + n + tri(gi) + gj] = c;
     }
     if (tid == 0) ticket[tile] = 0u;
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = atomicAdd(&ticket[HZ_MAX_TILES], 1u) == (unsigned)ntiles - 1u ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
+    if (!last_cta(&ticket[HZ_MAX_TILES], (unsigned)ntiles)) return;
     if (tid == 0) ticket[HZ_MAX_TILES] = 0u;
     if (peers.world > 1) {
         // the complete row goes into the window of every rank, then one release-store of the arrival flag per peer (as in

@@ -113,7 +113,6 @@ __global__ void __launch_bounds__(TNT, 2) mppib_temperature_kernel(const __grid_
     __shared__ float pC[RG][TS], pq[RG][TS];     // the row groups' partial sums
     __shared__ float sC[TS], sq[TS];             // the tile's C_k (+inf: invalid) and q_k
     __shared__ float wst[TWARPS][3 * JG];        // the warp states after the loop
-    __shared__ int s_last;
     const int K = p.K, T = p.T, NR = T * nu;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int rg = warp >> 1, half = warp & 1, s_own = half * 32 + lane;   // this thread's row group and sample of the tile
@@ -193,12 +192,7 @@ __global__ void __launch_bounds__(TNT, 2) mppib_temperature_kernel(const __grid_
         mine[1 + 3 * tid] = mm; mine[2 + 3 * tid] = a1; mine[3 + 3 * tid] = a2;
     }
     if (tid == 0) mine[0] = __int_as_float(n_valid);
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1 ? 1 : 0;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
+    if (!last_cta(ticket, gridDim.x)) return;
     // the last CTA: fold the CTA rows in CTA order into the shard row, publish it with peers open
     const int G = (int)gridDim.x;
     const PeerRow prow = peer_row(peers);
