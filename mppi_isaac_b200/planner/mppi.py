@@ -633,6 +633,14 @@ class MPPIPlanner:
         self._graph = None
         self._graph_failed = False
 
+    def persistent_state(self):
+        """{name: device buffer} of the state one plan leaves for the next -- everything the shift or K4 writes and the next plan reads:
+        U, the Philox plan counter, the distribution (adaptive, CEM, ESS), the smooth state and the mode state.  The capture restores it
+        after its warm-up plans and a keep_U rebuild carries it into the new planner."""
+        named = (("U", self.U), ("plan_ctr", self.plan_ctr), ("dist", self.dist), ("smooth_state", self.smooth_state),
+                 ("mode_state", self.mode_state))
+        return {name: t for name, t in named if t is not None}
+
     # ------------------------------------------------------------------------------------------
     def _cost_batched(self):
         c = self._running_cost(None)
@@ -740,36 +748,31 @@ class MPPIPlanner:
 
     def _try_capture(self):
         dev = torch.device(self.device)
+        main = torch.cuda.current_stream(dev)
+        # the warm-up plans move the state a plan carries; it is put back whether the capture succeeds or not, so the first plan that
+        # follows -- replayed or, after a failed capture, eager -- is the plan an eager planner would run
+        keep = {name: t.clone() for name, t in self.persistent_state().items()}
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(main)                           # after the snapshot: the warm-ups must not overwrite what is being copied
         try:
-            side = torch.cuda.Stream(device=dev)
-            side.wait_stream(torch.cuda.current_stream(dev))
-            u_keep, ctr_keep = self.U.clone(), self.plan_ctr.clone()
-            dist_keep = None if self.dist is None else self.dist.clone()      # the warm-up plans adapt the distribution too
-            smooth_keep = None if self.smooth_state is None else self.smooth_state.clone()   # ... and move the smooth state
-            modes_keep = None if self.mode_state is None else self.mode_state.clone()       # ... and the mode state
             with torch.cuda.stream(side):
                 for _ in range(2):                       # warm-up outside capture (allocator, lazy init)
                     self._plan_batched()
-            torch.cuda.current_stream(dev).wait_stream(side)
+            main.wait_stream(side)
             torch.cuda.synchronize(dev)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._plan_batched()
-            self.U.copy_(u_keep)
-            self.plan_ctr.copy_(ctr_keep)
-            if dist_keep is not None:
-                self.dist.copy_(dist_keep)
-            if smooth_keep is not None:
-                self.smooth_state.copy_(smooth_keep)
-            if modes_keep is not None:
-                self.mode_state.copy_(modes_keep)
             self._graph = g
             self._graph_epoch = getattr(self.sim, "model_epoch", 0)
         except Exception as e:  # capture is an optimisation; the eager path is the same kernels
             self._graph = None
             self._graph_failed = True
             print(f"[mppi_isaac_b200] CUDA-graph capture failed ({type(e).__name__}: {e}); running the plan eagerly")
+            main.wait_stream(side)
             torch.cuda.synchronize(dev)
+        for name, t in self.persistent_state().items():
+            t.copy_(keep[name])
 
     # ------------------------------------------------------------------------------------------
     def command(self, state=None):

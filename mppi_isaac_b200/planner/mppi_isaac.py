@@ -79,13 +79,13 @@ class MPPIisaacPlanner(object):
         self.mppi = self._make_mppi()
         self._sim_build = self.sim.build_epoch         # MPPIPlanner.__init__ re-configures the sim (one more handle)
         if old is not None and old.U.shape == self.mppi.U.shape:
-            self.mppi.U.copy_(old.U)           # the warm start survives a rebuilt simulator, as in the reference (mppi is not rebuilt there)
-            if old.dist is not None and self.mppi.dist is not None and old.dist.shape == self.mppi.dist.shape:
-                self.mppi.dist.copy_(old.dist)         # and so does the adapted (lambda, cov) of adaptive MPPI
-            if old.smooth_state is not None and self.mppi.smooth_state is not None and old.smooth_state.shape == self.mppi.smooth_state.shape:
-                self.mppi.smooth_state.copy_(old.smooth_state)   # and the last executed action of mppi_mode smooth
-            if old.mode_state is not None and self.mppi.mode_state is not None and old.mode_state.shape == self.mppi.mode_state.shape:
-                self.mppi.mode_state.copy_(old.mode_state)       # and, with n_modes > 1, the executed mode and its free energies
+            # the warm start survives a rebuilt simulator, as in the reference (mppi is not rebuilt there): U, the plan counter (so the
+            # random stream continues instead of repeating the draws of plans 0, 1, ...), the adapted distribution, the last executed
+            # action of mppi_mode smooth and the mode state of n_modes > 1 -- each where the new planner has it in the same shape
+            new = self.mppi.persistent_state()
+            for name, t in old.persistent_state().items():
+                if name in new and new[name].shape == t.shape:
+                    new[name].copy_(t)
             # the annealing schedule is rebuilt from the config, not carried over: a keep_U rebuild starts from the configured decays
             self.mppi.refresh_mean_action()              # spline MPPI: U_exec of the carried knots
 
