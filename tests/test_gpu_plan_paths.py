@@ -19,7 +19,8 @@ import pytest
 import torch
 
 import plan_paths as pp
-from mppi_isaac_b200.model.blob import CEM, ESS, FEATURES
+from mppi_isaac_b200.model.blob import FEATURES
+from plan_reference import plan_gate, reference_backend
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -227,32 +228,6 @@ PRIOR_COMMAND = (0.25, -0.125, 0.5)
 class ConstPrior:
     def compute_command(self, sim):
         return torch.tensor(PRIOR_COMMAND)
-
-
-def reference_backend(case):
-    if CEM in case.features:
-        import cem_oracle as ce
-        return ce.CemOracleBackend(nthreads=8)
-    if pp.HORIZON in case.features:
-        import adaptive_horizon_oracle as aho
-        return aho.AdaptiveHorizonOracleBackend(nthreads=8)
-    if ESS in case.features:
-        import colored_oracle as co
-        import temperature_oracle as tmo
-
-        class TemperatureColoredOracleBackend(tmo.TemperatureMixin, co.ColoredOracleBackend):
-            """The temperature rule over the colored checker backend: ESS with colored or Halton noise, diag or full update_cov."""
-        return TemperatureColoredOracleBackend(nthreads=8)
-    import constraint_oracle as cn
-    return cn.ConstraintOracleBackend(nthreads=8)
-
-
-def plan_gate(case, u_lim):
-    """The whole-plan gate of the mode's own test: test_gpu_adaptive_horizon's and, off the panda, test_gpu_adaptive_full's 5e-4; the
-    plan-parity gate 2e-4 max(1, u_lim) of every other mode (DESIGN.md section 2)."""
-    if pp.HORIZON in case.features or case.cov == "full":
-        return 5e-4
-    return 2e-4 * max(1.0, u_lim)
 
 
 @pytest.mark.parametrize("case", PRIOR_CASES, ids=[c.id for c in PRIOR_CASES])
