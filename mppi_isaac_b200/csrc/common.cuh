@@ -183,6 +183,26 @@ static inline int partial_row_capacity(const MppibParams& p, int nu) {
 // and its null / prior rows by c, K2 keys the per-rollout randomisation by r.  R <= 1 (and a zero-initialised block) keeps kg for both.
 __device__ __forceinline__ uint32_t sample_control(uint32_t kg, int R) { return R > 1 ? kg >> (__ffs(R) - 1) : kg; }
 __device__ __forceinline__ uint32_t sample_world(uint32_t kg, int R) { return R > 1 ? kg & (uint32_t)(R - 1) : kg; }
+// Counter-based Philox-4x32-10, its uniform in (0, 1) and the Box-Muller pair: K1's control noise and K2's per-rollout randomisation.
+// UNROLL is the unroll of the ten rounds: K1 unrolls them all (10), K2 draws once per rollout and keeps them rolled (1).
+template <int UNROLL>
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
+#pragma unroll UNROLL
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x, hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
+        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+        k0 += W0; k1 += W1;
+    }
+    return c;
+}
+__device__ __forceinline__ float u01(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
+    const float r = sqrtf(-2.0f * logf(u01(a)));
+    float s, c;
+    sincospif(2.0f * u01(b), &s, &c);
+    z0 = r * c; z1 = r * s;
+}
 // Multi-modal MPPI (n_modes = M > 1): global sample kg is drawn around mode kg / Kc of U[M][T][nu], Kc = mode_samples.  M <= 1 (and a
 // zero-initialised block) keeps mode 0 for every sample.
 __device__ __forceinline__ int sample_mode(uint32_t kg, const MppibParams& p) { return p.n_modes > 1 ? (int)(kg / (uint32_t)p.mode_samples) : 0; }

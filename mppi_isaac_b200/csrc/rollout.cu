@@ -197,6 +197,9 @@ __device__ __forceinline__ void s1_dynamics(const MppibModel& m, float* sm, int 
     st6(sm, i * NSLOT + F_PB, lane, pb);
 }
 
+// the name contact_model.cuh writes a scaled vector with
+__device__ __forceinline__ V3 scale(float s, V3 a) { return s * a; }
+
 #include "contact.cuh"
 
 template <bool CHAIN, bool CONTACT>

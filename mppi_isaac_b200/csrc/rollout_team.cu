@@ -3,7 +3,9 @@
 // not cover: panda + gripper, omnipanda, the planar differential-drive bases (boxer, albert, jackal), and BASELINE C3 / C4 / C5
 // (boxer_push, heijn_push, panda_pick).  Same spec as rollout.cu + contact.cuh (the thread-per-rollout kernel, kept for scenes outside
 // this kernel's limits and as the A/B reference: MPPIB_K2_TEAM=0) and as oracle/oracle.cpp; tested against the same oracle under
-// both mappings (tests/test_gpu_mappings.py).
+// both mappings (tests/test_gpu_mappings.py).  The contact model (randomisation, shape poses, broad phase, box and sphere contacts,
+// tangents, free-body integration) is contact_model.cuh, shared with the thread-per-rollout kernel and compiled here with this
+// kernel's algebra (lanes_math.cuh); the lane mapping, the contact records and the Gauss-Seidel solve are this file's own.
 //
 // Why.  The thread-per-rollout contact kernels are ONE warp per SM walking a data-dependent stream of 23 - 32 k instructions per
 // (sub)step: at the BASELINE shard sizes every CTA is resident at once, so their time is the latency of a single warp, and most of
@@ -28,24 +30,18 @@ using namespace lm;
 
 __device__ __forceinline__ V3 mk(float x, float y, float z) { return mk3(x, y, z); }
 __device__ __forceinline__ float dot6(const V6& a, const V6& b) { return dot(a.n, b.n) + dot(a.f, b.f); }
-__device__ __forceinline__ V3 mulM(const M3& m, V3 v) { return mulc(m, v.x, v.y, v.z); }
-__device__ __forceinline__ V3 mulMT(const M3& m, V3 v) {
+// the names contact_model.cuh writes its arithmetic with
+__device__ __forceinline__ V3 mul(const M3& m, V3 v) { return mulc(m, v.x, v.y, v.z); }
+__device__ __forceinline__ V3 mulT(const M3& m, V3 v) {
     return mk(m.m00 * v.x + m.m10 * v.y + m.m20 * v.z, m.m01 * v.x + m.m11 * v.y + m.m21 * v.z, m.m02 * v.x + m.m12 * v.y + m.m22 * v.z);
 }
-__device__ __forceinline__ M3 mulMM(const M3& a, const M3& b) {
-    M3 o;
-    o.m00 = a.m00 * b.m00 + a.m01 * b.m10 + a.m02 * b.m20; o.m01 = a.m00 * b.m01 + a.m01 * b.m11 + a.m02 * b.m21; o.m02 = a.m00 * b.m02 + a.m01 * b.m12 + a.m02 * b.m22;
-    o.m10 = a.m10 * b.m00 + a.m11 * b.m10 + a.m12 * b.m20; o.m11 = a.m10 * b.m01 + a.m11 * b.m11 + a.m12 * b.m21; o.m12 = a.m10 * b.m02 + a.m11 * b.m12 + a.m12 * b.m22;
-    o.m20 = a.m20 * b.m00 + a.m21 * b.m10 + a.m22 * b.m20; o.m21 = a.m20 * b.m01 + a.m21 * b.m11 + a.m22 * b.m21; o.m22 = a.m20 * b.m02 + a.m21 * b.m12 + a.m22 * b.m22;
-    return o;
-}
 
-// ---- shared-memory layout of ONE rollout (floats; same field order as contact.cuh so the two kernels can be read side by side)
-enum : int { REF_STATIC = -1, REF_FREE0 = 64 };
-enum : int { FB_X = 0, FB_Q = 3, FB_V = 7, FB_W = 10, FB_MASS = 13, FB_HALF = 14, FB_IINV = 17, FB_R = 20, FB_IW = 29, FBN = 35 };   // FB_MASS: inverse mass
-enum : int { SH_R = 0, SH_C = 9, SH_HALF = 12, SH_MU = 15, SH_RAD = 16, SHN = 17 };
-// contact record, 16-byte groups: [ln lt1 lt2 mu] the state of the sweeps | [bias 1/(kn+gamma) 1/kt1 1/kt2] their constants | [p ids] [n -]
-// and, in the roomy layout, [t1 -] (compact: the tangents are recomputed from n, tangent_frame()).
+#include "contact_model.cuh"
+using namespace contact;
+
+// ---- shared-memory layout of ONE rollout (floats): the free-body and shape records of contact_model.cuh, then
+// contact records in 16-byte groups: [ln lt1 lt2 mu] the state of the sweeps | [bias 1/(kn+gamma) 1/kt1 1/kt2] their constants | [p ids]
+// [n -] and, in the roomy layout, [t1 -] (compact: the tangents are recomputed from n, tangents()).
 // Two layouts of the per-rollout block.  ROOMY (robots of up to 8 joints): 20-float contact records, contact rows as one float4 per
 // coordinate -- one LDS.128 per coordinate slot and visit; these kernels run latency-bound with every CTA resident.  COMPACT (9 - 16
 // joints, e.g. panda_pick: 15 coordinates x 24 contacts of rows): 16-float records, rows as three planes of floats -- 20 % less shared
@@ -53,7 +49,6 @@ enum : int { SH_R = 0, SH_C = 9, SH_HALF = 12, SH_MU = 15, SH_RAD = 16, SHN = 17
 // the compact one only where it saves a wave of CTAs (launch_team_contact).
 enum : int { CT_LN = 0, CT_LT1 = 1, CT_LT2 = 2, CT_MU = 3, CT_D = 4, CT_KN = 5, CT_KT1 = 6, CT_KT2 = 7, CT_P = 8, CT_IDS = 11, CT_N = 12, CT_T1 = 16 };
 enum : int { JB_R = 0, JB_O = 9, JB_SN = 12, JB_SF = 15, JB_VP = 18, JB_INVD = 19, JBN = 20 };
-constexpr float K_ROW_MIN = 1e-9f;     // contact rows with a smaller effective inverse mass [1/kg] are dropped (contact.cuh, oracle.cpp)
 constexpr int MAXS_ALL = 5;                 // generalised coordinates per lane in the contact solve: nb + 6 nfree <= G + 24 over G >= 8 lanes
 struct TLayout {
     int fb0, sh0, ct0, net0, rw0, jb0, ncs, ctn, total;
@@ -69,12 +64,6 @@ struct TLayout {
 };
 __host__ __device__ inline int team_stride(int total, int G) { return ((total + 31) & ~31) + G; }   // stride % 32 == G: the teams of a warp start G banks apart
 
-__device__ __forceinline__ void tangent_frame(V3 n, V3& t1, V3& t2) {
-    const V3 e = fabsf(n.x) < 0.9f ? mk(1.f, 0.f, 0.f) : mk(0.f, 1.f, 0.f);
-    t1 = cross(n, e);
-    t1 = scale(rsqrtf(dot(t1, t1)), t1);
-    t2 = cross(n, t1);
-}
 __device__ __forceinline__ V3 ld3(const float* xs, int b) { return mk(xs[b], xs[b + 1], xs[b + 2]); }
 __device__ __forceinline__ void st3(float* xs, int b, V3 v) { xs[b] = v.x; xs[b + 1] = v.y; xs[b + 2] = v.z; }
 __device__ __forceinline__ M3 ldM3(const float* xs, int b) {
@@ -82,55 +71,6 @@ __device__ __forceinline__ M3 ldM3(const float* xs, int b) {
 }
 __device__ __forceinline__ void stM3(float* xs, int b, const M3& m) {
     xs[b] = m.m00; xs[b + 1] = m.m01; xs[b + 2] = m.m02; xs[b + 3] = m.m10; xs[b + 4] = m.m11; xs[b + 5] = m.m12; xs[b + 6] = m.m20; xs[b + 7] = m.m21; xs[b + 8] = m.m22;
-}
-
-// ---- Philox-keyed per-rollout randomisation: the same counters as contact.cuh / oracle actor_noise
-__device__ __forceinline__ uint4 philox(uint4 c, uint32_t k0, uint32_t k1) {
-    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll 1
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x, hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-        k0 += W0; k1 += W1;
-    }
-    return c;
-}
-__device__ __forceinline__ float u01(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
-__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
-    const float r = sqrtf(-2.0f * logf(u01(a)));
-    float s, c; sincospif(2.0f * u01(b), &s, &c);
-    z0 = r * c; z1 = r * s;
-}
-__device__ __forceinline__ void actor_noise(const MppibParams& p, uint32_t kg, int actor, V3& nsize, float& umass, float& ufric) {
-    const uint4 r0 = philox(make_uint4(kg, (uint32_t)actor, 0x5EEDu, 0u), p.rand_seed, 0x4D505049u);
-    const uint4 r1 = philox(make_uint4(kg, (uint32_t)actor, 0x5EEDu, 1u), p.rand_seed, 0x4D505049u);
-    float dummy;
-    box_muller(r0.x, r0.y, nsize.x, nsize.y);
-    box_muller(r0.z, r0.w, nsize.z, dummy);
-    umass = 2.0f * u01(r1.x) - 1.0f;
-    ufric = 2.0f * u01(r1.y) - 1.0f;
-}
-
-__device__ __forceinline__ int shape_ref(const MppibModel& m, int s) {
-    const int kind = m.shape_owner_kind[s];
-    if (kind == MPPIB_OWNER_FREE) return REF_FREE0 + m.shape_owner[s];
-    if (kind == MPPIB_OWNER_LINK && m.shape_owner[s] >= 0) return m.shape_owner[s];
-    return REF_STATIC;
-}
-// candidate partners of shape a (contact.cuh partner_mask)
-__device__ __forceinline__ uint32_t partner_mask(const MppibModel& m, int a) {
-    const int ns = m.nshapes;
-    uint32_t mask = 0;
-    if (m.shape_owner_kind[a] == MPPIB_OWNER_FREE) {
-        for (int b = 0; b < ns; ++b) {
-            if (b == a || shape_ref(m, b) == shape_ref(m, a)) continue;
-            if (m.shape_owner_kind[b] == MPPIB_OWNER_FREE && b < a) continue;
-            mask |= 1u << b;
-        }
-    } else if (m.shape_owner_kind[a] == MPPIB_OWNER_LINK && shape_ref(m, a) != REF_STATIC) {
-        for (int b = 0; b < ns; ++b) if (m.shape_owner_kind[b] == MPPIB_OWNER_STATIC) mask |= 1u << b;
-    }
-    return mask;
 }
 
 // team-wide helpers: G lanes, lane-in-team i, `tb` = first lane of the team in the warp
@@ -353,7 +293,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     }
 
     // =====================================================================================================================
-    // contact pipeline (team-parallel restatement of contact.cuh; the oracle's loop orders are kept)
+    // contact pipeline (team-parallel; the oracle's loop orders are kept)
     // =====================================================================================================================
     const uint32_t kg = sample_world(p.k_offset + (uint32_t)kc, p.n_worlds);   // key of the per-rollout randomisation
     // generalised coordinates of the contact solve held by this lane: coordinate sl * GC + ic = joint (< nb), else component of a free body
@@ -378,48 +318,33 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     auto refresh_free = [&](int fb) {      // all lanes compute, lane 0 writes
         const Quat fq = {xs[fb + FB_Q], xs[fb + FB_Q + 1], xs[fb + FB_Q + 2], xs[fb + FB_Q + 3]};
         const M3 Rf = quat_to_R(fq);
-        const float i0 = xs[fb + FB_IINV], i1 = xs[fb + FB_IINV + 1], i2 = xs[fb + FB_IINV + 2];
+        const V3 iinv = ld3(xs, fb + FB_IINV);
         __syncwarp();
         if (ic == 0) {
             stM3(xs, fb + FB_R, Rf);
-            xs[fb + FB_IW + 0] = Rf.m00 * i0 * Rf.m00 + Rf.m01 * i1 * Rf.m01 + Rf.m02 * i2 * Rf.m02;
-            xs[fb + FB_IW + 1] = Rf.m10 * i0 * Rf.m10 + Rf.m11 * i1 * Rf.m11 + Rf.m12 * i2 * Rf.m12;
-            xs[fb + FB_IW + 2] = Rf.m20 * i0 * Rf.m20 + Rf.m21 * i1 * Rf.m21 + Rf.m22 * i2 * Rf.m22;
-            xs[fb + FB_IW + 3] = Rf.m00 * i0 * Rf.m10 + Rf.m01 * i1 * Rf.m11 + Rf.m02 * i2 * Rf.m12;
-            xs[fb + FB_IW + 4] = Rf.m00 * i0 * Rf.m20 + Rf.m01 * i1 * Rf.m21 + Rf.m02 * i2 * Rf.m22;
-            xs[fb + FB_IW + 5] = Rf.m10 * i0 * Rf.m20 + Rf.m11 * i1 * Rf.m21 + Rf.m12 * i2 * Rf.m22;
+            const S3 Iw = world_inv_inertia(Rf, iinv);
+            xs[fb + FB_IW + 0] = Iw.xx; xs[fb + FB_IW + 1] = Iw.yy; xs[fb + FB_IW + 2] = Iw.zz;
+            xs[fb + FB_IW + 3] = Iw.xy; xs[fb + FB_IW + 4] = Iw.xz; xs[fb + FB_IW + 5] = Iw.yz;
         }
         __syncwarp();
     };
     if (CONTACT) {
         // one-time per rollout: randomised shape / body parameters (lane = shape / free body), initial free-body states
         for (int s = ic; s < m.nshapes; s += GC) {
-            V3 half = mk(m.shape_half[s][0], m.shape_half[s][1], m.shape_half[s][2]);
-            float mu = m.shape_friction[s];
-            if (m.shape_actor[s] >= 0) {
-                V3 ns; float um, uf; actor_noise(p, kg, m.shape_actor[s], ns, um, uf);
-                half.x += 0.5f * m.shape_size_sigma[s][0] * ns.x; half.y += 0.5f * m.shape_size_sigma[s][1] * ns.y; half.z += 0.5f * m.shape_size_sigma[s][2] * ns.z;
-                mu *= 1.0f + m.shape_fric_pct[s] * uf;
-            }
+            V3 half; float mu, rad;
+            shape_params(m, p, kg, s, half, mu, rad);
             const int sb = L.sh0 + s * SHN;
             st3(xs, sb + SH_HALF, half);
             xs[sb + SH_MU] = mu;
-            xs[sb + SH_RAD] = m.shape_type[s] == MPPIB_SHAPE_SPHERE ? half.x : sqrtf(dot(half, half));
+            xs[sb + SH_RAD] = rad;
         }
         for (int f = ic; f < m.nfree; f += GC) {
             const int fb = L.fb0 + f * FBN;
-            V3 ns; float um, uf; actor_noise(p, kg, m.free_actor[f], ns, um, uf);
-            const float mass = m.free_mass[f] * (1.0f + m.free_mass_pct[f] * um);
-            V3 sg = mk(0.f, 0.f, 0.f);
-            for (int s = 0; s < m.nshapes; ++s)
-                if (m.shape_owner_kind[s] == MPPIB_OWNER_FREE && m.shape_owner[s] == f) { sg = mk(m.shape_size_sigma[s][0], m.shape_size_sigma[s][1], m.shape_size_sigma[s][2]); break; }
-            const V3 half = mk(m.free_half[f][0] + 0.5f * sg.x * ns.x, m.free_half[f][1] + 0.5f * sg.y * ns.y, m.free_half[f][2] + 0.5f * sg.z * ns.z);
-            const float m3 = mass / 3.0f;
-            xs[fb + FB_MASS] = 1.0f / mass;
+            float inv_mass; V3 half, iinv;
+            free_params(m, p, kg, f, inv_mass, half, iinv);
+            xs[fb + FB_MASS] = inv_mass;
             st3(xs, fb + FB_HALF, half);
-            xs[fb + FB_IINV] = 1.0f / (m3 * (half.y * half.y + half.z * half.z));
-            xs[fb + FB_IINV + 1] = 1.0f / (m3 * (half.x * half.x + half.z * half.z));
-            xs[fb + FB_IINV + 2] = 1.0f / (m3 * (half.x * half.x + half.y * half.y));
+            st3(xs, fb + FB_IINV, iinv);
             for (int r = 0; r < 13; ++r)
                 xs[fb + r] = state0 ? root0[13 * m.free_actor[f] + r] : state[(size_t)(2 * nb + 13 * f + r) * K + kc];
         }
@@ -436,21 +361,18 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
             const int own = m.shape_owner[s];
             if ((kind == MPPIB_OWNER_STATIC) != statics) continue;
             M3 Ro; V3 po;
-            if (kind == MPPIB_OWNER_STATIC) {
-                const float* rs = root0 + 13 * m.shape_actor[s];
-                const Quat qs = {rs[3], rs[4], rs[5], rs[6]};
-                Ro = quat_to_R(qs); po = mk(rs[0], rs[1], rs[2]);
-            } else if (kind == MPPIB_OWNER_LINK) {
+            if (kind == MPPIB_OWNER_STATIC) root_pose(root0, m.shape_actor[s], Ro, po);
+            else if (kind == MPPIB_OWNER_LINK) {
                 if (own < 0) { Ro = Rbase; po = obase; }
                 else { const int jb = L.jb0 + own * JBN; Ro = ldM3(xs, jb + JB_R); po = ld3(xs, jb + JB_O); }
             } else {
                 const int fb = L.fb0 + own * FBN;
                 Ro = ldM3(xs, fb + FB_R); po = ld3(xs, fb + FB_X);
             }
-            const Quat qlc = {m.shape_quat[s][0], m.shape_quat[s][1], m.shape_quat[s][2], m.shape_quat[s][3]};
+            M3 R; V3 c; shape_pose(m, s, Ro, po, R, c);
             const int sb = L.sh0 + s * SHN;
-            stM3(xs, sb + SH_R, mulMM(Ro, quat_to_R(qlc)));
-            st3(xs, sb + SH_C, po + mulc(Ro, m.shape_pos[s][0], m.shape_pos[s][1], m.shape_pos[s][2]));
+            stM3(xs, sb + SH_R, R);
+            st3(xs, sb + SH_C, c);
         }
         __syncwarp();
     };
@@ -463,7 +385,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
             const int cb = L.ct0 + slot * CTN;
             st3(xs, cb + CT_P, pt); st3(xs, cb + CT_N, n);
             xs[cb + CT_D] = d; xs[cb + CT_MU] = mu; xs[cb + CT_LN] = 0.f; xs[cb + CT_LT1] = 0.f; xs[cb + CT_LT2] = 0.f;
-            xs[cb + CT_IDS] = __int_as_float((refA + 2) | ((refB + 2) << 8) | ((slotA + 1) << 16) | ((slotB + 1) << 24));
+            xs[cb + CT_IDS] = __int_as_float(pack_sides(refA, refB, slotA, slotB));
         }
         nc = min(nc + __popc(bits), (int)m.max_contacts);
     };
@@ -476,98 +398,39 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
         const V3 ha = ld3(xs, sa + SH_HALF), hb = ld3(xs, sb + SH_HALF);
         const float mu = 0.5f * (xs[sa + SH_MU] + xs[sb + SH_MU]);
         const int refa = shape_ref(m, a), refb = shape_ref(m, b), slota = m.shape_slot[a], slotb = m.shape_slot[b];
-        const V3 cl = mulMT(Rb, ca - cbv);
-        bool c0 = fabsf(cl.x) > hb.x, c1 = fabsf(cl.y) > hb.y, c2 = fabsf(cl.z) > hb.z;
-        if (!(c0 || c1 || c2)) c0 = c1 = c2 = true;
-        const float mg = m.contact_margin;
+        bool c0, c1, c2; face_axes(Rb, ca, cbv, hb, c0, c1, c2);
         for (int i0 = 0; i0 < 27; i0 += GC) {
             const int idx = i0 + ic;
-            bool hit = on && idx < 27 && idx != 13;
-            const int ix = idx / 9 - 1, iy = (idx / 3) % 3 - 1, iz = idx % 3 - 1;
-            const V3 pt = mulM(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
-            const V3 x = mulMT(Rb, pt - cbv);
-            const float p0 = hb.x - fabsf(x.x), p1 = hb.y - fabsf(x.y), p2 = hb.z - fabsf(x.z);
-            if (!(p0 + mg > 0.f) || !(p1 + mg > 0.f) || !(p2 + mg > 0.f)) hit = false;
-            int ax = -1; float pen = 0.f;
-            if (c0) { ax = 0; pen = p0; }
-            if (c1 && (ax < 0 || p1 < pen)) { ax = 1; pen = p1; }
-            if (c2 && (ax < 0 || p2 < pen)) { ax = 2; pen = p2; }
-            const float xa = ax == 0 ? x.x : (ax == 1 ? x.y : x.z);
-            const float sg = xa >= 0.f ? 1.f : -1.f;
-            const V3 n = ax == 0 ? mk(sg * Rb.m00, sg * Rb.m10, sg * Rb.m20) : (ax == 1 ? mk(sg * Rb.m01, sg * Rb.m11, sg * Rb.m21) : mk(sg * Rb.m02, sg * Rb.m12, sg * Rb.m22));
+            V3 pt, n; float pen;
+            const bool inside = box_point(idx, Ra, ca, ha, Rb, cbv, hb, c0, c1, c2, m.contact_margin, pt, n, pen);
+            const bool hit = on && idx < 27 && idx != 13 && inside;
             if (!flip) append(hit, refa, refb, slota, slotb, pt, n, pen, mu);
             else append(hit, refb, refa, slotb, slota, pt, mk(-n.x, -n.y, -n.z), pen, mu);
         }
     };
-    // ONE contact of a sphere against a box or a sphere (contact.cuh sphere_contact); all lanes compute, lane 0 appends
-    auto sphere_contact = [&](int a, int b, bool on) {
+    // ONE contact of a sphere against a box or a sphere; all lanes compute, lane 0 appends
+    auto sphere_pair = [&](int a, int b, bool on) {
         const int sa = L.sh0 + a * SHN, sb = L.sh0 + b * SHN;
-        const float mu = 0.5f * (xs[sa + SH_MU] + xs[sb + SH_MU]), mg = m.contact_margin;
+        const float mu = 0.5f * (xs[sa + SH_MU] + xs[sb + SH_MU]);
         const int refa = shape_ref(m, a), refb = shape_ref(m, b), slota = m.shape_slot[a], slotb = m.shape_slot[b];
         const V3 ca = ld3(xs, sa + SH_C), cbv = ld3(xs, sb + SH_C);
-        bool hit = true; V3 pt = mk(0.f, 0.f, 0.f), n = mk(0.f, 0.f, 1.f); float pen = 0.f;
-        if (m.shape_type[a] == MPPIB_SHAPE_SPHERE && m.shape_type[b] == MPPIB_SHAPE_SPHERE) {
-            const V3 d = ca - cbv;
-            const float dist = sqrtf(dot(d, d)), ra = xs[sa + SH_HALF], rb = xs[sb + SH_HALF], rs = ra + rb;
-            if (!(dist < rs + mg) || !(dist > 0.f)) hit = false;
-            n = scale(1.0f / fmaxf(dist, 1e-30f), d);
-            pt = cbv + scale(rb, n); pen = rs - dist;
-        } else {
-            const bool sphere_is_a = m.shape_type[a] == MPPIB_SHAPE_SPHERE;
-            const int ss = sphere_is_a ? sa : sb, sx = sphere_is_a ? sb : sa;
-            const float r = xs[ss + SH_HALF];
-            const V3 cs = sphere_is_a ? ca : cbv, cx = sphere_is_a ? cbv : ca;
-            const M3 Rx = ldM3(xs, sx + SH_R);
-            const V3 hx = ld3(xs, sx + SH_HALF);
-            const V3 x = mulMT(Rx, cs - cx);
-            V3 qq = mk(fminf(fmaxf(x.x, -hx.x), hx.x), fminf(fmaxf(x.y, -hx.y), hx.y), fminf(fmaxf(x.z, -hx.z), hx.z));
-            const V3 dd = x - qq;
-            const float d2 = dot(dd, dd);
-            V3 nl = mk(0.f, 0.f, 0.f);
-            if (d2 > 0.f) {
-                const float dist = sqrtf(d2);
-                if (!(dist < r + mg)) hit = false;
-                nl = scale(1.0f / dist, dd);
-                pen = r - dist;
-            } else {
-                int ax = 0; float best = hx.x - fabsf(x.x);
-                const float p1 = hx.y - fabsf(x.y), p2 = hx.z - fabsf(x.z);
-                if (p1 < best) { best = p1; ax = 1; }
-                if (p2 < best) { best = p2; ax = 2; }
-                const float xa = ax == 0 ? x.x : (ax == 1 ? x.y : x.z);
-                const float sg = xa >= 0.f ? 1.f : -1.f;
-                if (ax == 0) { nl.x = sg; qq.x = sg * hx.x; } else if (ax == 1) { nl.y = sg; qq.y = sg * hx.y; } else { nl.z = sg; qq.z = sg * hx.z; }
-                pen = best + r;
-            }
-            n = mulM(Rx, nl);
-            pt = cx + mulM(Rx, qq);
-            if (!sphere_is_a) n = mk(-n.x, -n.y, -n.z);
+        const bool sph_a = m.shape_type[a] == MPPIB_SHAPE_SPHERE;
+        V3 pt, n; float pen; bool hit;
+        if (sph_a && m.shape_type[b] == MPPIB_SHAPE_SPHERE) hit = sphere_sphere(ca, xs[sa + SH_HALF], cbv, xs[sb + SH_HALF], m.contact_margin, pt, n, pen);
+        else {
+            const int sx = sph_a ? sb : sa;
+            hit = sphere_box(sph_a ? ca : cbv, xs[(sph_a ? sa : sb) + SH_HALF], ldM3(xs, sx + SH_R), sph_a ? cbv : ca, ld3(xs, sx + SH_HALF), m.contact_margin, pt, n, pen);
+            if (!sph_a) n = mk(-n.x, -n.y, -n.z);
         }
         append(on && hit && ic == 0, refa, refb, slota, slotb, pt, n, pen, mu);
     };
     auto near_shapes = [&](int a, int b) -> bool {
         const int sa = L.sh0 + a * SHN, sb = L.sh0 + b * SHN;
         const V3 d = ld3(xs, sa + SH_C) - ld3(xs, sb + SH_C);
-        const float mg = m.contact_margin;
         const bool sph = m.shape_type[a] == MPPIB_SHAPE_SPHERE || m.shape_type[b] == MPPIB_SHAPE_SPHERE;
-        const float r = xs[sa + SH_RAD] + xs[sb + SH_RAD] + (sph ? mg : 0.f);
-        if (dot(d, d) > r * r) return false;
+        if (!near_bounds(d, xs[sa + SH_RAD], xs[sb + SH_RAD], sph, m.contact_margin)) return false;
         if (sph) return true;
-        const M3 Ra = ldM3(xs, sa + SH_R), Rb = ldM3(xs, sb + SH_R);
-        const V3 ha = ld3(xs, sa + SH_HALF), hb = ld3(xs, sb + SH_HALF);
-        const V3 tbv = mulMT(Rb, d), ta = mulMT(Ra, d);
-        const V3 b0 = mk(Rb.m00, Rb.m10, Rb.m20), b1 = mk(Rb.m01, Rb.m11, Rb.m21), b2 = mk(Rb.m02, Rb.m12, Rb.m22);
-        const V3 a0 = mk(Ra.m00, Ra.m10, Ra.m20), a1 = mk(Ra.m01, Ra.m11, Ra.m21), a2 = mk(Ra.m02, Ra.m12, Ra.m22);
-        const float c00 = fabsf(dot(b0, a0)), c01 = fabsf(dot(b0, a1)), c02 = fabsf(dot(b0, a2));
-        const float c10 = fabsf(dot(b1, a0)), c11 = fabsf(dot(b1, a1)), c12 = fabsf(dot(b1, a2));
-        const float c20 = fabsf(dot(b2, a0)), c21 = fabsf(dot(b2, a1)), c22 = fabsf(dot(b2, a2));
-        if (fabsf(tbv.x) > hb.x + c00 * ha.x + c01 * ha.y + c02 * ha.z + mg) return false;
-        if (fabsf(ta.x) > ha.x + c00 * hb.x + c10 * hb.y + c20 * hb.z + mg) return false;
-        if (fabsf(tbv.y) > hb.y + c10 * ha.x + c11 * ha.y + c12 * ha.z + mg) return false;
-        if (fabsf(ta.y) > ha.y + c01 * hb.x + c11 * hb.y + c21 * hb.z + mg) return false;
-        if (fabsf(tbv.z) > hb.z + c20 * ha.x + c21 * ha.y + c22 * ha.z + mg) return false;
-        if (fabsf(ta.z) > ha.z + c02 * hb.x + c12 * hb.y + c22 * hb.z + mg) return false;
-        return true;
+        return near_boxes(d, ldM3(xs, sa + SH_R), ld3(xs, sa + SH_HALF), ldM3(xs, sb + SH_R), ld3(xs, sb + SH_HALF), m.contact_margin);
     };
     // partners of shape a: the broad phase of up to GC partners in parallel (lane = partner), then the near ones in ascending order
     auto pairs_of = [&](int a) {
@@ -584,7 +447,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
                 const int ln = __ffs(ubits) - 1; ubits &= ubits - 1;
                 const int bb = __shfl_sync(FULL, b, ln, GC);  // (the same shape for every team: b depends on the lane only)
                 const bool on = (mybits >> ln) & 1u;
-                if (m.shape_type[a] == MPPIB_SHAPE_SPHERE || m.shape_type[bb] == MPPIB_SHAPE_SPHERE) sphere_contact(a, bb, on);
+                if (m.shape_type[a] == MPPIB_SHAPE_SPHERE || m.shape_type[bb] == MPPIB_SHAPE_SPHERE) sphere_pair(a, bb, on);
                 else { points_in_box(a, bb, false, on); points_in_box(bb, a, true, on); }
             }
             for (int j = 0; j < GC && mask; ++j) mask &= mask - 1;                               // drop the partners just handled
@@ -604,7 +467,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
                 static_assert(GC >= 8, "one corner per lane");
                 const int idx = ic;
                 const int ix = (idx >> 2) * 2 - 1, iy = ((idx >> 1) & 1) * 2 - 1, iz = (idx & 1) * 2 - 1;
-                const V3 pt = mulM(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
+                const V3 pt = mul(Ra, mk(ix * ha.x, iy * ha.y, iz * ha.z)) + ca;
                 bool hit = idx < 8 && pt.z < m.ground_margin;
                 if (__any_sync(FULL, __popc(team_ballot<GC>(hit, tbc)) > 4)) {          // warp-uniform
                     int rank = 0;
@@ -638,7 +501,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
                 for (; ub; ub &= ub - 1) {
                     const int b = __ffs(ub) - 1;
                     const bool on = (ma >> b) & 1u;
-                    if (m.shape_type[aa] == MPPIB_SHAPE_SPHERE || m.shape_type[b] == MPPIB_SHAPE_SPHERE) sphere_contact(aa, b, on);
+                    if (m.shape_type[aa] == MPPIB_SHAPE_SPHERE || m.shape_type[b] == MPPIB_SHAPE_SPHERE) sphere_pair(aa, b, on);
                     else { points_in_box(aa, b, false, on); points_in_box(b, aa, true, on); }
                 }
             }
@@ -688,9 +551,9 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
             const bool act = c < nc;                         // (a team past its own contacts computes on stale records and stores nothing)
             const int cb = L.ct0 + c * CTN;
             const int ids = act ? __float_as_int(xs[cb + CT_IDS]) : 0;
-            const int refA = (ids & 0xFF) - 2, refB = ((ids >> 8) & 0xFF) - 2;
+            const int refA = ref_a(ids), refB = ref_b(ids);
             const V3 pt = ld3(xs, cb + CT_P), n = ld3(xs, cb + CT_N);
-            V3 t1, t2; tangent_frame(n, t1, t2);
+            V3 t1, t2; tangents(n, t1, t2);
             float kn_ = 0.f, kt1 = 0.f, kt2 = 0.f;
 #pragma unroll
             for (int sl = 0; sl < MAXS; ++sl) {
@@ -800,7 +663,7 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
             const V3 wb = ld3(xs, fb + FB_W);
             const M3 Rf = ldM3(xs, fb + FB_R);
             __syncwarp();
-            if (ic == 0) st3(xs, fb + FB_W, mulM(Rf, wb));
+            if (ic == 0) st3(xs, fb + FB_W, mul(Rf, wb));
         }
         __syncwarp();
         if (last_substep) {                                  // net contact force per body = the last substep's impulses / h
@@ -809,11 +672,12 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
                 for (int c = 0; c < nc; ++c) {
                     const int cb = L.ct0 + c * CTN;
                     const int ids = __float_as_int(xs[cb + CT_IDS]);
+                    // (slot_a / slot_b written out: with the calls, the roomy <8, 8, true, 1, 8> instantiation spills 8 bytes more)
                     const int slotA = ((ids >> 16) & 0xFF) - 1, slotB = ((ids >> 24) & 0xFF) - 1;
                     if (slotA < 0 && slotB < 0) continue;
                     const V3 n = ld3(xs, cb + CT_N);
                     V3 t1, t2;
-                    if (COMPACT) tangent_frame(n, t1, t2);
+                    if (COMPACT) tangents(n, t1, t2);
                     else { t1 = ld3(xs, cb + CT_T1); t2 = cross(n, t1); }
                     const V3 F = scale(ih, scale(xs[cb + CT_LN], n) + scale(xs[cb + CT_LT1], t1) + scale(xs[cb + CT_LT2], t2));
                     if (slotA >= 0) { xs[L.net0 + 3 * slotA] += F.x; xs[L.net0 + 3 * slotA + 1] += F.y; xs[L.net0 + 3 * slotA + 2] += F.z; }
@@ -826,16 +690,13 @@ mppib_rollout_team_kernel(const __grid_constant__ MppibModel m, const __grid_con
     auto integrate_free = [&]() {
         for (int f = 0; f < m.nfree; ++f) {
             const int fb = L.fb0 + f * FBN;
-            const V3 x = ld3(xs, fb + FB_X), v = ld3(xs, fb + FB_V), w = ld3(xs, fb + FB_W);
-            const Quat fq = {xs[fb + FB_Q], xs[fb + FB_Q + 1], xs[fb + FB_Q + 2], xs[fb + FB_Q + 3]};
-            const Quat wq = {w.x, w.y, w.z, 0.f};
-            const Quat dqq = qmul(wq, fq);
-            Quat r = {fq.x + 0.5f * h * dqq.x, fq.y + 0.5f * h * dqq.y, fq.z + 0.5f * h * dqq.z, fq.w + 0.5f * h * dqq.w};
-            const float il = rsqrtf(r.x * r.x + r.y * r.y + r.z * r.z + r.w * r.w);
+            V3 x = ld3(xs, fb + FB_X);
+            Quat fq = {xs[fb + FB_Q], xs[fb + FB_Q + 1], xs[fb + FB_Q + 2], xs[fb + FB_Q + 3]};
+            integrate_pose(x, fq, ld3(xs, fb + FB_V), ld3(xs, fb + FB_W), h);
             __syncwarp();
             if (ic == 0) {
-                xs[fb + FB_X] = x.x + h * v.x; xs[fb + FB_X + 1] = x.y + h * v.y; xs[fb + FB_X + 2] = x.z + h * v.z;
-                xs[fb + FB_Q] = r.x * il; xs[fb + FB_Q + 1] = r.y * il; xs[fb + FB_Q + 2] = r.z * il; xs[fb + FB_Q + 3] = r.w * il;
+                st3(xs, fb + FB_X, x);
+                xs[fb + FB_Q] = fq.x; xs[fb + FB_Q + 1] = fq.y; xs[fb + FB_Q + 2] = fq.z; xs[fb + FB_Q + 3] = fq.w;
             }
             __syncwarp();
             refresh_free(fb);

@@ -11,27 +11,6 @@
 
 namespace {
 
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
-        uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-        k0 += W0; k1 += W1;
-    }
-    return c;
-}
-
-__device__ __forceinline__ float u01(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
-
-__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
-    float r = sqrtf(-2.0f * logf(u01(a)));
-    float s, c;
-    sincospif(2.0f * u01(b), &s, &c);
-    z0 = r * c; z1 = r * s;
-}
-
 // The Philox key of a plan: (seed_lo, seed_hi ^ plan_lo), with plan_hi the last counter word; plan = plan_idx + *plan_ctr (nullable),
 // so that a captured graph draws fresh noise on every replay.
 struct PhiloxKey { uint32_t k0, k1, plan_hi; };
@@ -41,7 +20,7 @@ __device__ __forceinline__ PhiloxKey philox_key(uint32_t key0, uint32_t seed_hi,
 }
 // the white draws z[0..4) of controls 4*blk .. 4*blk + 3 of control sample kc at step t
 __device__ __forceinline__ void philox_gauss4(const PhiloxKey& key, uint32_t kc, int t, int blk, float* z) {
-    const uint4 r = philox4x32_10(make_uint4(kc, (uint32_t)t, (uint32_t)blk, key.plan_hi), key.k0, key.k1);
+    const uint4 r = philox4x32_10<10>(make_uint4(kc, (uint32_t)t, (uint32_t)blk, key.plan_hi), key.k0, key.k1);
     box_muller(r.x, r.y, z[0], z[1]);
     box_muller(r.z, r.w, z[2], z[3]);
 }
